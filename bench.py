@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """Benchmark of the Multi-HMR hot path (BASELINE.json: images/sec, multiHMR_896_L, batch 8 per GPU).
 
-  python bench.py --gpus N --steps K --warmup W            this repo: sm_100a engine through the C-ABI
+  python bench.py --gpus N --steps K --warmup W            this repo: sm_90a engine through the C-ABI
+  python bench.py ... --dump-outputs DIR                   also writes what the last timed step computed as
+                                                           DIR/<name>.npy (float32 / float64)
   python bench.py --impl reference --gpus N --steps K ...  reference arm: the reference's algorithm on the
                                                            host CPU cores (oracle port, fp32 PyTorch)
 
@@ -64,15 +66,14 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as fh:
             p = json.load(fh)
-        return dict(tflops=float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 1400.0))),
-                    tflops_burst=float(p.get("bf16_tflops", 1590.0)), hbm_gbs=float(p.get("hbm_gbs", 6650.0)),
-                    source="MEASURED_PEAKS.json (measured)")
-    return dict(tflops=1400.0, tflops_burst=1590.0, hbm_gbs=6650.0, source="B200_PROFILING.md fallback")
+        return dict(tflops=float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 989.0))),
+                    hbm_gbs=float(p.get("hbm_gbs", 3350.0)), source="MEASURED_PEAKS.json (measured)")
+    # NVIDIA H100 SXM data sheet (700 W card), dense fp16 tensor-core rate and HBM3 bandwidth: not measured
+    return dict(tflops=989.0, hbm_gbs=3350.0, source="H100 SXM data sheet, dense fp16")
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons sampled DURING the timed region (B200_PROFILING.md): the
-    sampler runs from before the warm-up, and only samples stamped inside [mark_start, mark_stop] count."""
+    """nvidia-smi clocks + throttle reasons sampled DURING the timed region: the sampler runs from before the warm-up, and only samples stamped inside [mark_start, mark_stop] count."""
 
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -328,6 +329,8 @@ def run_ours(args):
     sampler.start()
     ms_total, P_last, clocks = bench.timed(bench.step_device, args.steps, args.warmup, sampler)
     launches = bench.model.last_launch_count()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(bench.model.last_outputs, int(P_last), args.dump_outputs)
     value = world * B * args.steps / (ms_total / 1e3)
 
     # ---- end to end through the public API with host buffers
@@ -347,7 +350,7 @@ def run_ours(args):
         torch.cuda.empty_cache()
         w2 = CONFIGS["c2"]
         b2 = OursBench(w2, 1, 0, dev)
-        steps2 = max(5, args.steps // 2)
+        steps2 = args.steps
         ms2, P2, _ = b2.timed(b2.step_device, steps2, 3)
         ms2e, _, _ = b2.timed(b2.step_e2e, steps2, 2)
         secondary = {"workload": f"{w2['name']} batch {w2['batch_per_gpu']}, synthetic 672x672", "steps": steps2,
@@ -384,23 +387,14 @@ def run_ours(args):
     vit_tflops_step = vit_flops_per_image(w["backbone"], S) * B * args.steps / (ms_total / 1e3) / 1e12
     roofline = None
     if dom:
-        traffic, traffic_src = None, None  # DRAM bytes per launch of the dominant kernel (ncu --set full capture)
-        tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tpath) and args.config == "c3":
-            with open(tpath) as fh:
-                tj = json.load(fh)
-            traffic = tj.get(dom, {}).get("dram_bytes_per_launch")
-            traffic_src = tj.get("_source")
         roofline = {"bound": "tensor", "kernel": dom, "achieved": round(fam[dom]["tflops"], 1),
                     "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": round(fam[dom]["tflops"] / peaks["tflops"], 4),
-                    "traffic": traffic, "traffic_source": traffic_src,
-                    "peak_source": peaks["source"] + ", sustained cuBLAS bf16",
+                    "peak_source": peaks["source"],
                     "timing": f"CUDA events around every launch, separate pass of {prof_steps} steps "
                               f"({ms_prof / prof_steps:.2f} ms/step with the events in)",
                     "families": {k: {a: round(b, 4) for a, b in v.items()} for k, v in fam.items()},
                     "vit_backbone": {"tflops_whole_step": round(vit_tflops_step, 1),
-                                     "frac_of_peak": round(vit_tflops_step / peaks["tflops"], 4),
-                                     "frac_of_nominal_2250": round(vit_tflops_step / 2250.0, 4)},
+                                     "frac_of_peak": round(vit_tflops_step / peaks["tflops"], 4)},
                     "other_ms_per_step": {k: round(prof[k][0] / prof_steps, 3)
                                           for k in ("misc", "layernorm", "gemm_other", "head", "smplx", "refine")
                                           if k in prof}}
@@ -417,7 +411,7 @@ def run_ours(args):
                    "images_per_gpu": B, "global_batch": world * B, "persons_in_batch": int(P_last),
                    "det_thresh": w["det_thresh"], "nms_kernel_size": w["nms_kernel_size"],
                    "parallelism": f"dp{world} (image shards, 1 all-gather of person records)" if world > 1 else "dp1",
-                   "l2": "working set per step (0.6 GB fp16 weights + >1 GB activations) exceeds the 126 MB L2"},
+                   "l2": "working set per step (0.6 GB fp16 weights + >1 GB activations) exceeds the 50 MB L2"},
         "clocks": clocks, "gpu_launches": int(launches),
         "e2e": {"value": round(e2e_value, 3), "unit": "images/s", "h2d_bytes_per_step": int(h2d_bytes),
                 "d2h_bytes_per_step": int(d2h_bytes), "ms_per_step": round(ms_e2e / args.steps, 3),
@@ -432,6 +426,40 @@ def run_ours(args):
 # ------------------------------------------------------------------------------------------------
 # CPU side: the oracle port timed on the host cores
 # ------------------------------------------------------------------------------------------------
+# person-indexed outputs of Model.forward_raw: rows [0, P) are the persons of the step
+PER_PERSON = ("det_score", "offset", "loc", "dist_pp", "dist", "rotmat", "rotvec", "shape", "expression", "transl",
+              "transl_pelvis", "v3d", "v2d", "j3d", "j2d")
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(t: dict, P: int, out_dir: str):
+    """Writes the arrays a caller of the timed path receives (Model.forward_raw: the detection score map, the
+    detected token indices and every per-person output, rows [0, P)) as out_dir/<name>.npy: floating outputs in
+    float32, integer ones in float64 (exact).  Above DUMP_LIMIT_BYTES in all, every per-person array keeps the same
+    fixed, seeded sample of persons (sample_rows.npy lists them)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"scores_map": t["scores_map"], "det_idx": t["det_idx"][:, :P]}
+    for k in PER_PERSON:
+        if t.get(k) is not None:
+            arrays[k] = t[k][:P]
+    total = sum(v.numel() * 8 for v in arrays.values())
+    if total > DUMP_LIMIT_BYTES and P > 0:
+        per_row = sum(arrays[k][0].numel() * 8 for k in PER_PERSON if k in arrays)
+        keep = max(1, (DUMP_LIMIT_BYTES - arrays["scores_map"].numel() * 8 - arrays["det_idx"].numel() * 8) // per_row)
+        rows = torch.randperm(P, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+        for k in PER_PERSON:
+            if k in arrays:
+                arrays[k] = arrays[k][rows.to(arrays[k].device)]
+        np.save(os.path.join(out_dir, "sample_rows.npy"), rows.numpy().astype(np.float64))
+    for k, v in arrays.items():
+        v = v.detach().cpu()
+        v = v.to(torch.float32) if v.is_floating_point() else v.to(torch.float64)
+        np.save(os.path.join(out_dir, f"{k}.npy"), v.numpy())
+
+
 def usable_cpus() -> dict:
     """Cores this process may actually use: scheduler affinity AND the cgroup CPU quota (a container with a
     quota of 16 CPUs on a 128-thread host runs 8x oversubscribed with torch.set_num_threads(os.cpu_count()))."""
@@ -618,6 +646,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the (slow) CPU oracle leg")
     ap.add_argument("--config", default="c3", choices=sorted(CONFIGS), help="BASELINE.json config (headline: c3)")
     ap.add_argument("--no-secondary", action="store_true", help="skip the short c2 (672x672) leg of the default run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     set_workload(args.config)
     _reserve_stdout()

@@ -1,5 +1,5 @@
 /*
- * libmhmr_sm100.so — C-ABI of the B200-native Multi-HMR inference path.
+ * libmhmr_sm90.so — C-ABI of the H100-native Multi-HMR inference path.
  *
  * Drop-in boundary for the ONE hot path of naver/multi-hmr: `Model.forward(x, K)` as called by
  * `demo.py:forward_model` (reference demo.py:108-126, model.py:205-349).  The reference has no native
@@ -42,10 +42,10 @@ const char* mhmr_last_error(void);
 #define MHMR_EPI_BIAS_F32 5      /* out32 = acc (+ bias)              — HPH to_kv, cross_attn_transformer.py:187 */
 
 /* C = epilogue(A[M,K] x W[N,K]^T): fp16 operands (K contiguous, torch nn.Linear weight layout), fp32
- * accumulation on the tcgen05 tensor cores.  Replaces torch.nn.functional.linear on the hot path
+ * accumulation on the wgmma tensor cores.  Replaces torch.nn.functional.linear on the hot path
  * (reference blocks/dinov2.py:25 -> dinov2 Attention/Mlp; model.py:135; cross_attn_transformer.py:187).
  * Row remap for MHMR_EPI_ROWADD_F32: out_row = (m / rows_in) * rows_out + row_off + m % rows_in.
- * block_n: 128 or 256 = single-CTA 128 x block_n tiles; 512 = CTA pairs (tcgen05 cta_group::2), 256 x 256 tiles. */
+ * block_n: 128 or 256 = single-CTA 128 x block_n tiles; 512 = CTA pairs (2-CTA cluster sharing the weight tile), 256 x 256 tiles. */
 int mhmr_op_gemm_f16(const void* A, int64_t lda, const void* W, int64_t ldw, int M, int N, int K,
                      int epilogue, const float* bias, const float* gamma, const float* rowadd,
                      void* out, int64_t ldo, int rows_in, int rows_out, int row_off, int block_n,

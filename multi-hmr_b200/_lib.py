@@ -1,4 +1,4 @@
-"""ctypes binding of libmhmr_sm100.so (the C-ABI declared in include/mhmr.h).
+"""ctypes binding of libmhmr_sm90.so (the C-ABI declared in include/mhmr.h).
 
 The library is built in-tree by build.py.  Importing this module never falls back to another
 implementation: if the shared object is missing it is (re)built, and if that fails the import raises.
@@ -10,7 +10,7 @@ import os
 import re
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "libmhmr_sm100.so")
+LIB_PATH = os.path.join(_HERE, "libmhmr_sm90.so")
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "mhmr.h")
 
 c_void_p, c_int, c_int64, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float

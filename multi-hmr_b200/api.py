@@ -3,7 +3,7 @@
 
     open_image, get_camera_parameters, load_model, forward_model
 
-Only the forward itself is B200-native; image decoding stays on the host (PIL), as in the reference.
+Only the forward itself is H100-native; image decoding stays on the host (PIL), as in the reference.
 """
 from __future__ import annotations
 

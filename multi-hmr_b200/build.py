@@ -1,4 +1,4 @@
-"""Builds libmhmr_sm100.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libmhmr_sm90.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
 Usage: python multi-hmr_b200/build.py [--force] [--verbose]
 """
@@ -13,11 +13,11 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
-LIB = os.path.join(HERE, "libmhmr_sm100.so")
+LIB = os.path.join(HERE, "libmhmr_sm90.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -67,7 +67,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         objs = list(ex.map(lambda s: _compile(s, force, verbose), srcs))
     newest = max(os.path.getmtime(o) for o in objs)
     if force or not os.path.exists(LIB) or os.path.getmtime(LIB) < newest:
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs]
+        cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB, *objs]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:
             raise RuntimeError("link failed:\n" + res.stdout + res.stderr)

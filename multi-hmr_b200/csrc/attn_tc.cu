@@ -1,59 +1,22 @@
-// Multi-head self-attention of the DINOv2 backbone (head dim 64) on tcgen05 tensor cores.
+// Multi-head self-attention of the DINOv2 backbone (head dim 64) on wgmma tensor cores.
 //
 // Replaces `softmax(q k^T / 8) v` of dinov2 `Attention.forward` (reached from the reference at
 // blocks/dinov2.py:25; SURVEY.md §2.4 k4).  Flash-style: the T x T score matrix never leaves the SM.
 //
-//   grid  = one PERSISTENT CTA per SM.  Work items = (image, head, pair of 128-row query tiles), assigned
-//           statically (item i -> CTA i mod grid), query pair fastest so that the CTAs running at the same time
-//           share the K/V of few (image, head) pairs in L2; the ragged last pair of every (image, head) comes
-//           last.  TMEM, barriers and the K/V rings live across items: the next item's Q is prefetched into the
-//           other half of a double-buffered Q area and its first Q K^T is issued while the softmax warps still
-//           finish the previous item, so a CTA pays its prologue and tail once per launch instead of once per
-//           item (r01: 2176 CTAs = 14.7 waves, each with TMEM allocation, barrier init, cold Q/K loads and an
-//           un-overlapped O epilogue: ~18 % of the kernel).
-//   CTA   = 384 threads = 3 warpgroups: warp 0 TMA, warp 1 MMA issuer (warps 2-3 idle) | warps 4-7 softmax
-//           of query tile 0 | warps 8-11 softmax of query tile 1 (1 thread = 1 query row; setmaxnreg
-//           80 / 208 / 208 registers)
-//   TMEM  = 512 columns: per query tile  S (128 fp32) | P (64 cols = 128 fp16, A operand of P V) | O (64 fp32)
-//   smem  = Q (2 items x 2 tiles x 16 KB) | K ring | V ring (16 KB tiles of 128 keys, 128B swizzle, one TMA each)
-//   S = Q K^T : tcgen05.mma SS, M=128 N=128 K=64     (K tile K-major)
-//   O += P V  : tcgen05.mma TS, M=128 N=64  K=128    (V tile MN-major)
-//   MMA order per key tile j:  S0(j+1) = Q0 K(j+1)^T | O1 += P1(j-1) V(j-1) | S1(j+1) | O0 += P0(j) V(j)
-//   (j+1 of the last key tile of an item = key tile 0 of the CTA's next item)
-// Online softmax in fp32 in the exp2 domain (packed f32x2 FMA/ADD, 3-input max) with lazy rescaling of O
-// (only when the running max grows by more than 2^8), so the O read-modify-write through tcgen05.ld/st is rare.
+//   grid  = one CTA per (image, head, 128-row query tile); query tile fastest, so that the CTAs running at the
+//           same time share the K / V of few (image, head) pairs in L2.
+//   CTA   = 384 threads = 3 warpgroups: warpgroup 0 loads Q once and streams K / V tiles of 128 keys through a
+//           ring of smem stages (TMA, one elected lane of warp 0); warpgroups 1 and 2 each own 64 query rows.
+//   smem  = Q (16 KB) | kStages x (K 16 KB | V 16 KB), 128B swizzle, one TMA box per tile.
+//   S = Q K^T : wgmma m64n128k16, A = Q (smem, K-major), B = K tile (smem, K-major); S in registers.
+//   O += P V  : wgmma m64n64k16, A = P (registers: the fp16 S fragments ARE the A fragments of the next MMA),
+//               B = V tile (smem, MN-major).
+// Online softmax in fp32 in the exp2 domain; each thread holds 2 rows x 32 columns of S, the row max and sum
+// are reduced over the 4 lanes that share a row.
 //
-// What bounds it (SM-clock traces of the protocol events, tools/attn_trace.py, profiles/r01d_attention_timeline.md):
-// per key tile a softmax warp needs >= 1024 clk of MUFU.EX2 issue (128 exponentials, 4 lanes/clk per SM
-// sub-partition) and ~1100 clk of everything else (TMEM load, row max, scale-and-shift, row sum, fp16 packing,
-// P store, barrier round trips).  The MUFU unit of a sub-partition is only kept busy when the two warps that
-// share it are in DIFFERENT phases.  Two independent co-resident CTAs (the first design) drift into the same
-// phase and stay there (2250 clk per tile pair in anti-phase, 3450 clk in phase).  Here both query tiles live in
-// ONE CTA and the two warps of a sub-partition hand a token back and forth:
-//   exps(tile 0, j) -> exps(tile 1, j) -> exps(tile 0, j+1) ...
-// The exponentials are issued as one uninterrupted MUFU run (a branch keeps ptxas from weaving other work
-// into it); everything else runs under the partner's run.  K / V tiles are fetched once per 256 query rows.
-//
-// Issue warps run the whole warp on uniform control flow and elect one lane per issue (elect_one_sync): under
-// `if (lane == 0)` every TMA / MMA / commit costs ~80 clk in an elect-and-retry loop.
-//
-// Barrier phases are tracked with running per-pipeline counters (key tiles fetched, Q K^T / P V issued per
-// query tile, tiles consumed per softmax warp, tokens passed), never with the key-tile index of an item.
-//
-// Ragged sequence (T = N + 1 is 1 mod 128 for every Multi-HMR resolution):
-//   * the last key tile only computes the 16-column groups that hold real keys (QK^T with N = 16..128,
-//     PV with K = 16..128, softmax over the needed 32-column chunks);
-//   * softmax warps whose 32 query rows are all beyond T only keep the barrier protocol alive;
-//   * the last item of an (image, head) holds a single query tile when ceil(T/128) is odd.
-//
-// Diagnostics (never on the product path): MHMR_ATTN_ABLATE=1 (no exponentials) / 4 (protocol only) time the
-// kernel with parts of the softmax removed (wrong results); MHMR_ATTN_ABLATE=7 MHMR_ATTN_TRACE=<file> dumps the
-// SM-clock timeline of the first item of a few CTAs.
-#include <cstdio>
-#include <cstdlib>
-#include <type_traits>
-#include <vector>
-
+// Ragged sequence (T = N + 1 is 1 mod 128 for every Multi-HMR resolution): keys beyond T in the last tile are
+// masked to -inf (the rows there belong to the next image or are zero-filled by TMA); query rows beyond T are
+// computed and not stored.
 #include "kernels.cuh"
 
 namespace mhmr {
@@ -64,667 +27,179 @@ constexpr int kHeadDim = 64;
 constexpr int kBlockQ = 128;
 constexpr int kBlockKV = 128;
 constexpr int kTileBytes = 128 * kHeadDim * 2;  // 16 KB: Q, K or V tile
-constexpr int kBarrierBytes = 512;              // mbarriers + the TMEM slot
-constexpr int kStagesK = 4, kStagesV = 4;
-constexpr int kQTiles = 4;    // two items x two query tiles
-constexpr int kDefaultSimtTail = -1; // MHMR_ATTN_TAIL: 1 / 0 force the SIMT tail rows on / off, -1 = decide per problem
-constexpr int kPassAt = 112;  // exponentials issued before the MUFU token is handed on (measured optimum)
-
-constexpr uint32_t kColS = 0;
-constexpr uint32_t kColP = 128;
-constexpr uint32_t kColO = 192;
-constexpr float kRescaleThreshold = 8.0f;  // log2 units
-
-// A condition the compilers cannot fold (always true).  ptxas schedules within basic blocks: a branch on it
-// keeps the instructions that follow from being woven into the instructions before it.
-__device__ __forceinline__ bool opaque_true() {
-  uint32_t v;
-  asm volatile("mov.u32 %0, %%laneid;" : "=r"(v)::"memory");
-  return v < 32u;
-}
-
-// Timeline tracing (MHMR_ATTN_ABLATE=7 MHMR_ATTN_TRACE=file): SM-clock stamps of the protocol events of a few CTAs.
-__device__ uint32_t* g_attn_trace = nullptr;
-constexpr int kTraceIters = 40, kTraceEvents = 16, kTraceCtas = 8;
-__device__ __forceinline__ uint32_t clk_after(float dep) {
-  uint32_t t;
-  asm volatile("mov.u32 %0, %%clock;" : "=r"(t) : "f"(dep) : "memory");
-  return t;
-}
-
+constexpr int kStages = 3;
 constexpr int kAttnThreads = 384;
-constexpr int kRegsIssue = 88, kRegsSoftmax = 208;  // 128 * (88 + 2 * 208) <= 64 K registers
-// Q tiles + K ring + V ring + 1 KB that covers both the 1024-byte alignment of the tiles and the barriers
-// (in front of the tiles when the alignment pad leaves room, behind them otherwise)
-constexpr int attn_smem_bytes(int sk, int sv) { return kTileBytes * (kQTiles + sk + sv) + 1024; }
+constexpr int kRegsProducer = 40, kRegsConsumer = 232;
+// Q + K/V ring + 1 KB alignment pad + barriers
+constexpr int kAttnSmemBytes = kTileBytes * (1 + 2 * kStages) + 1024 + 256;
 
-// Work item -> (image, head, first query row).  Items [0, n_main) are the query-tile pairs qp < n_qp - 1 (query
-// pair fastest); items [n_main, n_items) are the ragged last pairs of every (image, head): cheaper, scheduled last.
-struct AttnItem {
-  int img, head, q0;
-  bool two;
-};
-__device__ __forceinline__ AttnItem attn_decode_item(int idx, int n_qp, int heads, int bh, int T) {
-  AttnItem it;
-  const int n_main = bh * (n_qp - 1);
-  int r, qp;
-  if (idx < n_main) {
-    qp = idx % (n_qp - 1);
-    r = idx / (n_qp - 1);
-  } else {
-    qp = n_qp - 1;
-    r = idx - n_main;
-  }
-  it.head = r % heads;
-  it.img = r / heads;
-  it.q0 = qp * (2 * kBlockQ);
-  it.two = (it.q0 + kBlockQ) < T;
-  return it;
+__device__ __forceinline__ float ex2(float x) {
+  float e;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x));
+  return e;
+}
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-template <int kSK, int kSV, int kAb = 0>
 __global__ void __launch_bounds__(kAttnThreads, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __half* __restrict__ qkv, int64_t ld_qkv,
-                __half* __restrict__ out, int64_t ldo, int T, int D, int heads, int bh, int n_qp, int n_items,
-                int tail_rows, float scale_log2) {
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ out, int64_t ldo, int T, int D,
+                int heads, int n_qt, float scale_log2) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sQ = smem;                                  // [2 items][2 tiles]
-  uint8_t* sK = smem + kTileBytes * kQTiles;           // [kSK]
-  uint8_t* sV = smem + kTileBytes * (kQTiles + kSK);   // [kSV]
-  uint64_t* bars = reinterpret_cast<uint64_t*>((smem - smem_raw) >= kBarrierBytes ? smem_raw
-                                                                                  : smem + kTileBytes * (kQTiles + kSK + kSV));
-  uint64_t* q_full = bars;                 // [2]    TMA -> MMA : Q tiles of an item landed
-  uint64_t* q_empty = bars + 2;            // [2]    MMA -> TMA : every Q K^T of the item that used this half is complete
-  uint64_t* k_full = bars + 4;             // [kSK]  TMA -> MMA
-  uint64_t* v_full = k_full + kSK;         // [kSV]  TMA -> MMA
-  uint64_t* k_empty = v_full + kSV;        // [kSK]  MMA -> TMA : Q_t K_j^T complete for both query tiles
-  uint64_t* v_empty = k_empty + kSK;       // [kSV]  MMA -> TMA : P_t V_j complete for both query tiles
-  uint64_t* s_full = v_empty + kSV;        // [2]    MMA -> softmax t : S_t complete
-  uint64_t* s_empty = s_full + 2;          // [2]    softmax t -> MMA : S_t now in registers
-  uint64_t* p_full = s_empty + 2;          // [2]    softmax t -> MMA : P_t in TMEM (and O_t rescaled / drained)
-  uint64_t* pv_done = p_full + 2;          // [2]    MMA -> softmax t : O_t += P_t V complete
-  // MUFU token of each sub-partition.  (Plain shared-memory counters polled with volatile loads were tried
-  // instead of mbarriers: the hand-over is quicker, but the polling LDS share the MIO queue with the
-  // partner's MUFU.EX2 and the kernel gets 8 % slower.)
-  uint64_t* turn_a = pv_done + 2;          // [4]    tile-0 warp -> tile-1 warp of a sub-partition: exps done
-  uint64_t* turn_b = turn_a + 4;           // [4]    tile-1 warp -> tile-0 warp: exps done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(turn_b + 4);
-  static_assert((4 + 2 * kSK + 2 * kSV + 16) * 8 + 4 <= kBarrierBytes, "barrier area too small");
+  uint8_t* sQ = smem;
+  uint8_t* sKV = smem + kTileBytes;  // stage s: K at sKV + 2 s kTileBytes, V right behind it
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kTileBytes * (1 + 2 * kStages));
+  uint64_t* q_full = bars;                 // TMA -> consumers
+  uint64_t* kv_full = bars + 1;            // [kStages]  TMA -> consumers
+  uint64_t* kv_empty = kv_full + kStages;  // [kStages]  consumers -> TMA
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const int qt = blockIdx.x % n_qt;
+  const int bh = blockIdx.x / n_qt;
+  const int head = bh % heads, img = bh / heads;
+  const int q0 = qt * kBlockQ;
+  const int row0 = img * T;  // first token row of this image in the [B*T, 3D] matrix
   const int n_kv = (T + kBlockKV - 1) / kBlockKV;
-  const int last_valid = T - (n_kv - 1) * kBlockKV;
-  const int last_cols = (last_valid + 15) & ~15;
-  const int first_item = blockIdx.x, item_stride = gridDim.x;
 
   griddep_launch_dependents();
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmQKV);
-      for (int s = 0; s < 2; ++s) {
-        mbar_init(&q_full[s], 1);
-        mbar_init(&q_empty[s], 1);
-      }
-      for (int s = 0; s < kSK; ++s) {
-        mbar_init(&k_full[s], 1);
-        mbar_init(&k_empty[s], 1);
-      }
-      for (int s = 0; s < kSV; ++s) {
-        mbar_init(&v_full[s], 1);
-        mbar_init(&v_empty[s], 1);
-      }
-      for (int t = 0; t < 2; ++t) {
-        mbar_init(&s_full[t], 1);
-        mbar_init(&s_empty[t], 4);
-        mbar_init(&p_full[t], 4);
-        mbar_init(&pv_done[t], 1);
-      }
-      for (int q = 0; q < 4; ++q) {
-        mbar_init(&turn_a[q], 1);
-        mbar_init(&turn_b[q], 1);
-      }
-      fence_barrier_init();
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQKV);
+    mbar_init(q_full, 1);
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&kv_full[s], 1);
+      mbar_init(&kv_empty[s], 2);  // one arrive per consumer warpgroup
     }
-    __syncwarp();
-    tmem_alloc<512>(tmem_slot);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();  // qkv of the preceding GEMM is complete and visible
-  constexpr bool kTrace = (kAb == 7);
-  uint32_t* trace = nullptr;
-  if constexpr (kTrace) {
-    const int lin = blockIdx.x;
-    if (g_attn_trace != nullptr && lin >= 3 && (lin - 3) % 17 == 0 && (lin - 3) / 17 < kTraceCtas)
-      trace = g_attn_trace + ((lin - 3) / 17) * kTraceIters * kTraceEvents;
-  }
-  auto stamp = [&](int j, int ev, float dep) {
-    if constexpr (kTrace) {
-      if (trace != nullptr && j < kTraceIters) trace[j * kTraceEvents + ev] = clk_after(dep);
-    }
-  };
 
-  if (warp == 0) {
-    // ------------------------------ TMA producer ------------------------------
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsIssue));
-    uint32_t kt = 0, it = 0;  // key tiles fetched, items started
-    for (int item = first_item; item < n_items; item += item_stride, ++it) {
-      const AttnItem a = attn_decode_item(item, n_qp, heads, bh, T);
-      const int row0 = a.img * T;  // first token row of this image in the [B*T, 3D] matrix
-      const uint32_t qb = it & 1u;
-      mbar_wait(&q_empty[qb], ((it >> 1) & 1u) ^ 1u);
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsProducer));
+    if (warp == 0) {
       if (elect_one_sync()) {
-        uint8_t* dq = sQ + qb * 2 * kTileBytes;
-        mbar_arrive_expect_tx(&q_full[qb], a.two ? 2 * kTileBytes : kTileBytes);
-        // Q is read once per item, K / V by every item of the (image, head): keep K / V in L2 (r02 capture of the
-        // persistent kernel without hints: 327 MB of DRAM reads per launch for 201 MB of qkv)
-        tma_load_2d_hint(dq, &tmQKV, &q_full[qb], a.head * kHeadDim, row0 + a.q0, kCacheEvictFirst);
-        if (a.two)
-          tma_load_2d_hint(dq + kTileBytes, &tmQKV, &q_full[qb], a.head * kHeadDim, row0 + a.q0 + kBlockQ, kCacheEvictFirst);
-      }
-      for (int j = 0; j < n_kv; ++j, ++kt) {
-        const uint32_t sk = kt % kSK, sv = kt % kSV;
-        mbar_wait(&k_empty[sk], ((kt / kSK) & 1u) ^ 1u);
-        if (elect_one_sync()) {
-          mbar_arrive_expect_tx(&k_full[sk], kTileBytes);
-          tma_load_2d_hint(sK + sk * kTileBytes, &tmQKV, &k_full[sk], D + a.head * kHeadDim, row0 + j * kBlockKV, kCacheEvictLast);
-        }
-        mbar_wait(&v_empty[sv], ((kt / kSV) & 1u) ^ 1u);
-        if (elect_one_sync()) {
-          mbar_arrive_expect_tx(&v_full[sv], kTileBytes);
-          tma_load_2d_hint(sV + sv * kTileBytes, &tmQKV, &v_full[sv], 2 * D + a.head * kHeadDim, row0 + j * kBlockKV, kCacheEvictLast);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer --------------------------------
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsIssue));
-    constexpr uint32_t idesc_pv = make_idesc_f16(128, 64, false, true);  // B (V) is MN-major
-    uint32_t n_qk[2] = {0u, 0u};  // Q K^T issued on query tile t so far (all items)
-    uint32_t n_pv[2] = {0u, 0u};  // P V issued on query tile t so far
-    // S_t = Q_t K^T for key tile `kt_idx` (ring position) / `j` (index in the item); Q from half `qb`.
-    // `release_k`: last reader of the K stage; `release_q`: last Q K^T of the item on its last tile.
-    auto issue_qk = [&](uint32_t qb, uint32_t kt_idx, int j, int t, bool release_k, bool release_q) {
-      if (n_qk[t] > 0) mbar_wait(&s_empty[t], (n_qk[t] - 1u) & 1u);  // the previous S_t is in registers
-      tc_fence_after();
-      const uint32_t s = kt_idx % kSK;
-      const int ncols = (j == n_kv - 1) ? last_cols : kBlockKV;
-      const uint32_t idesc_qk = make_idesc_f16(128, ncols, false, false);
-      const uint64_t q_desc = make_sw128_desc(smem_u32(sQ + (qb * 2 + t) * kTileBytes), 16, 1024);
-      const uint64_t k_desc = make_sw128_desc(smem_u32(sK + s * kTileBytes), 16, 1024);
-      const uint32_t t_s = tmem_base + t * 256 + kColS;
-      if (elect_one_sync()) {
-#pragma unroll
-        for (int k = 0; k < kHeadDim / 16; ++k)
-          umma_f16_ss(t_s, q_desc + 2u * k, k_desc + 2u * k, idesc_qk, k > 0 ? 1u : 0u);
-        if (release_k) umma_commit(&k_empty[s]);
-        if (release_q) umma_commit(&q_empty[qb]);
-        umma_commit(&s_full[t]);
+        mbar_arrive_expect_tx(q_full, kTileBytes);
+        // Q is read by one CTA, K / V by every query tile of the (image, head): keep K / V in L2
+        tma_load_2d_hint(sQ, &tmQKV, q_full, head * kHeadDim, row0 + q0, kCacheEvictFirst);
       }
       __syncwarp();
-      ++n_qk[t];
-    };
-    // O_t += P_t V for key tile `kt_idx` / `j`; `release_v`: last reader of the V stage
-    auto issue_pv = [&](uint32_t kt_idx, int j, int t, bool release_v) {
-      mbar_wait(&p_full[t], n_pv[t] & 1u);
-      tc_fence_after();
-      const uint32_t s = kt_idx % kSV;
-      // V tile: 128 keys (K) x 64 dims (N), N contiguous: MN-major, 8-key groups 1024 B apart.
-      const uint64_t v_desc = make_sw128_desc(smem_u32(sV + s * kTileBytes), 1024, 1024);
-      const uint32_t t_p = tmem_base + t * 256 + kColP;
-      const uint32_t t_o = tmem_base + t * 256 + kColO;
-      const int ksteps = ((j == n_kv - 1) ? last_cols : kBlockKV) / 16;
-      if (elect_one_sync()) {
-        for (int k = 0; k < ksteps; ++k)  // A: 8 TMEM columns of P per K step; B: 16 keys = 2048 B per K step
-          umma_f16_ts(t_o, t_p + 8u * k, v_desc + 128u * k, idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-        if (release_v) umma_commit(&v_empty[s]);
-        umma_commit(&pv_done[t]);
-      }
-      __syncwarp();
-      ++n_pv[t];
-    };
-
-    uint32_t kt = 0, it = 0;
-    int item = first_item;
-    if (item < n_items) {
-      AttnItem cur = attn_decode_item(item, n_qp, heads, bh, T);
-      mbar_wait(&q_full[0], 0);
-      mbar_wait(&k_full[0], 0);
-      issue_qk(0, 0, 0, 0, !cur.two, !cur.two && n_kv == 1);
-      if (cur.two) issue_qk(0, 0, 0, 1, true, n_kv == 1);
-      while (true) {
-        const int next_item = item + item_stride;
-        const bool has_next = next_item < n_items;
-        AttnItem nxt = cur;
-        if (has_next) nxt = attn_decode_item(next_item, n_qp, heads, bh, T);
-        const uint32_t qb = it & 1u;
-        for (int j = 0; j < n_kv; ++j, ++kt) {
-          // the step that follows (item, j): (item, j + 1), or key tile 0 of the CTA's next item
-          const bool in_item = (j + 1 < n_kv);
-          const bool follow = in_item || has_next;
-          const AttnItem& f = in_item ? cur : nxt;
-          const uint32_t fqb = in_item ? qb : (qb ^ 1u);
-          const int fj = in_item ? j + 1 : 0;
-          const bool f_last = (fj == n_kv - 1);
-          if (follow) {
-            if (!in_item) mbar_wait(&q_full[fqb], ((it + 1u) >> 1) & 1u);
-            mbar_wait(&k_full[(kt + 1u) % kSK], ((kt + 1u) / kSK) & 1u);
-            issue_qk(fqb, kt + 1u, fj, 0, !f.two, !f.two && f_last);
-          }
-          if (cur.two && j >= 1) issue_pv(kt - 1u, j - 1, 1, true);
-          if (follow && f.two) issue_qk(fqb, kt + 1u, fj, 1, true, f_last);
-          mbar_wait(&v_full[kt % kSV], (kt / kSV) & 1u);
-          issue_pv(kt, j, 0, !cur.two);
+      for (int j = 0; j < n_kv; ++j) {
+        const int s = j % kStages;
+        mbar_wait(&kv_empty[s], ((j / kStages) & 1) ^ 1);
+        if (elect_one_sync()) {
+          uint8_t* dk = sKV + 2 * s * kTileBytes;
+          mbar_arrive_expect_tx(&kv_full[s], 2 * kTileBytes);
+          tma_load_2d_hint(dk, &tmQKV, &kv_full[s], D + head * kHeadDim, row0 + j * kBlockKV, kCacheEvictLast);
+          tma_load_2d_hint(dk + kTileBytes, &tmQKV, &kv_full[s], 2 * D + head * kHeadDim, row0 + j * kBlockKV,
+                           kCacheEvictLast);
         }
-        if (cur.two) issue_pv(kt - 1u, n_kv - 1, 1, true);
-        if (!has_next) break;
-        item = next_item;
-        cur = nxt;
-        ++it;
-      }
-    }
-  } else if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsIssue));
-    // ------------------------------ ragged tail rows (SIMT) ---------------------
-    // T = N + 1 leaves T mod 256 query rows (1 for every Multi-HMR resolution but 1288: 17) beyond the full
-    // query-tile pairs.  As a work item of the tensor-core path such a row costs almost a full item (one softmax
-    // warp works alone, 127 of 128 MMA rows are padding): 128 items = 5 % of the kernel at 896 / batch 8.  These two
-    // otherwise idle warps compute them instead, concurrently with the items of the CTA: task = (image, head, row),
-    // 8 lanes per key (8 head dims each), 8 keys in flight per iteration, fp32 online softmax in the exp2 domain.
-    if (tail_rows > 0) {
-      __shared__ float tail_scratch[8][12];
-      const int w2 = warp - 2, grp = lane >> 3, sub8 = lane & 7;
-      const int n_tasks = bh * tail_rows;
-      for (int task = gridDim.x - 1 - blockIdx.x; task < n_tasks; task += gridDim.x) {
-        const int r = task / tail_rows, qrow = n_qp * (2 * kBlockQ) + (task - r * tail_rows);
-        const int head = r % heads, img = r / heads;
-        const __half* base = qkv + static_cast<int64_t>(img) * T * ld_qkv + head * kHeadDim + 8 * sub8;
-        float q[8];
-        {
-          const uint4 pk = *reinterpret_cast<const uint4*>(base + static_cast<int64_t>(qrow) * ld_qkv);
-          const __half2* h2 = reinterpret_cast<const __half2*>(&pk);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float2 f = __half22float2(h2[i]);
-            q[2 * i] = f.x * scale_log2;
-            q[2 * i + 1] = f.y * scale_log2;
-          }
-        }
-        float m = -INFINITY, l = 0.f, acc[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-        constexpr int kU = 4;  // keys in flight per lane group
-        // warp-uniform trip count (the shuffles below need every lane): the loop runs over 32-key blocks, each lane
-        // group takes key kb + w2 * 4 + grp + 8 u of the block and masks the keys beyond T
-        for (int kb = 0; kb < T; kb += 8 * kU) {
-          const int k0 = kb + w2 * 4 + grp;
-          uint4 kk[kU], vv[kU];
-#pragma unroll
-          for (int u = 0; u < kU; ++u) {
-            const int key = k0 + 8 * u;
-            const int64_t off = static_cast<int64_t>(key < T ? key : 0) * ld_qkv;
-            kk[u] = *reinterpret_cast<const uint4*>(base + off + D);
-            vv[u] = *reinterpret_cast<const uint4*>(base + off + 2 * D);
-          }
-#pragma unroll
-          for (int u = 0; u < kU; ++u) {
-            const __half2* k2 = reinterpret_cast<const __half2*>(&kk[u]);
-            float sdot = 0.f;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 f = __half22float2(k2[i]);
-              sdot = fmaf(q[2 * i], f.x, sdot);
-              sdot = fmaf(q[2 * i + 1], f.y, sdot);
-            }
-            sdot += __shfl_xor_sync(0xffffffffu, sdot, 1);
-            sdot += __shfl_xor_sync(0xffffffffu, sdot, 2);
-            sdot += __shfl_xor_sync(0xffffffffu, sdot, 4);
-            if (k0 + 8 * u >= T) sdot = -INFINITY;
-            const float mn = fmaxf(m, sdot);
-            const float a = (mn == -INFINITY) ? 1.f : exp2f(m - mn);
-            const float p = (mn == -INFINITY) ? 0.f : exp2f(sdot - mn);
-            l = l * a + p;
-            const __half2* v2 = reinterpret_cast<const __half2*>(&vv[u]);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 f = __half22float2(v2[i]);
-              acc[2 * i] = fmaf(p, f.x, acc[2 * i] * a);
-              acc[2 * i + 1] = fmaf(p, f.y, acc[2 * i + 1] * a);
-            }
-            m = mn;
-          }
-        }
-        // merge the 4 lane groups of the warp, then the two warps through shared memory
-#pragma unroll
-        for (int o = 8; o <= 16; o <<= 1) {
-          const float m2 = __shfl_xor_sync(0xffffffffu, m, o);
-          const float l2 = __shfl_xor_sync(0xffffffffu, l, o);
-          const float mn = fmaxf(m, m2);
-          const float a = (m == -INFINITY) ? 0.f : exp2f(m - mn);
-          const float b = (m2 == -INFINITY) ? 0.f : exp2f(m2 - mn);
-          l = l * a + l2 * b;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float c2 = __shfl_xor_sync(0xffffffffu, acc[i], o);
-            acc[i] = acc[i] * a + c2 * b;
-          }
-          m = mn;
-        }
-        if (w2 == 1 && lane < 8) {
-          tail_scratch[lane][0] = m;
-          tail_scratch[lane][1] = l;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) tail_scratch[lane][2 + i] = acc[i];
-        }
-        asm volatile("bar.sync 1, 64;" ::: "memory");
-        if (w2 == 0 && lane < 8) {
-          const float m2 = tail_scratch[lane][0], l2 = tail_scratch[lane][1];
-          const float mn = fmaxf(m, m2);
-          const float a = (m == -INFINITY) ? 0.f : exp2f(m - mn);
-          const float b = (m2 == -INFINITY) ? 0.f : exp2f(m2 - mn);
-          const float inv = 1.0f / (l * a + l2 * b);
-          uint4 pk;
-          uint32_t* pw = reinterpret_cast<uint32_t*>(&pk);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const __half2 h = __floats2half2_rn((acc[2 * i] * a + tail_scratch[lane][2 + 2 * i] * b) * inv,
-                                                (acc[2 * i + 1] * a + tail_scratch[lane][3 + 2 * i] * b) * inv);
-            pw[i] = *reinterpret_cast<const uint32_t*>(&h);
-          }
-          *reinterpret_cast<uint4*>(out + (static_cast<int64_t>(img) * T + qrow) * ldo + head * kHeadDim + 8 * sub8) = pk;
-        }
-        asm volatile("bar.sync 1, 64;" ::: "memory");  // the scratch is free for the next task
-      }
-    }
-  } else {
-    // ------------------------------ Softmax warps ------------------------------
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsSoftmax));
-    const int t = (warp - 4) >> 2;        // query tile of this warp
-    const int sub = warp & 3;             // TMEM sub-partition (lane quarter) = SM sub-partition of this warp
-    const int row = sub * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(sub * 32) << 16;
-    const uint32_t t_s = tmem_base + lane_base + t * 256 + kColS;
-    const uint32_t t_p = tmem_base + lane_base + t * 256 + kColP;
-    const uint32_t t_o = tmem_base + lane_base + t * 256 + kColO;
-    uint64_t* my_s_full = &s_full[t];
-    uint64_t* my_s_empty = &s_empty[t];
-    uint64_t* my_p_full = &p_full[t];
-    uint64_t* my_pv_done = &pv_done[t];
-    uint64_t* turn_wait = (t == 0) ? &turn_b[sub] : &turn_a[sub];
-    uint64_t* turn_pass = (t == 0) ? &turn_a[sub] : &turn_b[sub];
-    uint32_t n_t = 0;   // key tiles this warp's query tile has been through (all items): phase of s_full / pv_done
-    uint32_t n_tok = 0; // tokens this warp has passed on (two-tile items only)
-    const int last_nch = (last_cols + 31) >> 5;  // 32-column chunks of the last tile that hold real keys
-    const bool tracer_warp = kTrace && sub == 0 && lane == 0;
-
-    for (int item = first_item, seq = 0; item < n_items; item += item_stride, ++seq) {
-      const AttnItem a = attn_decode_item(item, n_qp, heads, bh, T);
-      if (t == 1 && !a.two) continue;  // no second query tile in this item (the MMA warp issues nothing for it)
-      const bool two = a.two;
-      const int qt0 = a.q0 + t * kBlockQ;
-      const bool warp_has_rows = (qt0 + sub * 32) < T;  // warp-uniform
-      const bool row_valid = (qt0 + row) < T;
-      __half* const dst = out + static_cast<int64_t>(a.img * T + qt0 + row) * ldo + a.head * kHeadDim;
-      const uint32_t nb = n_t;                          // phase base of this item
-      // exps(tile 0) waits for the previous exps(tile 1) (none before the CTA's first); exps(tile 1) waits for
-      // exps(tile 0) of the same key tile
-      auto take_turn = [&]() {
-        if (two) {
-          if (t == 0) {
-            if (n_tok > 0) mbar_wait(turn_wait, (n_tok - 1u) & 1u);
-          } else {
-            mbar_wait(turn_wait, n_tok & 1u);
-          }
-        }
-      };
-      auto pass_turn = [&]() {
-        if (two) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(turn_pass);
-          ++n_tok;
-        }
-      };
-
-      if (!warp_has_rows) {
-        // All 32 rows of this warp are beyond the sequence: their S/P/O lanes hold garbage that is never
-        // stored and never mixes with other rows (the MMAs are row-independent); keep the protocol alive.
-        for (int j = 0; j < n_kv; ++j) {
-          mbar_wait(my_s_full, (nb + j) & 1u);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(my_s_empty);
-          take_turn();
-          pass_turn();
-          // arrive on p_full only once the previous P V of this query tile is over: this warp runs ahead of the
-          // warps that do have rows, and an early arrival would complete THEIR pending phase
-          if (nb + j > 0) mbar_wait(my_pv_done, (nb + j - 1u) & 1u);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(my_p_full);
-        }
-        mbar_wait(my_pv_done, (nb + n_kv - 1u) & 1u);
-        n_t = nb + n_kv;
-        continue;
-      }
-
-      float m_used = -INFINITY;  // running max (log2 domain) actually used as the exponent offset
-      float l = 0.0f;
-      const bool tracer = tracer_warp && seq == 0;
-      // One key tile.  On entry S_t(j) is complete in TMEM (the wait for it happened at the end of tile j-1 /
-      // at the start of the item).  The exponentials are issued as ONE uninterrupted run of MUFU.EX2 between
-      // take_turn and pass_turn; the scale-and-shift before and the row sum / fp16 packing after run under the
-      // partner warp's run.
-      auto softmax_tile = [&](auto nch_c, auto last_c, int j) {
-        constexpr int NCH = decltype(nch_c)::value;
-        constexpr bool kLast = decltype(last_c)::value;  // static: the key mask costs 2 instructions per score
-        uint32_t s[NCH][32];
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) tmem_ld_32x32(t_s + c * 32, s[c]);
-        tmem_ld_wait();
-        tc_fence_before();
         __syncwarp();
-        if (lane == 0) mbar_arrive(my_s_empty);
-        if (tracer) stamp(j, t * 8 + 0, __uint_as_float(s[0][0]));
-
-        if constexpr (kLast) {  // keys beyond T (or rows of the next image): -inf
-#pragma unroll
-          for (int c = 0; c < NCH; ++c)
-#pragma unroll
-            for (int k = 0; k < 32; ++k)
-              if (c * 32 + k >= last_valid) s[c][k] = 0xff800000u;
-        }
-        // row max: independent chains (3-input max), then combine
-        float mx = -INFINITY;
-        if constexpr (kAb == 4) mx = fmaxf(__uint_as_float(s[0][0]), __uint_as_float(s[0][1]));
-#pragma unroll
-        for (int c = 0; c < (kAb == 4 ? 0 : NCH); ++c) {
-          float m0 = fmaxf(__uint_as_float(s[c][0]), __uint_as_float(s[c][1]));
-#pragma unroll
-          for (int k = 2; k < 32; k += 2)
-            m0 = fmaxf(m0, fmaxf(__uint_as_float(s[c][k]), __uint_as_float(s[c][k + 1])));
-          mx = fmaxf(mx, m0);
-        }
-        const float m_new = fmaxf(m_used, mx * scale_log2);
-        const bool rescale = (m_new - m_used) > kRescaleThreshold;  // true on the first tile
-        float alpha = 1.0f;
-        if (rescale) {
-          alpha = exp2f(m_used - m_new);  // 0 on the first tile
-          m_used = m_new;
-        }
-        // (A) exponent arguments, in place
-        const float2 sc2 = make_float2(scale_log2, scale_log2);
-        const float2 nm2 = make_float2(-m_used, -m_used);
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-#pragma unroll
-          for (int k = 0; k < 32; k += 2) {
-            const float2 a2 = __ffma2_rn(make_float2(__uint_as_float(s[c][k]), __uint_as_float(s[c][k + 1])), sc2, nm2);
-            s[c][k] = __float_as_uint(a2.x);
-            s[c][k + 1] = __float_as_uint(a2.y);
-          }
-#pragma unroll
-          for (int k = 0; k < 32; k += 16)  // pin: the arguments exist before the token is requested
-            asm volatile("" : "+r"(s[c][k]), "+r"(s[c][k + 1]), "+r"(s[c][k + 2]), "+r"(s[c][k + 3]), "+r"(s[c][k + 4]),
-                              "+r"(s[c][k + 5]), "+r"(s[c][k + 6]), "+r"(s[c][k + 7]), "+r"(s[c][k + 8]), "+r"(s[c][k + 9]),
-                              "+r"(s[c][k + 10]), "+r"(s[c][k + 11]), "+r"(s[c][k + 12]), "+r"(s[c][k + 13]),
-                              "+r"(s[c][k + 14]), "+r"(s[c][k + 15]));
-        }
-        if (tracer) stamp(j, t * 8 + 1, 0.f);
-        // (B) this warp's turn on the MUFU pipe of its sub-partition
-        take_turn();
-        if (tracer) stamp(j, t * 8 + 2, 0.f);
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-#pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            if constexpr (kAb != 1 && kAb != 4) {
-              float e;
-              asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(__uint_as_float(s[c][k])));
-              s[c][k] = __float_as_uint(e);
-            }
-            // hand the token on kPassAt exponentials into the run (full tiles; at the end of a short last tile):
-            // the partner needs ~150 clk to wake up, its first exponentials then overlap this warp's last ones
-            if ((NCH == 4 && c * 32 + k + 1 == kPassAt) || (NCH < 4 && c == NCH - 1 && k == 31)) {
-              if (opaque_true()) pass_turn();
-            }
-          }
-        }
-        if (tracer) stamp(j, t * 8 + 3, __uint_as_float(s[NCH - 1][31]));
-        // (C) row sum and fp16 packing -- in a block of its own, so that it is not woven into the MUFU run
-        if (!opaque_true()) return;
-        float2 acc0 = make_float2(0.f, 0.f), acc1 = make_float2(0.f, 0.f);
-        uint32_t p[NCH][16];
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) {
-#pragma unroll
-          for (int k = 0; k < 32; k += 4) {
-            const float2 e0 = make_float2(__uint_as_float(s[c][k]), __uint_as_float(s[c][k + 1]));
-            const float2 e1 = make_float2(__uint_as_float(s[c][k + 2]), __uint_as_float(s[c][k + 3]));
-            acc0 = __fadd2_rn(acc0, e0);
-            acc1 = __fadd2_rn(acc1, e1);
-            const __half2 h0 = __floats2half2_rn(e0.x, e0.y), h1 = __floats2half2_rn(e1.x, e1.y);
-            p[c][k / 2] = *reinterpret_cast<const uint32_t*>(&h0);
-            p[c][k / 2 + 1] = *reinterpret_cast<const uint32_t*>(&h1);
-          }
-        }
-        l = l * alpha + ((acc0.x + acc0.y) + (acc1.x + acc1.y));
-        if (tracer) stamp(j, t * 8 + 4, l);
-
-        // S_t(j+1) complete also means P V(j-1) complete (the MMA warp issues it earlier): the P buffer is
-        // free and O is stable.  One wait serves both, and tile j+1 starts without waiting.
-        if (j + 1 < n_kv) {
-          mbar_wait(my_s_full, (nb + j + 1u) & 1u);
-        } else if (j > 0) {
-          mbar_wait(my_pv_done, (nb + j - 1u) & 1u);
-        }
-        tc_fence_after();
-        if (tracer) stamp(j, t * 8 + 5, 0.f);
-        if (j > 0 && __any_sync(0xffffffffu, rescale)) {  // rare after the first tiles: small chunks
-#pragma unroll 1
-          for (int c = 0; c < kHeadDim / 8; ++c) {
-            uint32_t o[8];
-            tmem_ld_32x8(t_o + c * 8, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int k = 0; k < 8; ++k) o[k] = __float_as_uint(__uint_as_float(o[k]) * alpha);
-            tmem_st_32x8(t_o + c * 8, o);
-          }
-        }
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) tmem_st_32x16(t_p + c * 16, p[c]);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(my_p_full);
-        if (tracer) stamp(j, t * 8 + 6, 0.f);
-      };
-
-      mbar_wait(my_s_full, nb & 1u);
-      tc_fence_after();
-      for (int j = 0; j < n_kv - 1; ++j) softmax_tile(std::integral_constant<int, 4>{}, std::false_type{}, j);
-      switch (last_nch) {
-        case 1: softmax_tile(std::integral_constant<int, 1>{}, std::true_type{}, n_kv - 1); break;
-        case 2: softmax_tile(std::integral_constant<int, 2>{}, std::true_type{}, n_kv - 1); break;
-        case 3: softmax_tile(std::integral_constant<int, 3>{}, std::true_type{}, n_kv - 1); break;
-        default: softmax_tile(std::integral_constant<int, 4>{}, std::true_type{}, n_kv - 1); break;
       }
+    }
+    return;
+  }
 
-      // Epilogue: O / l -> fp16 -> out[img*T + q, head*64 + :].  The first P V of the CTA's next item overwrites
-      // O; it is gated by this warp's next arrival on p_full, which comes after these loads.
-      mbar_wait(my_pv_done, (nb + n_kv - 1u) & 1u);
-      tc_fence_after();
-      const float inv_l = 1.0f / l;
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsConsumer));
+  const int cw = wg - 1;  // query rows 64 cw .. 64 cw + 63 of the tile
+  const int w = warp & 3;
+  const bool release_lane = (threadIdx.x & 127) == 0;
+  // accumulator fragments: register i holds row 16 w + lane / 4 + 8 ((i >> 1) & 1) of the warpgroup's 64 rows,
+  // column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
+  const uint64_t q_desc = make_sw128_desc(smem_u32(sQ + cw * 64 * 128), 16, 1024);
+  float o[32];
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t o[32];
-        tmem_ld_32x32(t_o + c * 32, o);
-        tmem_ld_wait();
-        if (row_valid) {
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait(q_full, 0);
+
+  for (int j = 0; j < n_kv; ++j) {
+    const int s = j % kStages;
+    mbar_wait(&kv_full[s], (j / kStages) & 1);
+    const uint32_t sk = smem_u32(sKV + 2 * s * kTileBytes);
+    const uint64_t k_desc = make_sw128_desc(sk, 16, 1024);
+    float sc[64];
+    wgmma_fence();
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4 pk;
-            uint32_t* pw = reinterpret_cast<uint32_t*>(&pk);
+    for (int k = 0; k < kHeadDim / 16; ++k) wgmma_m64n128_ss(sc, q_desc + 2u * k, k_desc + 2u * k, k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+
+    if (j == n_kv - 1) {  // keys beyond T
+      const int valid = T - j * kBlockKV;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const __half2 h = __floats2half2_rn(__uint_as_float(o[g * 8 + 2 * k]) * inv_l,
-                                                  __uint_as_float(o[g * 8 + 2 * k + 1]) * inv_l);
-              pw[k] = *reinterpret_cast<const uint32_t*>(&h);
-            }
-            *reinterpret_cast<uint4*>(dst + c * 32 + g * 8) = pk;
-          }
+      for (int i = 0; i < 64; ++i)
+        if (8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= valid) sc[i] = -INFINITY;
+    }
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int g = 0; g < 16; ++g) mx = fmaxf(mx, fmaxf(sc[4 * g + 2 * h], sc[4 * g + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx * scale_log2);
+      alpha[h] = ex2(m_run[h] - m_new);  // 0 on the first tile
+      m_run[h] = m_new;
+      float sum = 0.f;
+#pragma unroll
+      for (int g = 0; g < 16; ++g) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int i = 4 * g + 2 * h + e;
+          sc[i] = ex2(fmaf(sc[i], scale_log2, -m_new));
+          sum += sc[i];
         }
       }
-      tc_fence_before();
-      n_t = nb + n_kv;
+      l_run[h] = l_run[h] * alpha[h] + sum;  // partial over this lane's columns; reduced over the quad at the end
+    }
+#pragma unroll
+    for (int g = 0; g < 8; ++g) {
+      o[4 * g + 0] *= alpha[0];
+      o[4 * g + 1] *= alpha[0];
+      o[4 * g + 2] *= alpha[1];
+      o[4 * g + 3] *= alpha[1];
+    }
+    // P as fp16 A fragments, one set of 4 registers per 16 keys
+    uint32_t p[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      p[kk][0] = pack_half2(sc[8 * kk + 0], sc[8 * kk + 1]);
+      p[kk][1] = pack_half2(sc[8 * kk + 2], sc[8 * kk + 3]);
+      p[kk][2] = pack_half2(sc[8 * kk + 4], sc[8 * kk + 5]);
+      p[kk][3] = pack_half2(sc[8 * kk + 6], sc[8 * kk + 7]);
+    }
+    // V tile: 128 keys (K) x 64 dims (N), N contiguous: MN-major, 8-key groups 1024 B apart, 16 keys per step
+    const uint64_t v_desc = make_sw128_desc(sk + kTileBytes, 1024, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_m64n64_rs_bt(o, p[kk], v_desc + 128u * kk);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if (release_lane) mbar_arrive(&kv_empty[s]);
+  }
+
+  // epilogue: O / l -> fp16 -> out[img*T + q, head*64 + :]
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv_l = 1.0f / l;
+    const int q = q0 + cw * 64 + w * 16 + (lane >> 2) + 8 * h;
+    if (q < T) {
+      __half* dst = out + static_cast<int64_t>(row0 + q) * ldo + head * kHeadDim + 2 * (lane & 3);
+#pragma unroll
+      for (int g = 0; g < 8; ++g)
+        *reinterpret_cast<uint32_t*>(dst + 8 * g) = pack_half2(o[4 * g + 2 * h] * inv_l, o[4 * g + 2 * h + 1] * inv_l);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
-}
-
-int g_attn_ablate = -1;  // MHMR_ATTN_ABLATE: timing / tracing experiments only (see the header)
-
-struct AttnArgs {
-  CUtensorMap tm;
-  const __half* qkv;
-  int64_t ld_qkv;
-  __half* out;
-  int64_t ldo;
-  int T, D, heads, bh, n_qp, n_items, tail_rows;
-  float scale_log2;
-  int grid;
-  cudaStream_t stream;
-};
-
-template <int kAb>
-int attn_launch(const AttnArgs& a) {
-  constexpr int smem = attn_smem_bytes(kStagesK, kStagesV);
-  auto kern = attn_fwd_kernel<kStagesK, kStagesV, kAb>;
-  static PerDeviceOnce once;
-  if (once.first()) {
-    MHMR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(a.grid);
-  cfg.blockDim = dim3(kAttnThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = a.stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, a.tm, a.qkv, a.ld_qkv, a.out, a.ldo, a.T, a.D, a.heads, a.bh, a.n_qp,
-                                     a.n_items, a.tail_rows, a.scale_log2));
-  MHMR_CUDA_CHECK(cudaGetLastError());
-  return MHMR_OK;
 }
 
 }  // namespace
@@ -736,74 +211,30 @@ int attention_forward(const __half* qkv, int64_t ld_qkv, __half* out, int64_t ld
   MHMR_REQUIRE(D % kHeadDim == 0, "attention: embed dim must be a multiple of 64");
   MHMR_REQUIRE(ld_qkv % 8 == 0 && ldo % 8 == 0, "attention: row pitches must be multiples of 8");
   MHMR_REQUIRE(B > 0 && T > 0, "attention: empty problem");
-  AttnArgs a;
-  int rc = make_tmap_2d(&a.tm, qkv, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, static_cast<uint64_t>(B) * T,
-                        3ull * D, ld_qkv * 2, 128, 64, true);
+  CUtensorMap tm;
+  int rc = make_tmap_2d(&tm, qkv, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, static_cast<uint64_t>(B) * T, 3ull * D,
+                        ld_qkv * 2, 128, 64, true);
   if (rc != MHMR_OK) return rc;
-  if (g_attn_ablate < 0) {
-    const char* ab = std::getenv("MHMR_ATTN_ABLATE");
-    g_attn_ablate = (ab != nullptr) ? atoi(ab) : 0;
+  const int heads = D / kHeadDim;
+  const int n_qt = (T + kBlockQ - 1) / kBlockQ;
+  static PerDeviceOnce once;
+  if (once.first()) {
+    MHMR_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
   }
-  a.out = out;
-  a.ldo = ldo;
-  a.T = T;
-  a.D = D;
-  a.qkv = qkv;
-  a.ld_qkv = ld_qkv;
-  a.heads = D / kHeadDim;
-  a.bh = B * a.heads;
-  // query rows beyond the full 256-row pairs: few of them (<= 32) go to the SIMT tail warps, more stay a ragged item
-  static int simt_tail = -1;
-  if (simt_tail < 0) {
-    const char* te = std::getenv("MHMR_ATTN_TAIL");
-    simt_tail = (te != nullptr) ? atoi(te) : kDefaultSimtTail;
-  }
-  const int rem = T % (2 * kBlockQ);
-  bool use_tail = (simt_tail != 0 && rem >= 1 && rem <= 32);
-  if (use_tail && simt_tail < 0) {
-    // The tail warps share two sub-partitions' issue slots with softmax warps: worth it only while their work is a
-    // few per cent of the CTA's lifetime (measured r02e: -4.7 % at 896 / batch 8, +11 % at 672 / batch 4).
-    // ~200 issue-clk per 32 keys and row; ~2500 clk per key tile of an item.
-    const int sms = device_sm_count();
-    const int64_t n_full = static_cast<int64_t>(a.bh) * (T / (2 * kBlockQ));
-    const int64_t grid = n_full < sms ? (n_full > 0 ? n_full : 1) : sms;
-    const int64_t tasks_per_cta = (static_cast<int64_t>(a.bh) * rem + grid - 1) / grid;
-    const int64_t items_per_cta = (n_full + grid - 1) / grid;
-    const int64_t tail_cost = tasks_per_cta * ((T + 31) / 32) * 200;
-    const int64_t lifetime = items_per_cta * ((T + kBlockKV - 1) / kBlockKV) * 2500;
-    use_tail = n_full > 0 && tail_cost * 100 < lifetime * 3;
-  }
-  a.tail_rows = use_tail ? rem : 0;
-  a.n_qp = (a.tail_rows > 0) ? T / (2 * kBlockQ) : (T + 2 * kBlockQ - 1) / (2 * kBlockQ);
-  a.n_items = a.bh * a.n_qp;
-  a.scale_log2 = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e)
-  const int work = a.n_items > a.bh * a.tail_rows ? a.n_items : a.bh * a.tail_rows;
-  a.grid = work < device_sm_count() ? work : device_sm_count();
-  a.stream = stream;
-  if (g_attn_ablate == 1) return attn_launch<1>(a);
-  if (g_attn_ablate == 4) return attn_launch<4>(a);
-  const char* trace_path = std::getenv("MHMR_ATTN_TRACE");
-  if (g_attn_ablate == 7 && trace_path != nullptr) {
-    uint32_t* d_trace = nullptr;
-    const size_t trace_words = static_cast<size_t>(kTraceCtas) * kTraceIters * kTraceEvents;
-    MHMR_CUDA_CHECK(cudaMalloc(&d_trace, trace_words * 4));
-    MHMR_CUDA_CHECK(cudaMemset(d_trace, 0, trace_words * 4));
-    MHMR_CUDA_CHECK(cudaMemcpyToSymbol(g_attn_trace, &d_trace, sizeof(d_trace)));
-    rc = attn_launch<7>(a);
-    if (rc != MHMR_OK) return rc;
-    MHMR_CUDA_CHECK(cudaStreamSynchronize(stream));
-    std::vector<uint32_t> h(trace_words);
-    MHMR_CUDA_CHECK(cudaMemcpy(h.data(), d_trace, trace_words * 4, cudaMemcpyDeviceToHost));
-    if (FILE* f = fopen(trace_path, "wb")) {
-      fwrite(h.data(), 4, trace_words, f);
-      fclose(f);
-    }
-    cudaFree(d_trace);
-    d_trace = nullptr;
-    MHMR_CUDA_CHECK(cudaMemcpyToSymbol(g_attn_trace, &d_trace, sizeof(d_trace)));
-    return MHMR_OK;
-  }
-  return attn_launch<0>(a);
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(B * heads * n_qt);
+  cfg.blockDim = dim3(kAttnThreads);
+  cfg.dynamicSmemBytes = kAttnSmemBytes;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  const float scale_log2 = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e)
+  MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, attn_fwd_kernel, tm, out, ldo, T, D, heads, n_qt, scale_log2));
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
 }
 
 }  // namespace mhmr

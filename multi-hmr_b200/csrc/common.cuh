@@ -1,6 +1,6 @@
-// Shared device/host helpers for the sm_100a kernels of the Multi-HMR hot path.
+// Shared device/host helpers for the sm_90a kernels of the Multi-HMR hot path.
 //
-// Everything here is a thin inline-PTX wrapper (mbarrier, TMA, tcgen05/TMEM) or a
+// Everything here is a thin inline-PTX wrapper (mbarrier, TMA, clusters, wgmma) or a
 // host-side utility (error reporting, tensor-map encoding through the driver entry
 // point so the library has no link-time dependency on libcuda).
 #pragma once
@@ -17,7 +17,7 @@
 namespace mhmr {
 
 // Programmatic dependent launch (PDL).  Every kernel of the chain lets the next grid start its prologue
-// (barrier init, TMEM allocation, descriptor prefetch) while this grid drains, and waits for the full
+// (barrier init, descriptor prefetch) while this grid drains, and waits for the full
 // completion (and memory visibility) of the previous grid before it touches global memory.  Both are no-ops
 // when the kernel was launched without the programmatic-serialization attribute.
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -74,10 +74,9 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
-// One leader lane of a fully active warp (the same lane every time).  Issue loops (TMA, tcgen05.mma) run
+// One leader lane of a fully active warp (the same lane every time).  Issue loops (TMA) run
 // with the WHOLE warp on warp-uniform control flow and guard only the issuing instructions with this
-// predicate: their descriptors then live in uniform registers.  Under `if (lane == 0)` the compiler cannot
-// prove uniformity and wraps every TMA / MMA / commit in an elect-and-retry loop (~80 clk per instruction).
+// predicate: their descriptors then live in uniform registers.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred = 0;
   asm volatile(
@@ -179,146 +178,109 @@ constexpr uint64_t kCacheEvictFirst = 0x12F0000000000000ull;
 constexpr uint64_t kCacheEvictLast = 0x14F0000000000000ull;
 constexpr uint64_t kCacheEvictNormal = 0x1000000000000000ull;
 
-// ---- tcgen05 / TMEM ----------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- clusters ----------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(NCOLS)
-               : "memory");
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// Arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; one thread issues on behalf of the CTA.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
+// 2-D tile load global -> shared of every CTA in `cta_mask`, at the same offsets; each destination CTA's
+// barrier at `bar`'s offset receives the bytes.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar,
+                                                      int32_t c_inner, int32_t c_outer, uint16_t cta_mask) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
       :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on `bar` once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp receives lane (base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               :
-               : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]),
-        "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]),
-        "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]),
-        "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]),
-        "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-        "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)),
+        "r"(c_inner), "r"(c_outer), "h"(cta_mask)
       : "memory");
 }
 
-// Shared-memory matrix descriptor (sm_100 "version 1"), 128-byte swizzle.
-//   K-major operand:  rows of 64 fp16 (128 B); 8-row swizzle atoms of 1024 B stacked along M/N
-//                     (SBO = 1024 B); LBO unused.
-//   MN-major operand: rows of 64 fp16 along MN (128 B) indexed by k; 8 k-rows per atom (1024 B,
-//                     SBO between k-groups); LBO = byte distance between 64-wide MN chunks.
+// ---- wgmma (sm_90a warpgroup MMA) ----------------------------------------------------
+// Shared-memory matrix descriptor, 128-byte swizzle.
+//   K-major operand:  rows of 64 fp16 (128 B); 8-row swizzle atoms of 1024 B; SBO = byte distance between
+//                     consecutive 8-row groups along M/N; LBO unused.
+//   MN-major operand: rows of 64 fp16 along MN (128 B) indexed by k; 8 k-rows per atom (1024 B).
+// The swizzle is a function of the address bits, so atoms must be 1024-byte aligned.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t lbo_bytes,
                                                     uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;  // descriptor version (Blackwell)
-  d |= 2ull << 61;  // SWIZZLE_128B
+  d |= 1ull << 62;  // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16 with fp16 A/B, fp32 accumulate.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n, bool a_mn_major,
-                                                     bool b_mn_major) {
-  return (1u << 4)                                    // D format: F32
-         | (0u << 7)                                  // A format: F16
-         | (0u << 10)                                 // B format: F16
-         | ((a_mn_major ? 1u : 0u) << 15)             // A major
-         | ((b_mn_major ? 1u : 0u) << 16)             // B major
-         | (static_cast<uint32_t>(n >> 3) << 17)      // N / 8
-         | (static_cast<uint32_t>(m >> 4) << 24);     // M / 16
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Keeps the compiler from moving accumulator accesses across an in-flight wgmma.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+#define MHMR_WG_D8(o) "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), \
+                      "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+// D[64 x 64] (+)= A[smem] * B[smem]^T, fp16 operands, both K-major, fp32 accumulate.
+__device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : MHMR_WG_D8(0), MHMR_WG_D8(8), MHMR_WG_D8(16), MHMR_WG_D8(24)
+      : "l"(da), "l"(db), "r"(acc));
+}
+// D[64 x 128] (+)= A[smem] * B[smem]^T, fp16 operands, both K-major, fp32 accumulate.
+__device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : MHMR_WG_D8(0), MHMR_WG_D8(8), MHMR_WG_D8(16), MHMR_WG_D8(24), MHMR_WG_D8(32), MHMR_WG_D8(40),
+        MHMR_WG_D8(48), MHMR_WG_D8(56)
+      : "l"(da), "l"(db), "r"(acc));
+}
+// D[64 x 64] += A[registers, fp16 fragments] * B[smem], B MN-major (transposed); fp32 accumulate.
+__device__ __forceinline__ void wgmma_m64n64_rs_bt(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+      : MHMR_WG_D8(0), MHMR_WG_D8(8), MHMR_WG_D8(16), MHMR_WG_D8(24)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+#undef MHMR_WG_D8
+
+// Elementwise float2 arithmetic (two independent fp32 operations, round to nearest).
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 __device__ __forceinline__ float gelu_erf(float x) {
   return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
@@ -340,27 +302,26 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
   return 0.5f * x * (1.0f + copysignf(erf_abs, x));
 }
 
-// Two erf-GELUs at once on the packed f32x2 pipes (same Abramowitz-Stegun form as gelu_erf_fast): the
-// fc1 epilogue is issue-bound, and the packed form halves its floating-point instruction count.
+// Two erf-GELUs at once (same Abramowitz-Stegun form as gelu_erf_fast).
 __device__ __forceinline__ float2 gelu_erf_fast2(float2 x) {
   const float2 ax = make_float2(fabsf(x.x), fabsf(x.y));
-  const float2 z = __fmul2_rn(ax, make_float2(0.70710678118654752440f, 0.70710678118654752440f));
-  const float2 d = __ffma2_rn(z, make_float2(0.3275911f, 0.3275911f), make_float2(1.0f, 1.0f));
+  const float2 z = mul2(ax, make_float2(0.70710678118654752440f, 0.70710678118654752440f));
+  const float2 d = fma2(z, make_float2(0.3275911f, 0.3275911f), make_float2(1.0f, 1.0f));
   float2 t, e;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t.x) : "f"(d.x));
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t.y) : "f"(d.y));
-  const float2 a = __fmul2_rn(__fmul2_rn(z, z), make_float2(-1.4426950408889634f, -1.4426950408889634f));
+  const float2 a = mul2(mul2(z, z), make_float2(-1.4426950408889634f, -1.4426950408889634f));
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(a.x));
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(a.y));
-  float2 p = __ffma2_rn(make_float2(1.061405429f, 1.061405429f), t, make_float2(-1.453152027f, -1.453152027f));
-  p = __ffma2_rn(p, t, make_float2(1.421413741f, 1.421413741f));
-  p = __ffma2_rn(p, t, make_float2(-0.284496736f, -0.284496736f));
-  p = __ffma2_rn(p, t, make_float2(0.254829592f, 0.254829592f));
-  const float2 pte = __fmul2_rn(__fmul2_rn(p, t), e);
-  const float2 erf_abs = __ffma2_rn(pte, make_float2(-1.0f, -1.0f), make_float2(1.0f, 1.0f));
+  float2 p = fma2(make_float2(1.061405429f, 1.061405429f), t, make_float2(-1.453152027f, -1.453152027f));
+  p = fma2(p, t, make_float2(1.421413741f, 1.421413741f));
+  p = fma2(p, t, make_float2(-0.284496736f, -0.284496736f));
+  p = fma2(p, t, make_float2(0.254829592f, 0.254829592f));
+  const float2 pte = mul2(mul2(p, t), e);
+  const float2 erf_abs = fma2(pte, make_float2(-1.0f, -1.0f), make_float2(1.0f, 1.0f));
   const float2 s = make_float2(copysignf(erf_abs.x, x.x), copysignf(erf_abs.y, x.y));
-  const float2 hx = __fmul2_rn(x, make_float2(0.5f, 0.5f));
-  return __ffma2_rn(hx, s, hx);
+  const float2 hx = mul2(x, make_float2(0.5f, 0.5f));
+  return fma2(hx, s, hx);
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,4 +1,4 @@
-// Fused GEMM epilogue shared by the 1-CTA and the 2-CTA (cta_group::2) tcgen05 kernels.
+// Fused GEMM epilogue of the wgmma kernels (gemm_tc.cu).
 #pragma once
 #include "gemm_tc.cuh"
 
@@ -8,8 +8,8 @@ constexpr int kScratchStride = 36;               // floats per scratch row (32 +
 constexpr int kScratchBytes = 32 * kScratchStride * 4;
 
 
-// The accumulator chunk (32 rows x 32 columns, one row per thread after tcgen05.ld) is transposed through
-// a per-warp smem scratch so that global memory is accessed with lanes along the contiguous dimension:
+// The accumulator chunk (32 rows x 32 columns) is staged by the caller in a per-warp smem scratch (row r at
+// r * kScratchStride) and read back so that global memory is accessed with lanes along the contiguous dimension:
 //   fp32 outputs: 8 lanes x float4 cover one 128-byte row segment, 4 rows per warp instruction;
 //   fp16 outputs: 4 lanes x (8 halves) cover one 64-byte row segment, 8 rows per warp instruction.
 // Per-warp, per-tile state of the folded-LayerNorm epilogues (gemm_tc.cuh); empty work for the other kinds.
@@ -96,51 +96,12 @@ __device__ __forceinline__ void unpack_half8(const uint4& u, float (&f)[8]) {
   }
 }
 
-// Residual prefetch of the split-stream epilogue.  The epilogue of attn.proj is bound by the round trips of its residual
-// reads (ncu r02j: 42 % of the stall samples on the long scoreboard, 3 TB/s of traffic with ~32 KB in flight per SM):
-// each lane fetches the (hi, lo) values of the NEXT chunk it will process with cp.async into a per-warp 4 KB buffer
-// (slot (plane, k) at 512 B, lane at 16 B: a lane only ever reads back what it fetched itself), issued
-// right after the current chunk's values have been read out, one whole chunk (TMEM load, transpose, math, stores) ahead.
-constexpr int kPrefetchBytes = 2 * 4 * 32 * 16;   // per epilogue warp
-
 template <int EPI>
-__device__ __forceinline__ void epilogue_prefetch_resid(uint8_t* pre, const GemmEpi& ep, int M, int m_base, int n0,
-                                                        int lane) {
-  if constexpr (EPI == EPI_LS_RESID_SPLIT) {
-    const int cg = lane & 3, rs = lane >> 2;
-    const int n = n0 + cg * 8;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int m = m_base + k * 8 + rs;
-      if (m < M) {
-        const int64_t off = static_cast<int64_t>(m) * ep.ldx16 + n;
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(pre + (k * 32 + lane) * 16)),
-                     "l"(ep.x16 + off)
-                     : "memory");
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(pre + ((4 + k) * 32 + lane) * 16)),
-                     "l"(ep.xlo + off)
-                     : "memory");
-      }
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  }
-}
-
-template <int EPI>
-__device__ __forceinline__ void epilogue_chunk(const uint32_t (&r)[32], float* scratch, const GemmEpi& ep,
-                                               int M, int N, int m_base, int n0, int lane, EpiRowState& st,
-                                               uint8_t* pre = nullptr, int next_m_base = 0, int next_n0 = -1) {
+__device__ __forceinline__ void epilogue_chunk(const float* scratch, const GemmEpi& ep, int M, int N, int m_base,
+                                               int n0, int lane, EpiRowState& st) {
   constexpr bool kLn = epi_is_ln_consumer<EPI>();
   constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_RELU_F16 || kLn);
   constexpr bool kResid = (EPI == EPI_LS_RESID_F32);
-  // (a) rows -> scratch
-  float* my = scratch + lane * kScratchStride;
-#pragma unroll
-  for (int q = 0; q < 8; ++q)
-    *reinterpret_cast<float4*>(my + q * 4) =
-        make_float4(__uint_as_float(r[q * 4]), __uint_as_float(r[q * 4 + 1]), __uint_as_float(r[q * 4 + 2]),
-                    __uint_as_float(r[q * 4 + 3]));
-  __syncwarp();
   if constexpr (EPI == EPI_LS_RESID_SPLIT) {
     // residual stream as two fp16 planes: same lane mapping as the fp16 outputs (8 columns x 2 planes = 2 x 16 B)
     const int cg = lane & 3, rs = lane >> 2;
@@ -151,29 +112,14 @@ __device__ __forceinline__ void epilogue_chunk(const uint32_t (&r)[32], float* s
     *reinterpret_cast<float4*>(gg) = __ldg(reinterpret_cast<const float4*>(ep.gamma + n));
     *reinterpret_cast<float4*>(gg + 4) = __ldg(reinterpret_cast<const float4*>(ep.gamma + n + 4));
     uint4 hi[4], lo[4];
-    if (pre != nullptr) {
-      // this chunk's values were fetched one chunk ago; read them out, then let the next chunk's fetch fly
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const bool ok = (m_base + k * 8 + rs) < M;
-        hi[k] = ok ? *reinterpret_cast<const uint4*>(pre + (k * 32 + lane) * 16) : make_uint4(0u, 0u, 0u, 0u);
-        lo[k] = ok ? *reinterpret_cast<const uint4*>(pre + ((4 + k) * 32 + lane) * 16) : make_uint4(0u, 0u, 0u, 0u);
-      }
-      // the reads above are performed before the asynchronous refill of the same slots (same lane): a warp barrier
-      // orders them explicitly instead of relying on the in-order load/store unit
-      __syncwarp();
-      if (next_n0 >= 0) epilogue_prefetch_resid<EPI>(pre, ep, M, next_m_base, next_n0, lane);
-    } else {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int m = m_base + k * 8 + rs;
-        const int64_t off = static_cast<int64_t>(m) * ep.ldx16 + n;
-        hi[k] = lo[k] = make_uint4(0u, 0u, 0u, 0u);
-        if (m < M) {
-          hi[k] = *reinterpret_cast<const uint4*>(ep.x16 + off);
-          lo[k] = *reinterpret_cast<const uint4*>(ep.xlo + off);
-        }
+    for (int k = 0; k < 4; ++k) {
+      const int m = m_base + k * 8 + rs;
+      const int64_t off = static_cast<int64_t>(m) * ep.ldx16 + n;
+      hi[k] = lo[k] = make_uint4(0u, 0u, 0u, 0u);
+      if (m < M) {
+        hi[k] = *reinterpret_cast<const uint4*>(ep.x16 + off);
+        lo[k] = *reinterpret_cast<const uint4*>(ep.xlo + off);
       }
     }
 #pragma unroll
@@ -224,15 +170,15 @@ __device__ __forceinline__ void epilogue_chunk(const uint32_t (&r)[32], float* s
         // rstd * acc + b'  (the folded weight rows are centred: the mean term is already inside acc)
         const float rstd = __shfl_sync(0xffffffffu, st.rstd, rl);
         const float2 r2 = make_float2(rstd, rstd);
-        y[0] = __ffma2_rn(make_float2(v0.x, v0.y), r2, make_float2(b0.x, b0.y));
-        y[1] = __ffma2_rn(make_float2(v0.z, v0.w), r2, make_float2(b0.z, b0.w));
-        y[2] = __ffma2_rn(make_float2(v1.x, v1.y), r2, make_float2(b1.x, b1.y));
-        y[3] = __ffma2_rn(make_float2(v1.z, v1.w), r2, make_float2(b1.z, b1.w));
+        y[0] = fma2(make_float2(v0.x, v0.y), r2, make_float2(b0.x, b0.y));
+        y[1] = fma2(make_float2(v0.z, v0.w), r2, make_float2(b0.z, b0.w));
+        y[2] = fma2(make_float2(v1.x, v1.y), r2, make_float2(b1.x, b1.y));
+        y[3] = fma2(make_float2(v1.z, v1.w), r2, make_float2(b1.z, b1.w));
       } else {
-        y[0] = __fadd2_rn(make_float2(v0.x, v0.y), make_float2(b0.x, b0.y));
-        y[1] = __fadd2_rn(make_float2(v0.z, v0.w), make_float2(b0.z, b0.w));
-        y[2] = __fadd2_rn(make_float2(v1.x, v1.y), make_float2(b1.x, b1.y));
-        y[3] = __fadd2_rn(make_float2(v1.z, v1.w), make_float2(b1.z, b1.w));
+        y[0] = add2(make_float2(v0.x, v0.y), make_float2(b0.x, b0.y));
+        y[1] = add2(make_float2(v0.z, v0.w), make_float2(b0.z, b0.w));
+        y[2] = add2(make_float2(v1.x, v1.y), make_float2(b1.x, b1.y));
+        y[3] = add2(make_float2(v1.z, v1.w), make_float2(b1.z, b1.w));
       }
 #pragma unroll
       for (int i = 0; i < 4; ++i) {

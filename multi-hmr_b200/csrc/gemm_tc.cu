@@ -1,13 +1,17 @@
-// tcgen05 + TMA + TMEM persistent GEMM (see gemm_tc.cuh for the contract).
+// wgmma + TMA persistent GEMM (see gemm_tc.cuh for the contract).
 //
-// CTA = 384 threads, one CTA per SM, persistent over output tiles (128 x BN):
-//   warp 0    : TMA producer   (one elected lane)   global -> 128B-swizzled smem ring
-//   warp 1    : MMA issuer     (one elected lane)   tcgen05.mma kind::f16, M=128, N=BN, K=16
-//   warp 2    : TMEM allocator (2 x BN fp32 columns: double-buffered accumulator)
-//   warps 4-11: epilogue       tcgen05.ld 32x32b -> registers -> smem transpose -> fused epilogue with
-//                              coalesced 128-bit global accesses (two warps per TMEM sub-partition)
-// Pipelines: smem full/empty ring (TMA <-> MMA) and TMEM full/empty pair (MMA <-> epilogue), so the
-// epilogue of tile i overlaps the main loop of tile i+1.
+// CTA = 384 threads = 3 warpgroups, one CTA per SM, persistent over output tiles (128 x BN):
+//   warpgroup 0   : TMA producer (warp 0, one elected lane)   global -> 128B-swizzled smem ring
+//   warpgroups 1-2: consumers; warpgroup 1 + c computes columns [c BN/2, (c+1) BN/2) of the tile with
+//                   wgmma m64 x (BN/2) x k16 (fp32 accumulators in registers), then runs the fused epilogue
+//                   (gemm_epilogue.cuh) on them.
+// Each consumer issues its 128 rows as two m64 wgmmas whose A descriptors interleave the 8-row swizzle atoms
+// (start +0 / +1024 B, stride 2048 B): warp w of the warpgroup then holds the 32 CONSECUTIVE rows 32w..32w+31,
+// the row block the epilogue works on.
+//
+// block_n 512: a cluster of two CTAs computes a 256 x 256 tile.  Each CTA stages its own 128 rows of A and
+// loads half of the 256-row weight tile, multicast into both CTAs, so the weight traffic from L2 per CTA
+// halves.  A smem stage is refilled only once the consumers of BOTH CTAs have released it.
 #include "gemm_tc.cuh"
 #include "gemm_epilogue.cuh"
 
@@ -17,9 +21,11 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 fp16 = 128 B = one swizzle row
-constexpr int UMMA_K = 16;
-constexpr int kEpiWarps = 8;
-constexpr int kThreads = 128 + 32 * kEpiWarps;  // TMA, MMA, TMEM-alloc, spare + epilogue warps
+constexpr int kConsumers = 2;
+constexpr int kThreads = 128 * (1 + kConsumers);
+constexpr int kEpiWarps = 4 * kConsumers;
+constexpr int kRegsProducer = 40, kRegsConsumer = 232;
+
 template <int BN>
 struct GemmCfg {
   static constexpr int kStages = (BN == 256) ? 3 : 5;
@@ -29,15 +35,22 @@ struct GemmCfg {
   static constexpr int kBarBytes = 256;
   static constexpr int kSmemBytes =
       kStages * kStageBytes + kEpiWarps * kScratchBytes + kBarBytes + 1024;  // +1024: manual align
-  static constexpr int kTmemCols = 2 * BN;                                  // 256 or 512
+  static constexpr int kAcc = BN / 4;  // fp32 accumulators per thread and m64 wgmma (n = BN / 2)
 };
 
-template <int BN, int EPI>
+template <int NACC>
+__device__ __forceinline__ void wgmma_ss(float (&d)[NACC], uint64_t da, uint64_t db, uint32_t acc) {
+  if constexpr (NACC == 64) wgmma_m64n128_ss(d, da, db, acc);
+  else wgmma_m64n64_ss(d, da, db, acc);
+}
+
+template <int BN, int CL, int EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                int M, int N, int K, GemmEpi ep) {
   using Cfg = GemmCfg<BN>;
   constexpr int kStages = Cfg::kStages;
+  constexpr int kAcc = Cfg::kAcc;
 
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment (128B swizzle atoms) by POINTER arithmetic, so that the compiler keeps the
@@ -45,144 +58,151 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   float* scratch_base = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes + kEpiWarps * kScratchBytes);
-  uint64_t* full_bar = bars;                  // [kStages]  TMA -> MMA
-  uint64_t* empty_bar = bars + kStages;       // [kStages]  MMA -> TMA
-  uint64_t* tfull_bar = bars + 2 * kStages;   // [2]        MMA -> epilogue
-  uint64_t* tempty_bar = tfull_bar + 2;       // [2]        epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint64_t* full_bar = bars;             // [kStages]  TMA -> consumers
+  uint64_t* empty_bar = bars + kStages;  // [kStages]  consumers (of every CTA of the cluster) -> TMA
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const uint32_t rank = (CL > 1) ? cluster_ctarank() : 0u;
 
-  const int num_m = (M + BM - 1) / BM;
+  const int num_m = (M + BM * CL - 1) / (BM * CL);
   const int num_n = (N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
   const int num_kb = (K + BK - 1) / BK;
+  const int first_tile = blockIdx.x / CL, tile_stride = gridDim.x / CL;
 
   griddep_launch_dependents();
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], kEpiWarps);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[s], kConsumers * CL);  // one arrive per consumer warpgroup of every CTA
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if constexpr (CL > 1) cluster_sync_all();  // the peer's barriers exist before any multicast or remote arrive
+  else __syncthreads();
   griddep_wait();  // the previous kernel's outputs (A rows, residual, statistics) are complete and visible
 
-  if (warp == 0) {
-    // ------------------------------ TMA producer ------------------------------
-    // (whole warp on the warp-uniform loop, one elected lane issues -- see elect_one_sync)
-    uint32_t stage = 0, phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile / num_n, n_blk = tile % num_n;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1u);
-        uint8_t* sa = smem + stage * Cfg::kStageBytes;
-        uint8_t* sb = sa + Cfg::kABytes;
-        if (elect_one_sync()) {
-          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
-          tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
-        }
-        __syncwarp();
-        if (++stage == kStages) { stage = 0; phase ^= 1u; }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer --------------------------------
-    constexpr uint32_t idesc = make_idesc_f16(BM, BN, false, false);
-    uint32_t stage = 0, phase = 0, acc_iter = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++acc_iter) {
-      const uint32_t as = acc_iter & 1u;
-      const uint32_t aphase = (acc_iter >> 1) & 1u;
-      mbar_wait(&tempty_bar[as], aphase ^ 1u);  // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint32_t sb = sa + Cfg::kABytes;
-        const uint64_t a_desc = make_sw128_desc(sa, 16, 1024);
-        const uint64_t b_desc = make_sw128_desc(sb, 16, 1024);
-        if (elect_one_sync()) {
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            // advance K by 16 fp16 = 32 B inside the 128-B swizzle row: +2 in (addr >> 4) units
-            umma_f16_ss(d_tmem, a_desc + 2u * k, b_desc + 2u * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsProducer));
+    if (warp == 0) {
+      // ------------------------------ TMA producer ------------------------------
+      uint32_t stage = 0, phase = 0;
+      for (int tile = first_tile; tile < num_tiles; tile += tile_stride) {
+        const int m_blk = tile / num_n, n_blk = tile % num_n;
+        const int row0 = m_blk * BM * CL + static_cast<int>(rank) * BM;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          uint8_t* sa = smem + stage * Cfg::kStageBytes;
+          uint8_t* sb = sa + Cfg::kABytes;
+          if (elect_one_sync()) {
+            mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+            tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, row0);
+            if constexpr (CL > 1) {
+              constexpr int kHalf = BN / CL;
+              tma_load_2d_multicast(sb + rank * (kHalf * BK * 2), &tmB, &full_bar[stage], kb * BK,
+                                    n_blk * BN + static_cast<int>(rank) * kHalf, static_cast<uint16_t>((1u << CL) - 1u));
+            } else {
+              tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
+            }
           }
-          umma_commit(&empty_bar[stage]);                       // smem slot free once MMAs retire
-          if (kb == num_kb - 1) umma_commit(&tfull_bar[as]);    // accumulator complete
+          __syncwarp();
+          if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
-        __syncwarp();
-        if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp >= 4) {
-    // ------------------------------ Epilogue -----------------------------------
-    const int ew = warp & 3;             // TMEM sub-partition of this warp: lanes [32*ew, 32*ew+32)
-    const int par = (warp - 4) >> 2;     // two warps per sub-partition split the column chunks
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsConsumer));
+    // ------------------------------ consumers -----------------------------------
+    const int cw = wg - 1;          // column half of the tile
+    const int w = warp & 3;         // rows 32w..32w+31 of the tile
+    const bool release_lane = (threadIdx.x & 127) == 0;
     float* scratch = scratch_base + (warp - 4) * (kScratchBytes / 4);
-    uint32_t acc_iter = 0;
+    auto release = [&](uint32_t s) {
+      if (release_lane) {
+        if constexpr (CL > 1) {
+#pragma unroll
+          for (int c = 0; c < CL; ++c) mbar_arrive_cluster(&empty_bar[s], static_cast<uint32_t>(c));
+        } else {
+          mbar_arrive(&empty_bar[s]);
+        }
+      }
+    };
+    uint32_t stage = 0, phase = 0;
     EpiStatsPrefetch pf;
-    if (static_cast<int>(blockIdx.x) < num_tiles)
-      epilogue_load_row_stats<EPI>(pf, ep, M, (static_cast<int>(blockIdx.x) / num_n) * BM + ew * 32, lane);
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++acc_iter) {
-      const int m_blk = tile / num_n, n_blk = tile % num_n;
-      const uint32_t as = acc_iter & 1u;
-      const uint32_t aphase = (acc_iter >> 1) & 1u;
-      const int m_base = m_blk * BM + ew * 32;
+    auto tile_m_base = [&](int tile) { return (tile / num_n) * BM * CL + static_cast<int>(rank) * BM + 32 * w; };
+    if (first_tile < num_tiles) epilogue_load_row_stats<EPI>(pf, ep, M, tile_m_base(first_tile), lane);
+    for (int tile = first_tile; tile < num_tiles; tile += tile_stride) {
+      const int n_blk = tile % num_n;
+      const int m_base = tile_m_base(tile);
       EpiRowState rowst;
       epilogue_tile_begin<EPI>(rowst, pf, ep, K);
-      if (tile + static_cast<int>(gridDim.x) < num_tiles)  // next tile's row statistics: under this tile's epilogue
-        epilogue_load_row_stats<EPI>(pf, ep, M, ((tile + static_cast<int>(gridDim.x)) / num_n) * BM + ew * 32, lane);
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * BN;
-      constexpr int kChunksPerWarp = BN / 32 / (kEpiWarps / 4);
-#pragma unroll 1
-      for (int ci = 0; ci < kChunksPerWarp; ++ci) {
-        const int c = ci * (kEpiWarps / 4) + par;
-        uint32_t r[32];
-        tmem_ld_32x32(t_row + c * 32, r);
-        tmem_ld_wait();
-        if (ci == kChunksPerWarp - 1) {  // accumulator fully read by this warp: hand it back early
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[as]);
+      if (tile + tile_stride < num_tiles)  // next tile's row statistics: under this tile's main loop
+        epilogue_load_row_stats<EPI>(pf, ep, M, tile_m_base(tile + tile_stride), lane);
+
+      float acc[2][kAcc];
+      uint32_t prev_stage = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
+        const uint32_t sb = sa + Cfg::kABytes + cw * (BN / 2) * (BK * 2);
+        const uint64_t a_desc0 = make_sw128_desc(sa, 16, 2048);
+        const uint64_t a_desc1 = make_sw128_desc(sa + 1024, 16, 2048);
+        const uint64_t b_desc = make_sw128_desc(sb, 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          // advance K by 16 fp16 = 32 B inside the 128-B swizzle row: +2 in (addr >> 4) units
+          const uint32_t accumulate = (kb > 0 || k > 0) ? 1u : 0u;
+          wgmma_ss<kAcc>(acc[0], a_desc0 + 2u * k, b_desc + 2u * k, accumulate);
+          wgmma_ss<kAcc>(acc[1], a_desc1 + 2u * k, b_desc + 2u * k, accumulate);
         }
-        const int n0 = n_blk * BN + c * 32;
-        if (n0 < N) epilogue_chunk<EPI>(r, scratch, ep, M, N, m_base, n0, lane, rowst);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k block's wgmmas are complete: its stage can be refilled
+        if (kb > 0) release(prev_stage);
+        prev_stage = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
-      epilogue_tile_end<EPI>(rowst, ep, M, m_base, n_blk * (kEpiWarps / 4) + par, lane);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
+      release(prev_stage);
+
+      // ------------------------------ epilogue ----------------------------------
+      // accumulator fragment of wgmma h: register i holds row 8h + 16((i >> 1) & 1) + lane / 4 of this warp's
+      // block, column 8 (i >> 2) + 2 (lane & 3) + (i & 1) of the warpgroup's half
+#pragma unroll
+      for (int c = 0; c < BN / 64; ++c) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int g = 0; g < 4; ++g)
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+              const int i = 4 * (4 * c + g) + 2 * rr;
+              const int r = (lane >> 2) + 8 * h + 16 * rr;
+              *reinterpret_cast<float2*>(scratch + r * kScratchStride + g * 8 + 2 * (lane & 3)) =
+                  make_float2(acc[h][i], acc[h][i + 1]);
+            }
+        __syncwarp();
+        const int n0 = n_blk * BN + cw * (BN / 2) + c * 32;
+        if (n0 < N) epilogue_chunk<EPI>(scratch, ep, M, N, m_base, n0, lane, rowst);
+        __syncwarp();
+      }
+      epilogue_tile_end<EPI>(rowst, ep, M, m_base, n_blk * kConsumers + cw, lane);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-  }
+  // no CTA of a cluster leaves while its peer may still arrive on its barriers
+  if constexpr (CL > 1) cluster_sync_all();
 }
 
-template <int BN, int EPI>
+template <int BN, int CL, int EPI>
 int launch_one(const GemmPlan* p, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_tc_kernel<BN, EPI>;
+  auto kern = gemm_tc_kernel<BN, CL, EPI>;
   static PerDeviceOnce once;
   if (once.first()) {
     MHMR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -193,27 +213,38 @@ int launch_one(const GemmPlan* p, cudaStream_t stream) {
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  if (CL > 1) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = CL;
+    attr[n].val.clusterDim.y = 1;
+    attr[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  if (pdl_enabled()) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = n;
   MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, p->tmA, p->tmB, p->M, p->N, p->K, p->ep));
   return MHMR_OK;
 }
 
-template <int BN>
+template <int BN, int CL>
 int launch_bn(const GemmPlan* p, cudaStream_t stream) {
   switch (p->epi) {
-    case EPI_BIAS_F16: return launch_one<BN, EPI_BIAS_F16>(p, stream);
-    case EPI_BIAS_GELU_F16: return launch_one<BN, EPI_BIAS_GELU_F16>(p, stream);
-    case EPI_BIAS_RELU_F16: return launch_one<BN, EPI_BIAS_RELU_F16>(p, stream);
-    case EPI_LS_RESID_F32: return launch_one<BN, EPI_LS_RESID_F32>(p, stream);
-    case EPI_ROWADD_F32: return launch_one<BN, EPI_ROWADD_F32>(p, stream);
-    case EPI_BIAS_F32: return launch_one<BN, EPI_BIAS_F32>(p, stream);
-    case EPI_LS_RESID_SPLIT: return launch_one<BN, EPI_LS_RESID_SPLIT>(p, stream);
-    case EPI_LN_BIAS_F16: return launch_one<BN, EPI_LN_BIAS_F16>(p, stream);
-    case EPI_LN_GELU_F16: return launch_one<BN, EPI_LN_GELU_F16>(p, stream);
+    case EPI_BIAS_F16: return launch_one<BN, CL, EPI_BIAS_F16>(p, stream);
+    case EPI_BIAS_GELU_F16: return launch_one<BN, CL, EPI_BIAS_GELU_F16>(p, stream);
+    case EPI_BIAS_RELU_F16: return launch_one<BN, CL, EPI_BIAS_RELU_F16>(p, stream);
+    case EPI_LS_RESID_F32: return launch_one<BN, CL, EPI_LS_RESID_F32>(p, stream);
+    case EPI_ROWADD_F32: return launch_one<BN, CL, EPI_ROWADD_F32>(p, stream);
+    case EPI_BIAS_F32: return launch_one<BN, CL, EPI_BIAS_F32>(p, stream);
+    case EPI_LS_RESID_SPLIT: return launch_one<BN, CL, EPI_LS_RESID_SPLIT>(p, stream);
+    case EPI_LN_BIAS_F16: return launch_one<BN, CL, EPI_LN_BIAS_F16>(p, stream);
+    case EPI_LN_GELU_F16: return launch_one<BN, CL, EPI_LN_GELU_F16>(p, stream);
     default: break;
   }
   set_last_error("gemm: unknown epilogue kind");
@@ -249,7 +280,7 @@ int gemm_plan_init(GemmPlan* plan, const __half* A, int64_t lda, const __half* W
   plan->M = M; plan->N = N; plan->K = K; plan->bn = bn; plan->epi = epi_kind; plan->ep = ep;
   int rc = make_tmap_2d(&plan->tmA, A, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, M, K, lda * 2, BM, BK, true);
   if (rc != MHMR_OK) return rc;
-  // CTA pair: every CTA stages half (128 rows) of the 256-row weight tile
+  // CTA pair: every CTA loads half (128 rows) of the 256-row weight tile
   rc = make_tmap_2d(&plan->tmB, W, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, N, K, ldw * 2, bn == 512 ? 128 : bn, BK,
                     true);
   if (rc != MHMR_OK) return rc;
@@ -270,12 +301,12 @@ int gemm_plan_grid(const GemmPlan* plan, int M) {
 
 int gemm_stat_slots(int N, int bn) {
   const int tile_n = (bn == 128) ? 128 : 256;  // bn 512 = CTA pair with 256-column tiles
-  return ((N + tile_n - 1) / tile_n) * (kEpiWarps / 4);
+  return ((N + tile_n - 1) / tile_n) * kConsumers;
 }
 
 int gemm_plan_run(const GemmPlan* plan, cudaStream_t stream) {
-  if (plan->bn == 512) return gemm_plan_run_2cta(plan, stream);
-  return plan->bn == 256 ? launch_bn<256>(plan, stream) : launch_bn<128>(plan, stream);
+  if (plan->bn == 512) return launch_bn<256, 2>(plan, stream);
+  return plan->bn == 256 ? launch_bn<256, 1>(plan, stream) : launch_bn<128, 1>(plan, stream);
 }
 
 }  // namespace mhmr

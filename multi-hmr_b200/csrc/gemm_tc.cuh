@@ -1,8 +1,8 @@
-// tcgen05 / TMA / TMEM GEMM family for the Multi-HMR hot path (sm_100a only).
+// wgmma / TMA GEMM family for the Multi-HMR hot path (sm_90a).
 //
 //   C[M,N] = epilogue( A[M,K] (fp16, K-major) x W[N,K]^T (fp16, K-major, i.e. torch Linear.weight) )
 //
-// fp32 accumulation in TMEM.  The epilogues cover every Linear of the reference's ViT backbone and
+// fp32 accumulation in registers.  The epilogues cover every Linear of the reference's ViT backbone and
 // of the dense part of the head (SURVEY.md §2.4 k1,k3,k5,k6,k7,k9,k15):
 //   EPI_BIAS_F16       out16 = acc + bias                       (qkv: dinov2 Attention.qkv)
 //   EPI_BIAS_GELU_F16  out16 = gelu_erf(acc + bias)             (mlp.fc1 + nn.GELU)
@@ -62,7 +62,7 @@ struct GemmEpi {
 struct GemmPlan {
   CUtensorMap tmA, tmB;
   int M = 0, N = 0, K = 0;
-  int bn = 256;          // 128 / 256: single-CTA tile width; 512: CTA pair (cta_group::2), 256 x 256 tile
+  int bn = 256;          // 128 / 256: single-CTA tile width; 512: CTA pair (2-CTA cluster), 256 x 256 tile
   int epi = EPI_BIAS_F16;
   GemmEpi ep;
   int grid = 0;
@@ -72,7 +72,6 @@ struct GemmPlan {
 int gemm_plan_init(GemmPlan* plan, const __half* A, int64_t lda, const __half* W, int64_t ldw, int M,
                    int N, int K, int epi_kind, const GemmEpi& ep, int bn);
 int gemm_plan_run(const GemmPlan* plan, cudaStream_t stream);
-int gemm_plan_run_2cta(const GemmPlan* plan, cudaStream_t stream);  // gemm_tc2.cu
 // launch geometry for `M` rows with this plan's tile shape
 int gemm_plan_grid(const GemmPlan* plan, int M);
 // partial-statistics slots per row that an EPI_LS_RESID_SPLIT GEMM with N columns and tile selector `bn` writes

@@ -1,4 +1,4 @@
-// Host-side utilities shared by all translation units of libmhmr_sm100.so.
+// Host-side utilities shared by all translation units of libmhmr_sm90.so.
 #include <cstdlib>
 #include "common.cuh"
 
@@ -77,10 +77,10 @@ bool PerDeviceOnce::first() {
 int device_sm_count() {
   static int sms[64] = {};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (sms[dev] == 0) {
     if (cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms[dev] <= 0)
-      sms[dev] = 148;
+      sms[dev] = 132;
   }
   return sms[dev];
 }

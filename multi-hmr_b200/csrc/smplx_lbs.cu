@@ -8,7 +8,7 @@
 //     coefficient vector cf[p] = [pose_feature(486) | betas | expression].
 //   * J_regressor is folded at load time: J(beta) = Jt + Jdirs . beta  (J is linear in beta), which removes
 //     a 2.3 MB read and a cross-CTA reduction.
-//   * one CTA per SM (72 vertices = 216 columns per CTA for V = 10475 on 148 SMs); the CTA's column slab
+//   * one CTA per SM (80 vertices = 240 columns per CTA for V = 10475 on the 132 SMs of an H100); the CTA's column slab
 //     is streamed through a TMA-fed shared-memory ring and 16 persons are accumulated per streamed row
 //     (the matrix is read from HBM once; further blocks of 16 persons re-stream it from L2).
 #include "kernels.cuh"

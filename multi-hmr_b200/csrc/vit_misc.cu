@@ -255,7 +255,7 @@ int normalize_u8(const uint8_t* img, const float* lut, float* out, int B, int H,
   MHMR_REQUIRE((reinterpret_cast<uintptr_t>(img) & 3u) == 0 && (reinterpret_cast<uintptr_t>(out) & 15u) == 0,
                "normalize_u8: image must be 4-byte aligned, output 16-byte aligned");
   const int64_t n_quads = static_cast<int64_t>(B) * H * (W / 4);
-  const int blocks = static_cast<int>(std::min<int64_t>((n_quads + 255) / 256, 148 * 8));
+  const int blocks = static_cast<int>(std::min<int64_t>((n_quads + 255) / 256, device_sm_count() * 8));
   normalize_u8_kernel<<<blocks, 256, 0, stream>>>(img, lut, out, H, W, n_quads);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
@@ -313,7 +313,7 @@ int split_rowstats(const float* X, __half* xhi, __half* xlo, int64_t ld16, float
 }
 
 int merge_split(const __half* xhi, const __half* xlo, float* X, int64_t n, cudaStream_t stream) {
-  merge_split_kernel<<<static_cast<int>(std::min<int64_t>((n + 255) / 256, 148 * 16)), 256, 0, stream>>>(xhi, xlo, X, n);
+  merge_split_kernel<<<static_cast<int>(std::min<int64_t>((n + 255) / 256, device_sm_count() * 16)), 256, 0, stream>>>(xhi, xlo, X, n);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }
@@ -329,7 +329,7 @@ int f32_to_f16_2d(const float* src, int64_t lds, __half* dst, int64_t ldd, int r
                   cudaStream_t stream) {
   const int64_t total = static_cast<int64_t>(rows) * cols;
   int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   if (blocks < 1) blocks = 1;
   f32_to_f16_2d_kernel<<<blocks, 256, 0, stream>>>(src, lds, dst, ldd, rows, cols);
   MHMR_CUDA_CHECK(cudaGetLastError());

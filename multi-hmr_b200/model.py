@@ -1,9 +1,9 @@
-"""Host-side mirror of the reference's `Model` (reference model.py:30-349) over libmhmr_sm100.so.
+"""Host-side mirror of the reference's `Model` (reference model.py:30-349) over libmhmr_sm90.so.
 
 Same constructor keywords, same `forward(x, idx, det_thresh, nms_kernel_size, K, is_training)` signature,
 same return conventions (list of per-person dicts in inference, flat dict when `is_training=True`), same
 `load_state_dict(sd, strict=False)` key names — but every tensor operation of the forward runs in the
-hand-written sm_100a kernels behind the C-ABI (`mhmr_forward`).  PyTorch is used for device memory,
+hand-written sm_90a kernels behind the C-ABI (`mhmr_forward`).  PyTorch is used for device memory,
 streams and (once, at load) the bicubic pos-embed interpolation.  There is no CPU fallback: a CUDA device
 and the built extension are required, otherwise construction / forward raise.
 """
@@ -74,7 +74,7 @@ def interpolate_pos_embed(pos_embed: torch.Tensor, grid: int) -> torch.Tensor:
 
 
 class Model:
-    """B200-native drop-in for reference `model.Model` (inference path)."""
+    """H100-native drop-in for reference `model.Model` (inference path)."""
 
     def __init__(self, backbone="dinov2_vitb14", pretrained_backbone=False, img_size=896,
                  camera_embedding="geometric", camera_embedding_num_bands=16,
@@ -95,7 +95,7 @@ class Model:
             raise NotImplementedError(f"person_center {person_center!r}: only the 55 kinematic SMPL-X joints are "
                                       "supported as person centre (vertex-picked joints / landmarks are not)")
         if not torch.cuda.is_available():
-            raise RuntimeError("multihmr_b200.Model needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("multihmr_b200.Model needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device(device if device is not None else "cuda:0")
         self.backbone_name = backbone
         self.img_size = img_size

@@ -1,4 +1,4 @@
-"""Stage-level operators of libmhmr_sm100.so as torch-tensor functions (unit parity + ncu targets).
+"""Stage-level operators of libmhmr_sm90.so as torch-tensor functions (unit parity + ncu targets).
 
 Each function borrows the tensors' device pointers for the duration of the call and launches on the
 current torch CUDA stream.  There is no CPU path: tensors must live on a CUDA device.

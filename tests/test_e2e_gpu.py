@@ -1,4 +1,4 @@
-"""GPU parity proper: the engine (sm_100a kernels behind the C-ABI) vs the golden fixtures = outputs of
+"""GPU parity proper: the engine (sm_90a kernels behind the C-ABI) vs the golden fixtures = outputs of
 the unmodified reference `Model.forward` on identical seeded inputs.  Tolerance: 1e-3 abs on detection
 scores, SMPL-X parameters and 3-D vertices (BASELINE.json north_star); see parity_util.TOL."""
 import pytest

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM family vs plain torch fp32 on the same fp16-rounded operands (floating-point kernel:
+"""wgmma GEMM family vs plain torch fp32 on the same fp16-rounded operands (floating-point kernel:
 torch fp32 reference, see task ③).  Tolerances are stated per test."""
 import pytest
 import torch
