@@ -94,7 +94,17 @@ typedef struct mhmr_config {
   int person_center_idx; /* index of Model(person_center=...) in smplx JOINT_NAMES ('head' = 15) */
   int num_verts;         /* body-model vertices (SMPL-X: 10475) */
   int refine_central;    /* 1: fp32 refinement of the detected tokens' residual streams (DESIGN.md §3); 0: bulk fp16 pass only */
+  /* Appended fields; all zero = the SMPL-X head above.  With head == MHMR_HEAD_ANNY, xat_depth / xat_num_heads are
+   * the Anny HPH's (multi_hmr_anny/multi_hmr.py:28-33, dim_head 32), person_center_idx is the index of the centre
+   * bone in the body model's bone_labels, num_betas is the shape-head width (11), and num_verts is unused. */
+  int head;              /* MHMR_HEAD_SMPLX (0) or MHMR_HEAD_ANNY (1) */
+  int xat_dim;           /* Anny: HPH width (512), multiple of 32 */
+  int xat_mlp_dim;       /* Anny: HPH FeedForward hidden width (2048), multiple of 32 */
+  int num_joints;        /* Anny: body-model bones / rotations per person (163) */
 } mhmr_config;
+
+#define MHMR_HEAD_SMPLX 0
+#define MHMR_HEAD_ANNY 1
 
 /* Per-call outputs: device buffers owned by the caller (torch tensors), sized for max_persons.
  * Person order = torch.where order (b, y, x) (model.py:149,616).  Nullable: v2d, z. */
@@ -155,6 +165,48 @@ int mhmr_forward_u8(mhmr_engine* h, const uint8_t* img_u8, const float* lut, con
 /* Waits for the forward enqueued last on `stream` and returns the person count; MHMR_ERR_CAPACITY if it
  * exceeded max_persons (outputs are then incomplete — never silently truncated). */
 int mhmr_sync_count(mhmr_engine* h, void* stream, int* num_persons);
+
+/* ------------------------------------------------------------------------------------------------
+ * Anny variant: `Multi_HMR.forward` of multi_hmr_anny/multi_hmr.py:98-246 on an engine created with
+ * head == MHMR_HEAD_ANNY.  The body model (the `anny` package) is NOT part of the library: mhmr_forward_anny computes
+ * everything up to its inputs (rotmat_homo, shape), the caller runs the body model, and mhmr_anny_place finishes
+ * (centre bone, translation, projection).  Weights are set under the checkpoint's own keys (encoder.backbone.*,
+ * encoder.mlp_det.*, encoder.mlp_fov_unique.*, dec_to_token.*, decoder.transformer.layers.*, mlp_{offset,pose,
+ * shape,dist}.*, useful_rotmat, init_body_pose, dec_pos_emb); encoder.backbone.pos_embed interpolated as above.
+ * Person order = (b, y, x); the depth sort of the reference is left to the caller.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct mhmr_anny_outputs {
+  float* scores_map;   /* [B, res, res]   sigmoid of the detection logits, NMS applied in inference mode       */
+  float* logits;       /* [B, res, res]   'scores_logits' (before NMS)                                          */
+  int32_t* count;      /* [1]             number of persons P                                                   */
+  int32_t* det_idx;    /* [3, max_persons] b, y, x                                                              */
+  float* K_regressed;  /* [B, 3, 3]       intrinsics from the regressed field of view (encoder.py:50-56)        */
+  float* fov;          /* [B]             regressed field of view, radians                                      */
+  float* K_det;        /* [max_persons, 3, 3] intrinsics used for each person (K, or K_regressed when K is NULL) */
+  float* offset;       /* [max_persons, 2]                                                                      */
+  float* loc;          /* [max_persons, 2]                                                                      */
+  float* dist;         /* [max_persons]   focal / clamp(exp(dist_pp), 1e-5)                                     */
+  float* dist_pp;      /* [max_persons]   raw mlp_dist output ('dist_postprocessed')                            */
+  float* shape;        /* [max_persons, num_betas] sigmoid(mlp_shape)                                           */
+  float* rotmat;       /* [max_persons, J, 3, 3]  after the useful_rotmat blend                                 */
+  float* rotmat_homo;  /* [max_persons, J, 4, 4]  homogeneous form (the body model's pose_parameters)           */
+  float* rotvec;       /* [max_persons, J, 3]                                                                   */
+  float* transl;       /* [max_persons, 3]  K^-1 [loc, 1] dist                                                  */
+  float* z;            /* [B, N, D] backbone features, nullable                                                 */
+} mhmr_anny_outputs;
+
+/* x [B,3,S,S] fp32 (mhmr_forward_anny) or img_u8 [B,S,S,3] + table (mhmr_forward_anny_u8); K [B,3,3] or NULL (the
+ * regressed intrinsics are used); forced_idx as in mhmr_forward.  nms_kernel_size must be odd.  Asynchronous. */
+int mhmr_forward_anny(mhmr_engine* h, const float* x, const float* K, int B, float det_thresh, int nms_kernel_size,
+                      const int64_t* forced_idx, int forced_P, const mhmr_anny_outputs* out, void* stream);
+int mhmr_forward_anny_u8(mhmr_engine* h, const uint8_t* img_u8, const float* lut, const float* K, int B,
+                         float det_thresh, int nms_kernel_size, const int64_t* forced_idx, int forced_P,
+                         const mhmr_anny_outputs* out, void* stream);
+/* After the body model, for P persons (device pointers): v3d [P,V,3] (vertices in, camera-space vertices out, in
+ * place), j3d [P,J,3] out from bone_poses [P,J,4,4] (translation column), both shifted by -bone(center) + transl;
+ * j2d [P,J,2] and (nullable) v2d [P,V,2] projected with K_det; transl_pelvis [P,3] = j3d[:, 0]. */
+int mhmr_anny_place(mhmr_engine* h, int P, int V, const float* bone_poses, const float* transl, const float* K_det,
+                    float* v3d, float* j3d, float* v2d, float* j2d, float* transl_pelvis, void* stream);
 
 /* Stage-level entry: backbone only (blocks/dinov2.py:16-26): x [B,3,S,S] -> z [B,N,D] fp32. */
 int mhmr_vit_forward(mhmr_engine* h, const float* x, int B, float* z, void* stream);

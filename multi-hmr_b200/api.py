@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from .model import Model
+from .model_anny import ModelAnny
 
 from .preprocess import IMG_NORM_MEAN, IMG_NORM_STD, device_table, normalize_rgb, normalize_rgb_table  # noqa: F401
 
@@ -96,15 +97,20 @@ def body_model_from_smplx_npz(path: str, num_betas: int = 10) -> dict:
     }
 
 
-def load_model(model_name, device=torch.device("cuda"), max_batch=8, max_persons=None):
+def load_model(model_name, device=torch.device("cuda"), max_batch=8, max_persons=None, body_model=None):
     """Open a checkpoint, build the engine from its saved arguments, load the weights (demo.py:70-106).
-    No download is attempted (this build has no network): a missing file is an error."""
+    No download is attempted (this build has no network): a missing file is an error.  A checkpoint whose name
+    contains 'anny' builds the Anny variant (demo.py:95-96) with `body_model`, or with the `anny` package's
+    full-body model when none is given."""
     ckpt_path = os.path.join(CACHE_DIR_MULTIHMR, model_name + ".pt")
     if not os.path.isfile(ckpt_path):
         raise FileNotFoundError(f"{ckpt_path} not found (place the reference checkpoint there)")
-    if "anny" in ckpt_path:
-        raise NotImplementedError("the Anny variant (multi_hmr_anny/) is outside this build (SURVEY.md §8f)")
     ckpt = torch.load(ckpt_path, map_location="cpu", weights_only=False)
+    if "anny" in ckpt_path:
+        model = ModelAnny(max_batch=max_batch, max_persons=max_persons, body_model=body_model, device=device,
+                          **vars(ckpt["args"]))
+        model.load_state_dict(ckpt["model_state_dict"], strict=False)
+        return model.finalize()
     kwargs = dict(vars(ckpt["args"]))
     kwargs["type"] = ckpt["args"].train_return_type
     kwargs["img_size"] = ckpt["args"].img_size[0]

@@ -49,6 +49,7 @@ struct HphLayer {
 
 struct mhmr_engine {
   mhmr_config cfg{};
+  std::string enc = "backbone.encoder.";   // state-dict prefix of the DINOv2 backbone
   int D = 0, depth = 0, heads = 0, res = 0, N = 0, T = 0, C = 0, Cp = 0, Cq = 0, nkv = 0, ndec = 0;
   bool finalized = false;
   std::map<std::string, DevBuf> weights;   // raw fp32 device copies, keyed like the state_dict
@@ -105,6 +106,17 @@ struct mhmr_engine {
   SmplxScratch sx;
   GemmPlan patch_plan, cls0_plan, kv_plan;
   int* h_count = nullptr;  // pinned host copy of the person count
+  int r_rows = 0;          // capacity of the refined rows (persons, plus one cls row per image for the Anny head)
+
+  // Anny head (multi_hmr_anny/): decoder tokens of every cell, camera from the cls token, stacked regressors
+  __half *Wdt16 = nullptr, *dec16 = nullptr;     // dec_to_token [dim, D]; tokens [max_batch*N, dim]
+  float* dt_rowadd = nullptr;                    // [N, dim] dec_pos_emb + dec_to_token bias
+  float *cls_x = nullptr, *cls_h = nullptr;      // [max_batch, D] bulk cls rows / mlp_fov_unique hidden
+  float *K_use = nullptr, *det_score = nullptr;  // [max_batch, 9] intrinsics used; [max_persons] (NMS scratch)
+  float *W1 = nullptr, *b1 = nullptr;            // [4 dim, dim]: first Linears of offset | dist | shape | pose
+  float* b_pose2 = nullptr;                      // [6J] mlp_pose.2 bias + init_body_pose
+  int* anny_ints = nullptr;                      // device [2]: batch size, refined rows
+  GemmPlan dt_plan;
 
   ~mhmr_engine() {
     for (void* p : owned) cudaFree(p);
@@ -164,7 +176,7 @@ int to_f16(mhmr_engine* e, const float* src, int64_t lds, int rows, int cols, in
 
 int finalize_vit(mhmr_engine* e, cudaStream_t st) {
   const int D = e->D, N = e->N, T = e->T, Bm = e->cfg.max_batch;
-  const std::string enc = "backbone.encoder.";
+  const std::string enc = e->enc;
   NEEDW(pw, enc + "patch_embed.proj.weight", static_cast<int64_t>(D) * 588);
   NEEDW(pb, enc + "patch_embed.proj.bias", D);
   NEEDW(cls, enc + "cls_token", D);
@@ -254,6 +266,27 @@ int finalize_vit(mhmr_engine* e, cudaStream_t st) {
     TRY(gemm_plan_init(&L.fc2, e->H16, 4 * D, L.Wfc2, 4 * D, static_cast<int>(M), D, 4 * D, epi_fc2, f2, pick_bn(D)));
   }
   if (e->w(enc + "norm.weight", D) == nullptr || e->w(enc + "norm.bias", D) == nullptr) return MHMR_ERR_STATE;
+  return MHMR_OK;
+}
+
+// workspaces of the central-stream refinement for `rows` token rows
+int alloc_refine(mhmr_engine* e, int rows, cudaStream_t st) {
+  const int D = e->D;
+  e->r_rows = rows;
+  TRY(e->alloc(&e->r_rowidx, rows));
+  TRY(e->alloc(&e->r_patch, static_cast<size_t>(rows) * 592));
+  TRY(e->alloc(&e->r_x, static_cast<size_t>(rows) * D));
+  TRY(e->alloc(&e->r_h, static_cast<size_t>(rows) * 4 * D));
+  TRY(e->alloc(&e->r_term, static_cast<size_t>(e->depth) * rows * D));
+  TRY(e->alloc(&e->r_barrier, 4));
+  std::vector<RefineLayer> rl(e->depth);
+  for (int l = 0; l < e->depth; ++l) {
+    const VitLayer& L = e->vit[l];
+    rl[l] = RefineLayer{L.O16, L.Wproj32, L.bproj, L.ls1, L.ln2_g, L.ln2_b, L.Wfc1_32, L.bfc1, L.Wfc2_32, L.bfc2, L.ls2};
+  }
+  TRY(e->alloc(&e->r_layers, rl.size()));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->r_layers, rl.data(), rl.size() * sizeof(RefineLayer), cudaMemcpyHostToDevice, st));
+  MHMR_CUDA_CHECK(cudaStreamSynchronize(st));  // rl lives on this stack frame
   return MHMR_OK;
 }
 
@@ -370,22 +403,7 @@ int finalize_head(mhmr_engine* e, cudaStream_t st) {
   TRY(e->alloc(&e->ffh, static_cast<size_t>(Pm) * kHphDim));
   TRY(e->alloc(&e->dec, static_cast<size_t>(Pm) * e->ndec));
   TRY(e->alloc(&e->K_det, static_cast<size_t>(Pm) * 9));
-  if (e->cfg.refine_central) {
-    TRY(e->alloc(&e->r_rowidx, Pm));
-    TRY(e->alloc(&e->r_patch, static_cast<size_t>(Pm) * 592));
-    TRY(e->alloc(&e->r_x, static_cast<size_t>(Pm) * D));
-    TRY(e->alloc(&e->r_h, static_cast<size_t>(Pm) * 4 * D));
-    TRY(e->alloc(&e->r_term, static_cast<size_t>(e->depth) * Pm * D));
-    TRY(e->alloc(&e->r_barrier, 4));
-    std::vector<RefineLayer> rl(e->depth);
-    for (int l = 0; l < e->depth; ++l) {
-      const VitLayer& L = e->vit[l];
-      rl[l] = RefineLayer{L.O16, L.Wproj32, L.bproj, L.ls1, L.ln2_g, L.ln2_b, L.Wfc1_32, L.bfc1, L.Wfc2_32, L.bfc2, L.ls2};
-    }
-    TRY(e->alloc(&e->r_layers, rl.size()));
-    MHMR_CUDA_CHECK(cudaMemcpyAsync(e->r_layers, rl.data(), rl.size() * sizeof(RefineLayer), cudaMemcpyHostToDevice, st));
-    MHMR_CUDA_CHECK(cudaStreamSynchronize(st));  // rl lives on this stack frame
-  }
+  if (e->cfg.refine_central) TRY(alloc_refine(e, Pm, st));
   return MHMR_OK;
 }
 
@@ -430,6 +448,121 @@ int finalize_body(mhmr_engine* e, cudaStream_t st) {
   TRY(e->alloc(&e->sx.Amat, static_cast<size_t>(Pm) * 55 * 12));
   TRY(e->alloc(&e->sx.xf, static_cast<size_t>(Pm) * 16));
   TRY(e->alloc(&e->sx.jposed, static_cast<size_t>(Pm) * 55 * 3));
+  return MHMR_OK;
+}
+
+// Anny head (multi_hmr_anny/multi_hmr.py:41-95, encoder.py:16-31, hph.py): weights under the checkpoint's own keys.
+int finalize_anny(mhmr_engine* e, cudaStream_t st) {
+  const int D = e->D, N = e->N, Bm = e->cfg.max_batch, Pm = e->cfg.max_persons, nb = e->cfg.num_betas;
+  const int dim = e->cfg.xat_dim, mlp = e->cfg.xat_mlp_dim, J = e->cfg.num_joints, depth = e->cfg.xat_depth;
+  const int inner = e->cfg.xat_num_heads * 32, J6 = 6 * J, J6p = (J6 + 3) & ~3;
+  const size_t BN = static_cast<size_t>(Bm) * N;
+  TRY(e->alloc(&e->z32, BN * D));
+  TRY(e->alloc(&e->ctx16, BN * e->Cp));
+  TRY(e->alloc(&e->scores_raw, BN));
+  TRY(e->alloc(&e->KV32, BN * e->nkv));
+  TRY(e->alloc(&e->Kinv, static_cast<size_t>(Bm) * 9));
+  TRY(e->alloc(&e->K_use, static_cast<size_t>(Bm) * 9));
+  TRY(e->alloc(&e->count, 4));
+  TRY(e->alloc(&e->img_off, static_cast<size_t>(Bm) + 1));
+  TRY(e->alloc(&e->det_score, Pm));
+  TRY(e->alloc(&e->anny_ints, 2));
+  TRY(e->alloc(&e->one, 4));
+  const int one_h = 1;
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->one, &one_h, sizeof(int), cudaMemcpyHostToDevice, st));
+  MHMR_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&e->h_count), sizeof(int)));
+
+  // detection: mlp_det hidden layer as a GEMM on the normed fp16 features (encoder.py:26,59)
+  NEEDW(c0w, "encoder.mlp_det.0.weight", static_cast<int64_t>(D) * D) NEEDW(c0b, "encoder.mlp_det.0.bias", D)
+  NEEDW(c2w, "encoder.mlp_det.2.weight", D) NEEDW(c2b, "encoder.mlp_det.2.bias", 1)
+  (void)c2w; (void)c2b;
+  TRY(to_f16(e, c0w, D, D, D, D, &e->Wcls0, st));
+  GemmEpi ce; ce.bias = c0b; ce.out = e->H16; ce.ldo = D;
+  TRY(gemm_plan_init(&e->cls0_plan, e->ctx16, e->Cp, e->Wcls0, D, static_cast<int>(BN), D, D, EPI_BIAS_RELU_F16, ce, pick_bn(D)));
+  // field of view from the cls token (encoder.py:29-31,50)
+  NEEDW(f0w, "encoder.mlp_fov_unique.0.weight", static_cast<int64_t>(D) * D) NEEDW(f0b, "encoder.mlp_fov_unique.0.bias", D)
+  NEEDW(f2w, "encoder.mlp_fov_unique.2.weight", D) NEEDW(f2b, "encoder.mlp_fov_unique.2.bias", 1)
+  NEEDW(fmax, "encoder.fov_max", 1)
+  (void)f0w; (void)f0b; (void)f2w; (void)f2b; (void)fmax;
+  TRY(e->alloc(&e->cls_x, static_cast<size_t>(Bm) * D));
+  TRY(e->alloc(&e->cls_h, static_cast<size_t>(Bm) * D));
+
+  // decoder tokens of every cell: dec_to_token(feat) + dec_pos_emb (multi_hmr.py:127-128), fp16 GEMM output
+  NEEDW(dtw, "dec_to_token.weight", static_cast<int64_t>(dim) * D) NEEDW(dtb, "dec_to_token.bias", dim)
+  NEEDW(pos, "dec_pos_emb", static_cast<int64_t>(N) * dim)
+  TRY(to_f16(e, dtw, D, dim, D, D, &e->Wdt16, st));
+  TRY(e->alloc(&e->dt_rowadd, static_cast<size_t>(N) * dim));
+  TRY(add_vec(pos, dtb, e->dt_rowadd, static_cast<int64_t>(N) * dim, dim, st));
+  TRY(e->alloc(&e->dec16, BN * dim));
+  GemmEpi te; te.rowadd = e->dt_rowadd; te.rows_in = N; te.out = e->dec16; te.ldo = dim;
+  TRY(gemm_plan_init(&e->dt_plan, e->ctx16, e->Cp, e->Wdt16, D, static_cast<int>(BN), dim, D, EPI_ROWADD_F16, te, pick_bn(dim)));
+
+  // HPH layers; the keys / values of all of them come from ONE GEMM over the tokens (to_kv, hph.py:88,99)
+  e->hph.resize(depth);
+  TRY(e->alloc(&e->Wkv16, static_cast<size_t>(e->nkv) * dim));
+  for (int l = 0; l < depth; ++l) {
+    HphLayer& L = e->hph[l];
+    const std::string p = "decoder.transformer.layers." + std::to_string(l) + ".";
+    NEEDW(a, p + "0.norm.weight", dim) NEEDW(b, p + "0.norm.bias", dim)
+    NEEDW(c, p + "0.fn.to_qkv.weight", 3ll * inner * dim)
+    NEEDW(d, p + "0.fn.to_out.0.weight", static_cast<int64_t>(dim) * inner) NEEDW(f, p + "0.fn.to_out.0.bias", dim)
+    NEEDW(g, p + "1.norm.weight", dim) NEEDW(hh, p + "1.norm.bias", dim)
+    NEEDW(kvw, p + "1.fn.to_kv.weight", 2ll * inner * dim)
+    NEEDW(qw, p + "1.fn.to_q.weight", static_cast<int64_t>(inner) * dim)
+    NEEDW(co, p + "1.fn.to_out.0.weight", static_cast<int64_t>(dim) * inner) NEEDW(cb, p + "1.fn.to_out.0.bias", dim)
+    NEEDW(n2g, p + "2.norm.weight", dim) NEEDW(n2b, p + "2.norm.bias", dim)
+    NEEDW(f0, p + "2.fn.net.0.weight", static_cast<int64_t>(mlp) * dim) NEEDW(f0bb, p + "2.fn.net.0.bias", mlp)
+    NEEDW(f3, p + "2.fn.net.3.weight", static_cast<int64_t>(dim) * mlp) NEEDW(f3b, p + "2.fn.net.3.bias", dim)
+    L.ln0_g = a; L.ln0_b = b; L.Wqkv = c; L.Wsa_out = d; L.bsa_out = f;
+    L.ln1_g = g; L.ln1_b = hh; L.Wq = qw; L.Wca_out = co; L.bca_out = cb;
+    L.ln2_g = n2g; L.ln2_b = n2b; L.Wff0 = f0; L.bff0 = f0bb; L.Wff3 = f3; L.bff3 = f3b;
+    TRY(f32_to_f16_2d(kvw, dim, e->Wkv16 + static_cast<size_t>(l) * 2 * inner * dim, dim, 2 * inner, dim, st));
+  }
+  GemmEpi ke; ke.out = e->KV32; ke.ldo = e->nkv;
+  TRY(gemm_plan_init(&e->kv_plan, e->dec16, dim, e->Wkv16, dim, static_cast<int>(BN), e->nkv, dim, EPI_BIAS_F32, ke, pick_bn(e->nkv)));
+
+  // regressors (multi_hmr.py:59-66): the four first Linears stacked; mlp_pose's init_body_pose columns folded into
+  // its bias, and init_body_pose added to the bias of its second Linear (:157)
+  NEEDW(o0w, "mlp_offset.0.weight", static_cast<int64_t>(dim) * dim) NEEDW(o0b, "mlp_offset.0.bias", dim)
+  NEEDW(o2w, "mlp_offset.2.weight", 2ll * dim) NEEDW(o2b, "mlp_offset.2.bias", 2)
+  NEEDW(d0w, "mlp_dist.0.weight", static_cast<int64_t>(dim) * dim) NEEDW(d0b, "mlp_dist.0.bias", dim)
+  NEEDW(d2w, "mlp_dist.2.weight", dim) NEEDW(d2b, "mlp_dist.2.bias", 1)
+  NEEDW(s0w, "mlp_shape.0.weight", static_cast<int64_t>(dim) * dim) NEEDW(s0b, "mlp_shape.0.bias", dim)
+  NEEDW(s2w, "mlp_shape.2.weight", static_cast<int64_t>(nb) * dim) NEEDW(s2b, "mlp_shape.2.bias", nb)
+  NEEDW(p0w, "mlp_pose.0.weight", static_cast<int64_t>(dim) * (dim + J6)) NEEDW(p0b, "mlp_pose.0.bias", dim)
+  NEEDW(p2w, "mlp_pose.2.weight", static_cast<int64_t>(J6) * dim) NEEDW(p2b, "mlp_pose.2.bias", J6)
+  NEEDW(useful, "useful_rotmat", J) NEEDW(init, "init_body_pose", J6)
+  (void)o2w; (void)o2b; (void)d2w; (void)d2b; (void)s2w; (void)s2b; (void)useful;
+  TRY(e->alloc(&e->W1, static_cast<size_t>(4) * dim * dim));
+  TRY(e->alloc(&e->b1, static_cast<size_t>(4) * dim));
+  const size_t blk = static_cast<size_t>(dim) * dim;
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->W1, o0w, blk * 4, cudaMemcpyDeviceToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->W1 + blk, d0w, blk * 4, cudaMemcpyDeviceToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->W1 + 2 * blk, s0w, blk * 4, cudaMemcpyDeviceToDevice, st));
+  TRY(repack_f32(p0w, dim + J6, 0, e->W1 + 3 * blk, dim, 0, dim, dim, false, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->b1, o0b, dim * 4, cudaMemcpyDeviceToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->b1 + dim, d0b, dim * 4, cudaMemcpyDeviceToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->b1 + 2 * dim, s0b, dim * 4, cudaMemcpyDeviceToDevice, st));
+  float *Wpi = nullptr, *init_pad = nullptr;
+  TRY(e->alloc(&Wpi, static_cast<size_t>(dim) * J6p));
+  TRY(repack_f32(p0w, dim + J6, dim, Wpi, J6p, 0, dim, J6, true, st));
+  TRY(e->alloc(&init_pad, J6p));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(init_pad, init, J6 * 4, cudaMemcpyDeviceToDevice, st));
+  TRY(skinny_linear(init_pad, J6p, e->one, 1, J6, Wpi, J6p, p0b, dim, nullptr, nullptr, 0.f, 0, nullptr, 0,
+                    e->b1 + 3 * dim, dim, st));
+  TRY(e->alloc(&e->b_pose2, J6));
+  TRY(add_vec(p2b, init, e->b_pose2, J6, J6, st));
+
+  // per-person buffers
+  TRY(e->alloc(&e->zc, static_cast<size_t>(Pm) * D));
+  TRY(e->alloc(&e->xa, static_cast<size_t>(Pm) * dim));
+  TRY(e->alloc(&e->qkvp, static_cast<size_t>(Pm) * 3 * inner));
+  TRY(e->alloc(&e->att, static_cast<size_t>(Pm) * inner));
+  TRY(e->alloc(&e->qca, static_cast<size_t>(Pm) * inner));
+  TRY(e->alloc(&e->ffh, static_cast<size_t>(Pm) * mlp));
+  TRY(e->alloc(&e->offh, static_cast<size_t>(Pm) * 4 * dim));
+  TRY(e->alloc(&e->dec, static_cast<size_t>(Pm) * J6p));
+  if (e->cfg.refine_central) TRY(alloc_refine(e, Pm + Bm, st));
   return MHMR_OK;
 }
 
@@ -494,8 +627,8 @@ int vit_forward(mhmr_engine* e, const ImgSrc& x, int B, float* z_out, cudaStream
     TRY(run_plan(e, MHMR_CAT_GEMM_FC2, L.fc2, M, st));
   }
   // final norm, cls dropped: fp32 features (head query side, optional user copy) + fp16 context columns
-  const float* ng = e->w("backbone.encoder.norm.weight");
-  const float* nb = e->w("backbone.encoder.norm.bias");
+  const float* ng = e->w(e->enc + "norm.weight");
+  const float* nb = e->w(e->enc + "norm.bias");
   if (e->ln_fold) {
     LAUNCH(MHMR_CAT_LAYERNORM,
            layernorm_split(e->Xn16, e->Xlo, ng, nb, e->ctx16, e->Cp, e->z32, D, M, D, 1e-6f, T, 1, st));
@@ -516,16 +649,19 @@ int vit_forward(mhmr_engine* e, const ImgSrc& x, int B, float* z_out, cudaStream
 // applied by person_gather.  Same arithmetic as dinov2 Block.forward (reached from blocks/dinov2.py:25).  Four
 // launches: patches / row indices, patch embedding, every projection term at once, the MLP chain of all blocks in one
 // persistent cooperative kernel (refine.cu).
+// With n_cls > 0 the cls rows of images 0..n_cls-1 are refined too, ahead of the persons (r_x rows [0, n_cls)), and
+// `rows` receives the device-side row count.
 int refine_streams(mhmr_engine* e, const ImgSrc& x, const int* det_b, const int* det_y, const int* det_x,
-                   const int* count, cudaStream_t st) {
-  const int D = e->D, Pm = e->cfg.max_persons;
+                   const int* count, int n_cls, int* rows, cudaStream_t st) {
+  const int D = e->D, Pm = e->cfg.max_persons, Rm = e->r_rows;
   LAUNCH(MHMR_CAT_REFINE, refine_prepare(x.f32, x.u8, x.lut, e->cfg.img_size, e->rowadd, D, det_b, det_y, det_x, count, Pm, e->res,
-                                         e->r_rowidx, e->r_patch, 592, e->r_x, st));
+                                         n_cls, e->cls_pos, n_cls > 0 ? rows : nullptr, e->r_rowidx, e->r_patch, 592, e->r_x, st));
+  const int* rc = n_cls > 0 ? rows : count;
   SkinnyExtra none;
-  LAUNCH(MHMR_CAT_REFINE, skinny_linear_ex(e->r_patch, 592, none, count, Pm, 588, e->Wpatch32, 588, nullptr, D, nullptr,
+  LAUNCH(MHMR_CAT_REFINE, skinny_linear_ex(e->r_patch, 592, none, rc, Rm, 588, e->Wpatch32, 588, nullptr, D, nullptr,
                                            nullptr, 0.f, 0, e->r_x, D, e->r_x, D, st));
-  LAUNCH(MHMR_CAT_REFINE, refine_proj_terms(e->r_layers, e->depth, e->r_rowidx, count, D, Pm, e->r_term, st));
-  LAUNCH(MHMR_CAT_REFINE, refine_mlp_chain(e->r_layers, e->depth, count, D, Pm, e->r_term, e->r_x, e->r_h, e->r_barrier, st));
+  LAUNCH(MHMR_CAT_REFINE, refine_proj_terms(e->r_layers, e->depth, e->r_rowidx, rc, D, Rm, e->r_term, st));
+  LAUNCH(MHMR_CAT_REFINE, refine_mlp_chain(e->r_layers, e->depth, rc, D, Rm, e->r_term, e->r_x, e->r_h, e->r_barrier, st));
   return MHMR_OK;
 }
 
@@ -540,7 +676,8 @@ int head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float d
   LAUNCH(MHMR_CAT_HEAD, ctx_fourier(e->Kinv, e->w("camera.freq_bands"), e->ctx16, e->Cp, B, res, D, e->Cp - D, st));
   // detection (model.py:133-158)
   TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->cls0_plan, BN, st));
-  LAUNCH(MHMR_CAT_HEAD, rowdot_sigmoid(e->H16, D, e->w("mlp_classif.2.weight"), e->w("mlp_classif.2.bias"), e->scores_raw, BN, D, st));
+  LAUNCH(MHMR_CAT_HEAD, rowdot_sigmoid(e->H16, D, e->w("mlp_classif.2.weight"), e->w("mlp_classif.2.bias"), e->scores_raw,
+                                       nullptr, true, BN, D, st));
   if (forced_idx != nullptr) {
     LAUNCH(MHMR_CAT_HEAD, forced_detections(e->scores_raw, o->scores_map, B, res, forced_idx, forced_P, det_b, det_y, det_x,
                          o->det_score, count_true, count, e->img_off, st));
@@ -554,10 +691,10 @@ int head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float d
   const std::string h = "x_attention_head.";
   const float* xr = nullptr;
   if (e->cfg.refine_central) {
-    TRY(refine_streams(e, x, det_b, det_y, det_x, count, st));
+    TRY(refine_streams(e, x, det_b, det_y, det_x, count, 0, nullptr, st));
     xr = e->r_x;
   }
-  LAUNCH(MHMR_CAT_HEAD, person_gather(e->z32, xr, e->w("backbone.encoder.norm.weight"), e->w("backbone.encoder.norm.bias"),
+  LAUNCH(MHMR_CAT_HEAD, person_gather(e->z32, xr, e->w(e->enc + "norm.weight"), e->w(e->enc + "norm.bias"),
                        e->Kinv, e->w("camera.freq_bands"), e->w(h + "cross_queries_x"),
                        e->w(h + "cross_queries_y"), e->w(h + "cross_values_x"), e->w(h + "cross_values_y"),
                        det_b, det_y, det_x, count, Pm, res, D, e->zc, e->query, e->vals, Cq, st));
@@ -606,6 +743,94 @@ int head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float d
   return MHMR_OK;
 }
 
+// Multi_HMR.forward (multi_hmr_anny/multi_hmr.py:98-175) up to the body model's inputs.  K == nullptr: the regressed
+// intrinsics are used.
+int anny_head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float det_thresh, int nms,
+                      const int64_t* forced_idx, int forced_P, const mhmr_anny_outputs* o, cudaStream_t st) {
+  const int D = e->D, N = e->N, T = e->T, res = e->res, Pm = e->cfg.max_persons, Bm = e->cfg.max_batch;
+  const int nb = e->cfg.num_betas, dim = e->cfg.xat_dim, mlp = e->cfg.xat_mlp_dim, J = e->cfg.num_joints;
+  const int heads = e->cfg.xat_num_heads, inner = heads * 32, BN = B * N, J6p = (6 * J + 3) & ~3;
+  int* det_b = o->det_idx; int* det_y = o->det_idx + Pm; int* det_x = o->det_idx + 2 * Pm;
+  int* count = e->count + 2;
+  const float* ng = e->w(e->enc + "norm.weight");
+  const float* nbias = e->w(e->enc + "norm.bias");
+  // detection (encoder.py:59-60, multi_hmr.py:116-124)
+  TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->cls0_plan, BN, st));
+  LAUNCH(MHMR_CAT_HEAD, rowdot_sigmoid(e->H16, D, e->w("encoder.mlp_det.2.weight"), e->w("encoder.mlp_det.2.bias"),
+                                       e->scores_raw, o->logits, false, BN, D, st));
+  if (forced_idx != nullptr) {
+    LAUNCH(MHMR_CAT_HEAD, forced_detections(e->scores_raw, o->scores_map, B, res, forced_idx, forced_P, det_b, det_y, det_x,
+                                            e->det_score, o->count, count, e->img_off, st));
+  } else {
+    LAUNCH(MHMR_CAT_HEAD, nms_compact(e->scores_raw, o->scores_map, B, res, nms, det_thresh, Pm, det_b, det_y, det_x,
+                                      e->det_score, o->count, count, e->img_off, st));
+  }
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->h_count, o->count, sizeof(int), cudaMemcpyDeviceToHost, st));
+  // decoder tokens of every cell and the keys / values of every HPH layer
+  TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->dt_plan, BN, st));
+  TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->kv_plan, BN, st));
+  // cls rows (camera) and person rows: fp32 refinement, or the bulk pass
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->anny_ints, &B, sizeof(int), cudaMemcpyHostToDevice, st));
+  const float *xr = nullptr, *cls_src = e->cls_x;
+  if (e->cfg.refine_central) {
+    TRY(refine_streams(e, x, det_b, det_y, det_x, count, B, e->anny_ints + 1, st));
+    xr = e->r_x + static_cast<size_t>(B) * D;
+    cls_src = e->r_x;
+  } else if (e->ln_fold) {
+    LAUNCH(MHMR_CAT_HEAD, cls_gather(e->Xn16, e->Xlo, D, T, B, D, e->cls_x, st));
+  } else {
+    LAUNCH(MHMR_CAT_HEAD, cls_gather(e->X, nullptr, D, T, B, D, e->cls_x, st));
+  }
+  // field of view and intrinsics (encoder.py:50-56)
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(cls_src, D, e->anny_ints, Bm, D, e->w("encoder.mlp_fov_unique.0.weight"), D,
+                                      e->w("encoder.mlp_fov_unique.0.bias"), D, ng, nbias, 1e-6f, 1, nullptr, 0, e->cls_h,
+                                      D, st));
+  LAUNCH(MHMR_CAT_HEAD, anny_camera(e->cls_h, D, e->w("encoder.mlp_fov_unique.2.weight"), e->w("encoder.mlp_fov_unique.2.bias"),
+                                    e->w("encoder.fov_max"), K, B, e->cfg.img_size, o->fov, o->K_regressed, e->K_use,
+                                    e->Kinv, st));
+  ++e->launches;  // anny_camera = 2 kernels
+  // queries: dec_to_token(final-normed feature) + dec_pos_emb at the detected cells (multi_hmr.py:131)
+  LAUNCH(MHMR_CAT_HEAD, anny_gather(e->z32, xr, ng, nbias, e->w("dec_pos_emb"), det_b, det_y, det_x, count, Pm, res, D,
+                                    dim, e->zc, e->xa, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->zc, D, count, Pm, D, e->w("dec_to_token.weight"), D, e->w("dec_to_token.bias"), dim,
+                                      nullptr, nullptr, 0.f, 0, e->xa, dim, e->xa, dim, st));
+  // HPH (hph.py:133-140): PreNorm self-attention, cross-attention, feed-forward
+  for (int l = 0; l < e->cfg.xat_depth; ++l) {
+    HphLayer& L = e->hph[l];
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wqkv, dim, nullptr, 3 * inner, L.ln0_g, L.ln0_b, 1e-5f, 0,
+                                        nullptr, 0, e->qkvp, 3 * inner, st));
+    LAUNCH(MHMR_CAT_HEAD, hph_self_attn(e->qkvp, 3 * inner, det_b, e->img_off, count, Pm, heads, e->att, inner, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->att, inner, count, Pm, inner, L.Wsa_out, inner, L.bsa_out, dim, nullptr, nullptr,
+                                        0.f, 0, e->xa, dim, e->xa, dim, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wq, dim, nullptr, inner, L.ln1_g, L.ln1_b, 1e-5f, 0,
+                                        nullptr, 0, e->qca, inner, st));
+    LAUNCH(MHMR_CAT_HEAD, hph_cross_attn(e->qca, inner, e->KV32, e->nkv, l * 2 * inner, l * 2 * inner + inner, det_b, count,
+                                         Pm, heads, N, e->att, inner, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->att, inner, count, Pm, inner, L.Wca_out, inner, L.bca_out, dim, nullptr, nullptr,
+                                        0.f, 0, e->xa, dim, e->xa, dim, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wff0, dim, L.bff0, mlp, L.ln2_g, L.ln2_b, 1e-5f, 2,
+                                        nullptr, 0, e->ffh, mlp, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->ffh, mlp, count, Pm, mlp, L.Wff3, mlp, L.bff3, dim, nullptr, nullptr, 0.f, 0,
+                                        e->xa, dim, e->xa, dim, st));
+  }
+  // regressors: hidden layers of offset | dist | shape | pose at once, then the four output Linears
+  float* hid = e->offh;
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, e->W1, dim, e->b1, 4 * dim, nullptr, nullptr, 0.f, 1,
+                                      nullptr, 0, hid, 4 * dim, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid, 4 * dim, count, Pm, dim, e->w("mlp_offset.2.weight"), dim, e->w("mlp_offset.2.bias"),
+                                      2, nullptr, nullptr, 0.f, 0, nullptr, 0, o->offset, 2, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + dim, 4 * dim, count, Pm, dim, e->w("mlp_dist.2.weight"), dim,
+                                      e->w("mlp_dist.2.bias"), 1, nullptr, nullptr, 0.f, 0, nullptr, 0, o->dist_pp, 1, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + 2 * dim, 4 * dim, count, Pm, dim, e->w("mlp_shape.2.weight"), dim,
+                                      e->w("mlp_shape.2.bias"), nb, nullptr, nullptr, 0.f, 0, nullptr, 0, o->shape, nb, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + 3 * dim, 4 * dim, count, Pm, dim, e->w("mlp_pose.2.weight"), dim, e->b_pose2,
+                                      6 * J, nullptr, nullptr, 0.f, 0, nullptr, 0, e->dec, J6p, st));
+  LAUNCH(MHMR_CAT_HEAD, anny_person_post(e->dec, J6p, J, e->w("useful_rotmat"), o->shape, nb, o->offset, o->dist_pp, e->K_use,
+                                         e->Kinv, det_b, det_y, det_x, count, Pm, o->rotmat, o->rotmat_homo, o->rotvec,
+                                         o->dist, o->loc, o->transl, o->K_det, st));
+  return MHMR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -615,15 +840,27 @@ int mhmr_create(const mhmr_config* cfg, mhmr_engine** out) {
   MHMR_REQUIRE(cfg->arch >= 0 && cfg->arch <= 2, "arch must be 0 (S), 1 (B) or 2 (L)");
   MHMR_REQUIRE(cfg->img_size > 0 && cfg->img_size % 14 == 0, "Invalid img size");  // model.py:65
   MHMR_REQUIRE(cfg->max_batch > 0 && cfg->max_persons > 0, "capacities must be positive");
-  MHMR_REQUIRE(cfg->num_betas == 10 || cfg->num_betas == 11, "num_betas must be 10 or 11");  // model.py:384
-  MHMR_REQUIRE(cfg->xat_depth >= 1 && cfg->xat_depth <= 8 && cfg->xat_num_heads >= 1, "bad HPH geometry");
-  MHMR_REQUIRE(cfg->person_center_idx >= 0 && cfg->person_center_idx < 55,
-               "person_center must be one of the 55 kinematic joints");
-  MHMR_REQUIRE(cfg->num_verts > 0, "num_verts must be positive");
+  MHMR_REQUIRE(cfg->head == MHMR_HEAD_SMPLX || cfg->head == MHMR_HEAD_ANNY, "head must be 0 (SMPL-X) or 1 (Anny)");
+  if (cfg->head == MHMR_HEAD_SMPLX) {
+    MHMR_REQUIRE(cfg->num_betas == 10 || cfg->num_betas == 11, "num_betas must be 10 or 11");  // model.py:384
+    MHMR_REQUIRE(cfg->xat_depth >= 1 && cfg->xat_depth <= 8 && cfg->xat_num_heads >= 1, "bad HPH geometry");
+    MHMR_REQUIRE(cfg->person_center_idx >= 0 && cfg->person_center_idx < 55,
+                 "person_center must be one of the 55 kinematic joints");
+    MHMR_REQUIRE(cfg->num_verts > 0, "num_verts must be positive");
+  } else {
+    // multi_hmr.py:28-36: the HPH kernels are built for dim_head = 32 (one lane per channel)
+    MHMR_REQUIRE(cfg->xat_depth >= 1 && cfg->xat_num_heads >= 1, "bad HPH geometry");
+    MHMR_REQUIRE(cfg->xat_dim > 0 && cfg->xat_dim % 32 == 0 && cfg->xat_mlp_dim > 0 && cfg->xat_mlp_dim % 32 == 0,
+                 "xat_dim and xat_mlp_dim must be positive multiples of 32");
+    MHMR_REQUIRE(cfg->num_joints >= 1 && cfg->num_betas >= 1, "num_joints and num_betas must be positive");
+    MHMR_REQUIRE(cfg->person_center_idx >= 0 && cfg->person_center_idx < cfg->num_joints,
+                 "person_center_idx must index a bone of the body model");
+  }
   auto e = std::make_unique<mhmr_engine>();
   e->cfg = *cfg;
   const ArchSpec& a = kArch[cfg->arch];
   e->D = a.D; e->depth = a.depth; e->heads = a.heads;
+  if (cfg->head == MHMR_HEAD_ANNY) e->enc = "encoder.backbone.";
   e->res = cfg->img_size / 14;
   e->N = e->res * e->res;
   e->T = e->N + 1;
@@ -673,8 +910,12 @@ int mhmr_finalize(mhmr_engine* h) {
   if (h->finalized) return MHMR_OK;
   cudaStream_t st = nullptr;
   TRY(finalize_vit(h, st));
-  TRY(finalize_head(h, st));
-  TRY(finalize_body(h, st));
+  if (h->cfg.head == MHMR_HEAD_ANNY) {
+    TRY(finalize_anny(h, st));
+  } else {
+    TRY(finalize_head(h, st));
+    TRY(finalize_body(h, st));
+  }
   MHMR_CUDA_CHECK(cudaStreamSynchronize(st));
   h->finalized = true;
   return MHMR_OK;
@@ -685,6 +926,7 @@ static int forward_impl(mhmr_engine* h, const ImgSrc& x, const float* K, int B, 
                         void* stream) {
   MHMR_REQUIRE(h != nullptr && K != nullptr && out != nullptr, "null argument");
   if (!h->finalized) { set_last_error("mhmr_forward before mhmr_finalize"); return MHMR_ERR_STATE; }
+  MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_SMPLX, "mhmr_forward needs an SMPL-X engine (use mhmr_forward_anny)");
   MHMR_REQUIRE(B >= 1 && B <= h->cfg.max_batch, "batch exceeds max_batch");
   MHMR_REQUIRE(forced_idx == nullptr || (forced_P >= 0 && forced_P <= h->cfg.max_persons),
                "forced_P exceeds max_persons");
@@ -717,6 +959,56 @@ int mhmr_forward_u8(mhmr_engine* h, const uint8_t* img_u8, const float* lut, con
   return forward_impl(h, src, K, B, det_thresh, nms_kernel_size, forced_idx, forced_P, out, stream);
 }
 
+static int forward_anny_impl(mhmr_engine* h, const ImgSrc& x, const float* K, int B, float det_thresh,
+                             int nms_kernel_size, const int64_t* forced_idx, int forced_P, const mhmr_anny_outputs* out,
+                             void* stream) {
+  MHMR_REQUIRE(h != nullptr && out != nullptr, "null argument");
+  if (!h->finalized) { set_last_error("mhmr_forward_anny before mhmr_finalize"); return MHMR_ERR_STATE; }
+  MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_ANNY, "mhmr_forward_anny needs an engine created with head = MHMR_HEAD_ANNY");
+  MHMR_REQUIRE(B >= 1 && B <= h->cfg.max_batch, "batch exceeds max_batch");
+  MHMR_REQUIRE(forced_idx == nullptr || (forced_P >= 0 && forced_P <= h->cfg.max_persons),
+               "forced_P exceeds max_persons");
+  // multi_hmr.py:118: an even kernel changes the pooled map's shape and the reference fails on the comparison
+  MHMR_REQUIRE(forced_idx != nullptr || nms_kernel_size <= 1 || nms_kernel_size % 2 == 1,
+               "nms_kernel_size must be odd");
+  MHMR_REQUIRE(out->scores_map && out->logits && out->count && out->det_idx && out->K_regressed && out->fov &&
+                   out->K_det && out->offset && out->loc && out->dist && out->dist_pp && out->shape && out->rotmat &&
+                   out->rotmat_homo && out->rotvec && out->transl,
+               "a required output buffer is null");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  h->launches = 0;
+  TRY(vit_forward(h, x, B, out->z, st));
+  return anny_head_forward(h, x, K, B, det_thresh, nms_kernel_size, forced_idx, forced_P, out, st);
+}
+
+int mhmr_forward_anny(mhmr_engine* h, const float* x, const float* K, int B, float det_thresh, int nms_kernel_size,
+                      const int64_t* forced_idx, int forced_P, const mhmr_anny_outputs* out, void* stream) {
+  MHMR_REQUIRE(x != nullptr, "null image");
+  ImgSrc src;
+  src.f32 = x;
+  return forward_anny_impl(h, src, K, B, det_thresh, nms_kernel_size, forced_idx, forced_P, out, stream);
+}
+
+int mhmr_forward_anny_u8(mhmr_engine* h, const uint8_t* img_u8, const float* lut, const float* K, int B,
+                         float det_thresh, int nms_kernel_size, const int64_t* forced_idx, int forced_P,
+                         const mhmr_anny_outputs* out, void* stream) {
+  MHMR_REQUIRE(img_u8 != nullptr && lut != nullptr, "null image / table");
+  ImgSrc src;
+  src.u8 = img_u8;
+  src.lut = lut;
+  return forward_anny_impl(h, src, K, B, det_thresh, nms_kernel_size, forced_idx, forced_P, out, stream);
+}
+
+int mhmr_anny_place(mhmr_engine* h, int P, int V, const float* bone_poses, const float* transl, const float* K_det,
+                    float* v3d, float* j3d, float* v2d, float* j2d, float* transl_pelvis, void* stream) {
+  MHMR_REQUIRE(h != nullptr, "null engine");
+  MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_ANNY, "mhmr_anny_place needs an Anny engine");
+  MHMR_REQUIRE(P >= 0 && P <= h->cfg.max_persons && V >= 0, "P exceeds max_persons");
+  MHMR_REQUIRE(bone_poses && transl && K_det && j3d && j2d && transl_pelvis && (V == 0 || v3d), "null argument");
+  return anny_place(bone_poses, transl, K_det, h->cfg.person_center_idx, P, V, h->cfg.num_joints, v3d, j3d, v2d, j2d,
+                    transl_pelvis, static_cast<cudaStream_t>(stream));
+}
+
 int mhmr_sync_count(mhmr_engine* h, void* stream, int* num_persons) {
   MHMR_REQUIRE(h != nullptr && num_persons != nullptr, "null argument");
   MHMR_CUDA_CHECK(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
@@ -745,6 +1037,7 @@ int mhmr_smplx_forward(mhmr_engine* h, int P, const float* rotvec, const float* 
                        void* stream) {
   MHMR_REQUIRE(h != nullptr, "null engine");
   if (!h->finalized) { set_last_error("mhmr_smplx_forward before mhmr_finalize"); return MHMR_ERR_STATE; }
+  MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_SMPLX, "mhmr_smplx_forward needs an SMPL-X engine");
   MHMR_REQUIRE(P >= 1 && P <= h->cfg.max_persons, "P exceeds max_persons");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   MHMR_CUDA_CHECK(cudaMemcpyAsync(h->count + 1, &P, sizeof(int), cudaMemcpyHostToDevice, st));

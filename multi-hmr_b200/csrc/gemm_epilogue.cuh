@@ -100,7 +100,8 @@ template <int EPI>
 __device__ __forceinline__ void epilogue_chunk(const float* scratch, const GemmEpi& ep, int M, int N, int m_base,
                                                int n0, int lane, EpiRowState& st) {
   constexpr bool kLn = epi_is_ln_consumer<EPI>();
-  constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_RELU_F16 || kLn);
+  constexpr bool kRowAdd16 = (EPI == EPI_ROWADD_F16);
+  constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_RELU_F16 || kLn || kRowAdd16);
   constexpr bool kResid = (EPI == EPI_LS_RESID_F32);
   if constexpr (EPI == EPI_LS_RESID_SPLIT) {
     // residual stream as two fp16 planes: same lane mapping as the fp16 outputs (8 columns x 2 planes = 2 x 16 B)
@@ -157,12 +158,22 @@ __device__ __forceinline__ void epilogue_chunk(const float* scratch, const GemmE
   } else if constexpr (kF16) {
     const int cg = lane & 3, rs = lane >> 2;  // 8 columns per lane, 8 rows per instruction
     const int n = n0 + cg * 8;
-    const float4 b0 = __ldg(reinterpret_cast<const float4*>(ep.bias + n));
-    const float4 b1 = __ldg(reinterpret_cast<const float4*>(ep.bias + n + 4));
+    float4 b0 = make_float4(0.f, 0.f, 0.f, 0.f), b1 = b0;
+    if constexpr (!kRowAdd16) {
+      b0 = __ldg(reinterpret_cast<const float4*>(ep.bias + n));
+      b1 = __ldg(reinterpret_cast<const float4*>(ep.bias + n + 4));
+    }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int rl = k * 8 + rs;
       const int m = m_base + rl;
+      if constexpr (kRowAdd16) {  // per-row addend: row m % rows_in of the table
+        if (m < M) {
+          const float* ra = ep.rowadd + static_cast<int64_t>(m % ep.rows_in) * N + n;
+          b0 = __ldg(reinterpret_cast<const float4*>(ra));
+          b1 = __ldg(reinterpret_cast<const float4*>(ra + 4));
+        }
+      }
       const float4 v0 = *reinterpret_cast<const float4*>(scratch + rl * kScratchStride + cg * 8);
       const float4 v1 = *reinterpret_cast<const float4*>(scratch + rl * kScratchStride + cg * 8 + 4);
       float2 y[4];

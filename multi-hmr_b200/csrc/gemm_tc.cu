@@ -245,6 +245,7 @@ int launch_bn(const GemmPlan* p, cudaStream_t stream) {
     case EPI_LS_RESID_SPLIT: return launch_one<BN, CL, EPI_LS_RESID_SPLIT>(p, stream);
     case EPI_LN_BIAS_F16: return launch_one<BN, CL, EPI_LN_BIAS_F16>(p, stream);
     case EPI_LN_GELU_F16: return launch_one<BN, CL, EPI_LN_GELU_F16>(p, stream);
+    case EPI_ROWADD_F16: return launch_one<BN, CL, EPI_ROWADD_F16>(p, stream);
     default: break;
   }
   set_last_error("gemm: unknown epilogue kind");
@@ -264,7 +265,7 @@ int gemm_plan_init(GemmPlan* plan, const __half* A, int64_t lda, const __half* W
   MHMR_REQUIRE(epi_kind >= 0 && epi_kind < EPI_NUM_KINDS, "gemm: bad epilogue kind");
   if (epi_kind != EPI_LS_RESID_SPLIT)
     MHMR_REQUIRE(ep.out != nullptr && ep.ldo % 8 == 0, "gemm: output missing or pitch not multiple of 8");
-  if (epi_kind != EPI_BIAS_F32 && epi_kind != EPI_ROWADD_F32)
+  if (epi_kind != EPI_BIAS_F32 && epi_kind != EPI_ROWADD_F32 && epi_kind != EPI_ROWADD_F16)
     MHMR_REQUIRE(ep.bias != nullptr, "gemm: bias required for this epilogue");
   if (epi_kind == EPI_LS_RESID_F32 || epi_kind == EPI_LS_RESID_SPLIT)
     MHMR_REQUIRE(ep.gamma != nullptr, "gemm: gamma required");
@@ -275,7 +276,7 @@ int gemm_plan_init(GemmPlan* plan, const __half* A, int64_t lda, const __half* W
   if (epi_kind == EPI_LN_BIAS_F16 || epi_kind == EPI_LN_GELU_F16)
     MHMR_REQUIRE(ep.stats != nullptr && ep.stat_slots > 0 && ep.stat_slots % 2 == 0 && ep.stat_slots <= 8,
                  "gemm: folded-LN consumer needs row statistics (even slot count, at most 8)");
-  if (epi_kind == EPI_ROWADD_F32)
+  if (epi_kind == EPI_ROWADD_F32 || epi_kind == EPI_ROWADD_F16)
     MHMR_REQUIRE(ep.rowadd != nullptr && ep.rows_in > 0, "gemm: rowadd/rows_in required");
   plan->M = M; plan->N = N; plan->K = K; plan->bn = bn; plan->epi = epi_kind; plan->ep = ep;
   int rc = make_tmap_2d(&plan->tmA, A, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, M, K, lda * 2, BM, BK, true);

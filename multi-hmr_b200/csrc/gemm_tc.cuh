@@ -10,6 +10,7 @@
 //   EPI_LS_RESID_F32   out32 += gamma * (acc + bias)  in place  (attn.proj / mlp.fc2 + LayerScale + residual)
 //   EPI_ROWADD_F32     out32[remap(m)] = acc + rowadd[m % rows_in]  (patch-embed + bias + pos-embed scatter)
 //   EPI_BIAS_F32       out32 = acc + bias (bias may be null)    (HPH to_kv, cross_attn_transformer.py:187)
+//   EPI_ROWADD_F16     out16 = acc + rowadd[m % rows_in]         (Anny dec_to_token + bias + dec_pos_emb)
 //
 // LayerNorm folded into the two Linears that follow it (dinov2 Block: norm1 -> attn.qkv, norm2 -> mlp.fc1).
 // With W'[n,k] = W[n,k] ln_gamma[k] - mean_k(W[n,:] ln_gamma) (rows centred, rounded to fp16) and
@@ -39,13 +40,14 @@ enum GemmEpiKind : int {
   EPI_LS_RESID_SPLIT = 6,
   EPI_LN_BIAS_F16 = 7,
   EPI_LN_GELU_F16 = 8,
-  EPI_NUM_KINDS = 9,
+  EPI_ROWADD_F16 = 9,
+  EPI_NUM_KINDS = 10,
 };
 
 struct GemmEpi {
   const float* bias = nullptr;    // [N]
   const float* gamma = nullptr;   // [N]            (EPI_LS_RESID_F32)
-  const float* rowadd = nullptr;  // [rows_in, N]   (EPI_ROWADD_F32)
+  const float* rowadd = nullptr;  // [rows_in, N]   (EPI_ROWADD_F32 / EPI_ROWADD_F16)
   void* out = nullptr;            // fp16 or fp32, row pitch ldo elements
   int64_t ldo = 0;
   // Row remap: out_row = (m / rows_in) * rows_out + row_off + (m % rows_in); rows_in == 0 => identity.

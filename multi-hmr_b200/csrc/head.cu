@@ -24,7 +24,8 @@ __device__ __forceinline__ float sigmoid_clamped(float x) {
 // scores[r] = clamp(sigmoid(hidden[r,:] . w + b))   — second Linear of mlp_classif (model.py:135)
 // ----------------------------------------------------------------------------------------------
 __global__ void rowdot_sigmoid_kernel(const __half* __restrict__ hid, int64_t ld, const float* __restrict__ w,
-                                      const float* __restrict__ b, float* __restrict__ scores, int M, int D) {
+                                      const float* __restrict__ b, float* __restrict__ scores,
+                                      float* __restrict__ logits, int clamp, int M, int D) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
   const int lane = threadIdx.x & 31;
@@ -40,7 +41,11 @@ __global__ void rowdot_sigmoid_kernel(const __half* __restrict__ hid, int64_t ld
     acc += a.x * w0.x + a.y * w0.y + c.x * w0.z + c.y * w0.w + d.x * w1.x + d.y * w1.y + e.x * w1.z + e.y * w1.w;
   }
   acc = warp_sum(acc);
-  if (lane == 0) scores[row] = sigmoid_clamped(acc + b[0]);
+  if (lane == 0) {
+    const float l = acc + b[0];
+    if (logits != nullptr) logits[row] = l;
+    scores[row] = clamp ? sigmoid_clamped(l) : 1.0f / (1.0f + expf(-l));  // Anny: no clamp (encoder.py:59-60)
+  }
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -276,16 +281,30 @@ person_gather_kernel(const float* __restrict__ z32, const float* __restrict__ xr
 // Central-stream refinement, step 0: per detected person, the token row index of its cell in the [B*T, .]
 // token matrices (cls row skipped), its 14x14x3 input patch in the order of the patch-embed weight
 // (c, ky, kx: dinov2 PatchEmbed Conv2d) and the fp32 (pos_embed + bias) row of its cell.
+// With n_cls > 0 the first n_cls refined rows are the cls tokens of images 0..n_cls-1 (start value cls_token +
+// pos_embed[0], a zero patch, so the patch embedding adds nothing) and person p is row n_cls + p;
+// rows_out = n_cls + *count.
 __global__ void __launch_bounds__(256)
 refine_prepare_kernel(const float* __restrict__ img, const uint8_t* __restrict__ img_u8,
                       const float* __restrict__ lut, int S, const float* __restrict__ rowadd, int D,
                       const int* __restrict__ det_b, const int* __restrict__ det_y,
-                      const int* __restrict__ det_x, const int* __restrict__ count, int res,
+                      const int* __restrict__ det_x, const int* __restrict__ count, int res, int n_cls,
+                      const float* __restrict__ cls_pos, int* __restrict__ rows_out,
                       int* __restrict__ rowidx, float* __restrict__ patch, int ldp, float* __restrict__ xr) {
-  const int p = blockIdx.x;
+  const int r = blockIdx.x;
+  const int N = res * res;
+  if (r == 0 && threadIdx.x == 0 && rows_out != nullptr) *rows_out = n_cls + *count;
+  if (r < n_cls) {
+    if (threadIdx.x == 0) rowidx[r] = r * (N + 1);
+    for (int k = threadIdx.x; k < ldp; k += 256) patch[static_cast<int64_t>(r) * ldp + k] = 0.f;
+    for (int c = threadIdx.x; c < D; c += 256) xr[static_cast<int64_t>(r) * D + c] = cls_pos[c];
+    return;
+  }
+  const int p = r - n_cls;
   if (p >= *count) return;
+  rowidx += n_cls; patch += static_cast<int64_t>(n_cls) * ldp; xr += static_cast<int64_t>(n_cls) * D;
   const int b = det_b[p], y = det_y[p], x = det_x[p];
-  const int N = res * res, n = y * res + x;
+  const int n = y * res + x;
   if (threadIdx.x == 0) rowidx[p] = b * (N + 1) + 1 + n;
   for (int k = threadIdx.x; k < ldp; k += 256) {
     float v = 0.f;
@@ -591,6 +610,60 @@ hph_cross_attn_kernel(const float* __restrict__ q, int ldq, const float* __restr
 }
 
 // ----------------------------------------------------------------------------------------------
+// Rotation helpers (roma.special_gramschmidt, roma.rotmat_to_rotvec)
+// ----------------------------------------------------------------------------------------------
+// R = [e1 e2 e1 x e2] (columns) from the two 3-vectors a, b by Gram-Schmidt; R[r][c]
+__device__ __forceinline__ void gram_schmidt(float a0, float a1, float a2, float b0, float b1, float b2,
+                                             float (&R)[3][3]) {
+  const float na = sqrtf(a0 * a0 + a1 * a1 + a2 * a2);
+  a0 /= na; a1 /= na; a2 /= na;
+  const float dp = a0 * b0 + a1 * b1 + a2 * b2;
+  b0 -= dp * a0; b1 -= dp * a1; b2 -= dp * a2;
+  const float nb = sqrtf(b0 * b0 + b1 * b1 + b2 * b2);
+  b0 /= nb; b1 /= nb; b2 /= nb;
+  const float c0 = a1 * b2 - a2 * b1, c1 = a2 * b0 - a0 * b2, c2 = a0 * b1 - a1 * b0;
+  R[0][0] = a0; R[0][1] = b0; R[0][2] = c0;
+  R[1][0] = a1; R[1][1] = b1; R[1][2] = c1;
+  R[2][0] = a2; R[2][1] = b2; R[2][2] = c2;
+}
+
+// rotation matrix -> unit quaternion (xyzw, largest of diagonal / trace) -> rotation vector rv[3]
+__device__ __forceinline__ void rotmat_to_rotvec(const float (&R)[3][3], float* rv) {
+  const float tr = R[0][0] + R[1][1] + R[2][2];
+  int choice = 0;
+  float best = R[0][0];
+  if (R[1][1] > best) { best = R[1][1]; choice = 1; }
+  if (R[2][2] > best) { best = R[2][2]; choice = 2; }
+  if (tr > best) { choice = 3; }
+  float q[4];
+  if (choice != 3) {
+    const int i = choice, jj = (i + 1) % 3, k = (jj + 1) % 3;
+    q[i] = 1.f - tr + 2.f * R[i][i];
+    q[jj] = R[jj][i] + R[i][jj];
+    q[k] = R[k][i] + R[i][k];
+    q[3] = R[k][jj] - R[jj][k];
+  } else {
+    q[0] = R[2][1] - R[1][2];
+    q[1] = R[0][2] - R[2][0];
+    q[2] = R[1][0] - R[0][1];
+    q[3] = 1.f + tr;
+  }
+  const float nq = sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+  q[0] /= nq; q[1] /= nq; q[2] /= nq; q[3] /= nq;
+  if (q[3] < 0.f) { q[0] = -q[0]; q[1] = -q[1]; q[2] = -q[2]; q[3] = -q[3]; }
+  const float half = atan2f(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]), q[3]);
+  const float ang = 2.f * half;
+  float sc;
+  if (fabsf(ang) <= 1e-3f) {
+    const float a2_ = ang * ang;
+    sc = 2.f + a2_ / 12.f + 7.f * a2_ * a2_ / 2880.f;
+  } else {
+    sc = ang / sinf(ang / 2.f);
+  }
+  rv[0] = sc * q[0]; rv[1] = sc * q[1]; rv[2] = sc * q[2];
+}
+
+// ----------------------------------------------------------------------------------------------
 // Per-person post-processing: 6D -> rotation matrix (utils/humans.py:12-22, roma.special_gramschmidt),
 // rotation matrix -> rotation vector (model.py:291, roma.rotmat_to_rotvec), distance (model.py:189-203),
 // location (model.py:272-275), translation K^-1 [loc,1] dist (blocks/smpl_layer.py:123).
@@ -612,55 +685,14 @@ __global__ void person_post_kernel(const float* __restrict__ dec, int ld_dec, in
   const int j = threadIdx.x;
   if (j < 53) {
     const float* x6 = d + j * 6;
-    float a0 = x6[0], a1 = x6[1], a2 = x6[2], b0 = x6[3], b1 = x6[4], b2 = x6[5];
-    const float na = sqrtf(a0 * a0 + a1 * a1 + a2 * a2);
-    a0 /= na; a1 /= na; a2 /= na;
-    const float dp = a0 * b0 + a1 * b1 + a2 * b2;
-    b0 -= dp * a0; b1 -= dp * a1; b2 -= dp * a2;
-    const float nb = sqrtf(b0 * b0 + b1 * b1 + b2 * b2);
-    b0 /= nb; b1 /= nb; b2 /= nb;
-    const float c0 = a1 * b2 - a2 * b1, c1 = a2 * b0 - a0 * b2, c2 = a0 * b1 - a1 * b0;
-    // columns (e1, e2, e3): R[r][c]
-    const float R[3][3] = {{a0, b0, c0}, {a1, b1, c1}, {a2, b2, c2}};
+    float R[3][3];
+    gram_schmidt(x6[0], x6[1], x6[2], x6[3], x6[4], x6[5], R);
     float* Ro = rotmat + (static_cast<int64_t>(p) * 53 + j) * 9;
 #pragma unroll
     for (int r = 0; r < 3; ++r)
 #pragma unroll
       for (int c = 0; c < 3; ++c) Ro[r * 3 + c] = R[r][c];
-    // rotmat -> unit quaternion (xyzw): largest of (diagonal, trace)
-    const float tr = R[0][0] + R[1][1] + R[2][2];
-    int choice = 0;
-    float best = R[0][0];
-    if (R[1][1] > best) { best = R[1][1]; choice = 1; }
-    if (R[2][2] > best) { best = R[2][2]; choice = 2; }
-    if (tr > best) { choice = 3; }
-    float q[4];
-    if (choice != 3) {
-      const int i = choice, jj = (i + 1) % 3, k = (jj + 1) % 3;
-      q[i] = 1.f - tr + 2.f * R[i][i];
-      q[jj] = R[jj][i] + R[i][jj];
-      q[k] = R[k][i] + R[i][k];
-      q[3] = R[k][jj] - R[jj][k];
-    } else {
-      q[0] = R[2][1] - R[1][2];
-      q[1] = R[0][2] - R[2][0];
-      q[2] = R[1][0] - R[0][1];
-      q[3] = 1.f + tr;
-    }
-    const float nq = sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    q[0] /= nq; q[1] /= nq; q[2] /= nq; q[3] /= nq;
-    if (q[3] < 0.f) { q[0] = -q[0]; q[1] = -q[1]; q[2] = -q[2]; q[3] = -q[3]; }
-    const float half = atan2f(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]), q[3]);
-    const float ang = 2.f * half;
-    float sc;
-    if (fabsf(ang) <= 1e-3f) {
-      const float a2_ = ang * ang;
-      sc = 2.f + a2_ / 12.f + 7.f * a2_ * a2_ / 2880.f;
-    } else {
-      sc = ang / sinf(ang / 2.f);
-    }
-    float* rv = rotvec + (static_cast<int64_t>(p) * 53 + j) * 3;
-    rv[0] = sc * q[0]; rv[1] = sc * q[1]; rv[2] = sc * q[2];
+    rotmat_to_rotvec(R, rotvec + (static_cast<int64_t>(p) * 53 + j) * 3);
   } else if (j == 53) {
     const int b = det_b[p];
     const float* Kb = K + b * 9;
@@ -714,10 +746,10 @@ int loc_to_transl(const float* loc, const float* dist, const float* K_det, int P
 // ------------------------------------------------------------------------------------------------
 // Host launchers
 // ------------------------------------------------------------------------------------------------
-int rowdot_sigmoid(const __half* hid, int64_t ld, const float* w, const float* b, float* scores, int M,
-                   int D, cudaStream_t st) {
+int rowdot_sigmoid(const __half* hid, int64_t ld, const float* w, const float* b, float* scores, float* logits,
+                   bool clamp, int M, int D, cudaStream_t st) {
   MHMR_REQUIRE(D % 8 == 0 && ld % 8 == 0, "rowdot: D and pitch must be multiples of 8");
-  rowdot_sigmoid_kernel<<<(M + 7) / 8, 256, 0, st>>>(hid, ld, w, b, scores, M, D);
+  rowdot_sigmoid_kernel<<<(M + 7) / 8, 256, 0, st>>>(hid, ld, w, b, scores, logits, clamp ? 1 : 0, M, D);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }
@@ -767,11 +799,13 @@ int person_gather(const float* z32, const float* xr, const float* norm_g, const 
 
 int refine_prepare(const float* img, const uint8_t* img_u8, const float* lut, int S, const float* rowadd, int D,
                    const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons, int res,
-                   int* rowidx, float* patch, int ldp, float* xr, cudaStream_t st) {
+                   int n_cls, const float* cls_pos, int* rows_out, int* rowidx, float* patch, int ldp, float* xr,
+                   cudaStream_t st) {
   MHMR_REQUIRE(ldp >= 588 && ldp % 4 == 0, "refine_prepare: patch pitch must be >= 588 and a multiple of 4");
   MHMR_REQUIRE((img != nullptr) != (img_u8 != nullptr), "refine_prepare: exactly one image source");
-  refine_prepare_kernel<<<max_persons, 256, 0, st>>>(img, img_u8, lut, S, rowadd, D, det_b, det_y, det_x, count, res, rowidx,
-                                                     patch, ldp, xr);
+  MHMR_REQUIRE(n_cls == 0 || cls_pos != nullptr, "refine_prepare: cls rows need cls_token + pos_embed[0]");
+  refine_prepare_kernel<<<n_cls + max_persons, 256, 0, st>>>(img, img_u8, lut, S, rowadd, D, det_b, det_y, det_x, count,
+                                                             res, n_cls, cls_pos, rows_out, rowidx, patch, ldp, xr);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }
@@ -849,6 +883,211 @@ int person_post(const float* dec, int ld_dec, int num_betas, const float* offset
   person_post_kernel<<<max_persons, 128, 0, st>>>(dec, ld_dec, num_betas, offset, K, Kinv, det_b, det_y, det_x,
                                                   count, focal_norm, rotmat, rotvec, shape, expr, dist_pp,
                                                   dist, loc, transl, K_det);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Anny variant (multi_hmr_anny/): camera from the cls token, decoder inputs, per-person post-processing and the
+// placement of the body model's output.  Same conventions as above: fp32, persons in (b, y, x) order, grids sized
+// for the capacity and the device-side count.
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+__global__ void cls_gather_kernel(const void* __restrict__ X, const __half* __restrict__ Xlo, int64_t ld, int T, int D,
+                                  float* __restrict__ out) {
+  const int b = blockIdx.x;
+  const int64_t row = static_cast<int64_t>(b) * T * ld;
+  for (int c = threadIdx.x; c < D; c += blockDim.x) {
+    float v;
+    if (Xlo != nullptr)
+      v = __half2float(static_cast<const __half*>(X)[row + c]) + __half2float(Xlo[row + c]);
+    else
+      v = static_cast<const float*>(X)[row + c];
+    out[static_cast<int64_t>(b) * D + c] = v;
+  }
+}
+
+// One warp per image: fov = fov_max * sigmoid(h . w2 + b2), f = (S/2) / tan(fov/2), K_regressed = [[f,0,S/2],
+// [0,f,S/2],[0,0,1]] (encoder.py:50-56), K_use = K given, else K_regressed.
+__global__ void anny_camera_kernel(const float* __restrict__ hid, int ldh, const float* __restrict__ w2,
+                                   const float* __restrict__ b2, const float* __restrict__ fov_max,
+                                   const float* __restrict__ K, int B, int D, float half_s, float* __restrict__ fov,
+                                   float* __restrict__ K_reg, float* __restrict__ K_use) {
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;
+  const int lane = threadIdx.x & 31;
+  float acc = 0.f;
+  for (int k = lane; k < D; k += 32) acc += hid[static_cast<int64_t>(b) * ldh + k] * w2[k];
+  acc = warp_sum(acc);
+  const float a = fov_max[0] * (1.0f / (1.0f + expf(-(acc + b2[0]))));
+  const float f = half_s / tanf(a / 2.0f);
+  const float kr[9] = {f, 0.f, half_s, 0.f, f, half_s, 0.f, 0.f, 1.f};
+  if (lane < 9) {
+    K_reg[b * 9 + lane] = kr[lane];
+    K_use[b * 9 + lane] = (K != nullptr) ? K[b * 9 + lane] : kr[lane];
+  }
+  if (lane == 0) fov[b] = a;
+}
+
+__global__ void __launch_bounds__(256)
+anny_gather_kernel(const float* __restrict__ z32, const float* __restrict__ xr, const float* __restrict__ norm_g,
+                   const float* __restrict__ norm_b, const float* __restrict__ pos, const int* __restrict__ det_b,
+                   const int* __restrict__ det_y, const int* __restrict__ det_x, const int* __restrict__ count,
+                   int res, int D, int dim, float* __restrict__ zc, float* __restrict__ xa) {
+  __shared__ float red[8];
+  const int p = blockIdx.x;
+  if (p >= *count) return;
+  const int n = det_y[p] * res + det_x[p];
+  const float* zr = z32 + (static_cast<int64_t>(det_b[p]) * res * res + n) * D;
+  float mean = 0.f, rstd = 1.f;
+  if (xr != nullptr) {
+    const float* r = xr + static_cast<int64_t>(p) * D;
+    float s = 0.f;
+    for (int c = threadIdx.x; c < D; c += 256) s += r[c];
+    mean = block_sum_256(s, red) / D;
+    float q = 0.f;
+    for (int c = threadIdx.x; c < D; c += 256) { const float d = r[c] - mean; q += d * d; }
+    rstd = rsqrtf(block_sum_256(q, red) / D + 1e-6f);
+  }
+  for (int c = threadIdx.x; c < D; c += 256)
+    zc[static_cast<int64_t>(p) * D + c] =
+        (xr != nullptr) ? (xr[static_cast<int64_t>(p) * D + c] - mean) * rstd * norm_g[c] + norm_b[c] : zr[c];
+  for (int c = threadIdx.x; c < dim; c += 256) xa[static_cast<int64_t>(p) * dim + c] = pos[static_cast<int64_t>(n) * dim + c];
+}
+
+// multi_hmr.py:143-175: thread j < J: 6D (rot6d.reshape(3, 2): columns (x0, x2, x4), (x1, x3, x5)) -> R by
+// Gram-Schmidt, R <- u_j R + (1 - u_j) I, rotvec, [[R, 0], [0, 1]]; then the per-person scalars and shape.
+__global__ void anny_person_post_kernel(const float* __restrict__ rot6d, int ld6, int J, const float* __restrict__ useful,
+                                        float* __restrict__ shape, int num_betas, const float* __restrict__ offset,
+                                        const float* __restrict__ dist_pp, const float* __restrict__ K_use,
+                                        const float* __restrict__ Kinv, const int* __restrict__ det_b,
+                                        const int* __restrict__ det_y, const int* __restrict__ det_x,
+                                        const int* __restrict__ count, float* __restrict__ rotmat,
+                                        float* __restrict__ rotmat_homo, float* __restrict__ rotvec,
+                                        float* __restrict__ dist, float* __restrict__ loc, float* __restrict__ transl,
+                                        float* __restrict__ K_det) {
+  const int p = blockIdx.x;
+  if (p >= *count) return;
+  for (int j = threadIdx.x; j < J; j += blockDim.x) {
+    const float* x6 = rot6d + static_cast<int64_t>(p) * ld6 + j * 6;
+    float R[3][3];
+    gram_schmidt(x6[0], x6[2], x6[4], x6[1], x6[3], x6[5], R);
+    const float u = useful[j];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) R[r][c] = u * R[r][c] + (1.0f - u) * (r == c ? 1.0f : 0.0f);
+    const int64_t pj = static_cast<int64_t>(p) * J + j;
+    float* Ro = rotmat + pj * 9;
+    float* Ho = rotmat_homo + pj * 16;
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const float v = (r < 3 && c < 3) ? R[r][c] : (r == 3 && c == 3 ? 1.0f : 0.0f);
+        if (r < 3 && c < 3) Ro[r * 3 + c] = v;
+        Ho[r * 4 + c] = v;
+      }
+    rotmat_to_rotvec(R, rotvec + pj * 3);
+  }
+  for (int i = threadIdx.x; i < num_betas; i += blockDim.x) {
+    const float v = shape[p * num_betas + i];
+    shape[p * num_betas + i] = 1.0f / (1.0f + expf(-v));
+  }
+  if (threadIdx.x == 0) {
+    const int b = det_b[p];
+    const float* Kb = K_use + b * 9;
+    const float* Ki = Kinv + b * 9;
+    for (int i = 0; i < 9; ++i) K_det[p * 9 + i] = Kb[i];
+    const float dd = Kb[0] / fmaxf(expf(dist_pp[p]), 1e-5f);
+    dist[p] = dd;
+    const float lx = (static_cast<float>(det_x[p]) + 0.5f + offset[p * 2 + 0]) * 14.f;
+    const float ly = (static_cast<float>(det_y[p]) + 0.5f + offset[p * 2 + 1]) * 14.f;
+    loc[p * 2 + 0] = lx;
+    loc[p * 2 + 1] = ly;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) transl[p * 3 + r] = (Ki[r * 3] * lx + Ki[r * 3 + 1] * ly + Ki[r * 3 + 2]) * dd;
+  }
+}
+
+// multi_hmr.py:180-186: x <- (x - bone(center)) + transl for every vertex and bone, then K_det (x / x_z)
+__global__ void anny_place_kernel(const float* __restrict__ bone_poses, const float* __restrict__ transl,
+                                  const float* __restrict__ K_det, int center, int V, int J, float* __restrict__ v3d,
+                                  float* __restrict__ j3d, float* __restrict__ v2d, float* __restrict__ j2d,
+                                  float* __restrict__ transl_pelvis) {
+  const int p = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= V + J) return;
+  const float* bp = bone_poses + static_cast<int64_t>(p) * J * 16;
+  const float c0 = bp[center * 16 + 3], c1 = bp[center * 16 + 7], c2 = bp[center * 16 + 11];
+  const float t0 = transl[p * 3], t1 = transl[p * 3 + 1], t2 = transl[p * 3 + 2];
+  float x, y, z;
+  float *o3, *o2;
+  if (i < V) {
+    o3 = v3d + (static_cast<int64_t>(p) * V + i) * 3;
+    o2 = (v2d != nullptr) ? v2d + (static_cast<int64_t>(p) * V + i) * 2 : nullptr;
+    x = o3[0]; y = o3[1]; z = o3[2];
+  } else {
+    const int j = i - V;
+    o3 = j3d + (static_cast<int64_t>(p) * J + j) * 3;
+    o2 = j2d + (static_cast<int64_t>(p) * J + j) * 2;
+    x = bp[j * 16 + 3]; y = bp[j * 16 + 7]; z = bp[j * 16 + 11];
+  }
+  x = (x - c0) + t0; y = (y - c1) + t1; z = (z - c2) + t2;
+  o3[0] = x; o3[1] = y; o3[2] = z;
+  if (i == V) { transl_pelvis[p * 3] = x; transl_pelvis[p * 3 + 1] = y; transl_pelvis[p * 3 + 2] = z; }
+  if (o2 != nullptr) {
+    const float* K = K_det + p * 9;
+    const float u = x / z, v = y / z, w = z / z;
+    o2[0] = K[0] * u + K[1] * v + K[2] * w;
+    o2[1] = K[3] * u + K[4] * v + K[5] * w;
+  }
+}
+
+}  // namespace
+
+int cls_gather(const void* X, const __half* Xlo, int64_t ld, int T, int B, int D, float* out, cudaStream_t st) {
+  cls_gather_kernel<<<B, 256, 0, st>>>(X, Xlo, ld, T, D, out);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
+}
+
+int anny_camera(const float* hid, int ldh, const float* w2, const float* b2, const float* fov_max, const float* K,
+                int B, int S, float* fov, float* K_reg, float* K_use, float* Kinv, cudaStream_t st) {
+  anny_camera_kernel<<<(B + 7) / 8, 256, 0, st>>>(hid, ldh, w2, b2, fov_max, K, B, ldh, static_cast<float>(S) / 2.0f,
+                                                  fov, K_reg, K_use);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return invert_K(K_use, Kinv, B, st);
+}
+
+int anny_gather(const float* z32, const float* xr, const float* norm_g, const float* norm_b, const float* pos,
+                const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons, int res,
+                int D, int dim, float* zc, float* xa, cudaStream_t st) {
+  anny_gather_kernel<<<max_persons, 256, 0, st>>>(z32, xr, norm_g, norm_b, pos, det_b, det_y, det_x, count, res, D,
+                                                  dim, zc, xa);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
+}
+
+int anny_person_post(const float* rot6d, int ld6, int J, const float* useful, float* shape, int num_betas,
+                     const float* offset, const float* dist_pp, const float* K_use, const float* Kinv,
+                     const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
+                     float* rotmat, float* rotmat_homo, float* rotvec, float* dist, float* loc, float* transl,
+                     float* K_det, cudaStream_t st) {
+  anny_person_post_kernel<<<max_persons, 192, 0, st>>>(rot6d, ld6, J, useful, shape, num_betas, offset, dist_pp, K_use,
+                                                       Kinv, det_b, det_y, det_x, count, rotmat, rotmat_homo, rotvec,
+                                                       dist, loc, transl, K_det);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
+}
+
+int anny_place(const float* bone_poses, const float* transl, const float* K_det, int center, int P, int V, int J,
+               float* v3d, float* j3d, float* v2d, float* j2d, float* transl_pelvis, cudaStream_t st) {
+  MHMR_REQUIRE(P >= 0 && P <= 65535 && V >= 0 && J >= 1 && center >= 0 && center < J, "anny_place: bad sizes");
+  if (P == 0) return MHMR_OK;
+  anny_place_kernel<<<dim3((V + J + 255) / 256, P), 256, 0, st>>>(bone_poses, transl, K_det, center, V, J, v3d, j3d,
+                                                                  v2d, j2d, transl_pelvis);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }

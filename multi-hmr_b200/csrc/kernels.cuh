@@ -33,8 +33,9 @@ int repack_f32(const float* src, int64_t lds, int scol, float* dst, int64_t ldd,
 int add_vec(const float* a, const float* b, float* out, int64_t n, int64_t b_period, cudaStream_t stream);
 
 // ---- head.cu ---------------------------------------------------------------------------------
-int rowdot_sigmoid(const __half* hid, int64_t ld, const float* w, const float* b, float* scores, int M,
-                   int D, cudaStream_t st);
+// scores[r] = sigmoid(hid[r,:] . w + b), clamped to [1e-4, 1-1e-4] when `clamp` (SMPL-X head); logits nullable
+int rowdot_sigmoid(const __half* hid, int64_t ld, const float* w, const float* b, float* scores, float* logits,
+                   bool clamp, int M, int D, cudaStream_t st);
 int nms_compact(const float* scores, float* scores_out, int B, int res, int nms_k, float thresh,
                 int max_persons, int* det_b, int* det_y, int* det_x, float* det_score, int* count,
                 int* count_clamped, int* img_off, cudaStream_t st);
@@ -51,10 +52,10 @@ int person_gather(const float* z32, const float* xr, const float* norm_g, const 
                   const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons, int res,
                   int D, float* zc, float* query, float* vals, int ldq, cudaStream_t st);
 // central-stream refinement (engine.cu:refine_streams): row indices, input patches and pos-embed rows of the
-// detected cells
+// detected cells, after n_cls leading cls rows (rows_out, nullable: n_cls + persons)
 int refine_prepare(const float* img, const uint8_t* img_u8, const float* lut, int S, const float* rowadd, int D, const int* det_b, const int* det_y,
-                   const int* det_x, const int* count, int max_persons, int res, int* rowidx, float* patch,
-                   int ldp, float* xr, cudaStream_t st);
+                   const int* det_x, const int* count, int max_persons, int res, int n_cls, const float* cls_pos,
+                   int* rows_out, int* rowidx, float* patch, int ldp, float* xr, cudaStream_t st);
 int kv_add_rows(float* KV, int64_t ldkv, const float* dKV, int ncols, const int* det_b, const int* det_y,
                 const int* det_x, const int* count, int max_persons, int res, cudaStream_t st);
 int skinny_linear(const float* x, int ldx, const int* count, int max_persons, int K, const float* W, int ldw,
@@ -91,6 +92,27 @@ int person_post(const float* dec, int ld_dec, int num_betas, const float* offset
                 const float* Kinv, const int* det_b, const int* det_y, const int* det_x, const int* count,
                 int max_persons, float focal_norm, float* rotmat, float* rotvec, float* shape, float* expr,
                 float* dist_pp, float* dist, float* loc, float* transl, float* K_det, cudaStream_t st);
+
+// ---- head.cu: Anny variant (multi_hmr_anny/) -------------------------------------------------------
+// out[b, :] = fp32 row b*T of the residual stream (X fp32, or the two-term split hi = X, lo = Xlo)
+int cls_gather(const void* X, const __half* Xlo, int64_t ld, int T, int B, int D, float* out, cudaStream_t st);
+// field of view, K_regressed, the intrinsics used (K or K_regressed) and their inverse from the hidden layer of
+// mlp_fov_unique (encoder.py:50-56)
+int anny_camera(const float* hid, int ldh, const float* w2, const float* b2, const float* fov_max, const float* K,
+                int B, int S, float* fov, float* K_reg, float* K_use, float* Kinv, cudaStream_t st);
+// per person: zc = final-normed feature (LN of the refined row xr, or the bulk row of z32), xa = dec_pos_emb[cell]
+int anny_gather(const float* z32, const float* xr, const float* norm_g, const float* norm_b, const float* pos,
+                const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons, int res,
+                int D, int dim, float* zc, float* xa, cudaStream_t st);
+// 6D -> R (J joints), useful_rotmat blend, rotvec, homogeneous 4x4; loc, dist, transl, sigmoid(shape), K_det
+int anny_person_post(const float* rot6d, int ld6, int J, const float* useful, float* shape, int num_betas,
+                     const float* offset, const float* dist_pp, const float* K_use, const float* Kinv,
+                     const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
+                     float* rotmat, float* rotmat_homo, float* rotvec, float* dist, float* loc, float* transl,
+                     float* K_det, cudaStream_t st);
+// after the body model: centre bone, translation, projection
+int anny_place(const float* bone_poses, const float* transl, const float* K_det, int center, int P, int V, int J,
+               float* v3d, float* j3d, float* v2d, float* j2d, float* transl_pelvis, cudaStream_t st);
 
 // ---- smplx_lbs.cu ----------------------------------------------------------------------------
 struct SmplxDeviceModel {

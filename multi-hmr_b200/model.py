@@ -44,7 +44,7 @@ DEFAULT_PERSONS_PER_IMAGE = 16
 class _Config(ctypes.Structure):
     _fields_ = [(n, c_int) for n in ("arch", "img_size", "max_batch", "max_persons", "xat_depth",
                                      "xat_num_heads", "num_betas", "person_center_idx", "num_verts",
-                                     "refine_central")]
+                                     "refine_central", "head", "xat_dim", "xat_mlp_dim", "num_joints")]
 
 
 _OUT_FIELDS = ("scores_map", "count", "det_idx", "det_score", "offset", "loc", "dist_pp", "dist", "rotmat",

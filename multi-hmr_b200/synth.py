@@ -41,18 +41,7 @@ def _randn(g, *shape, std=1.0):
     return torch.randn(*shape, generator=g) * std
 
 
-def make_state_dict(backbone: str = "dinov2_vitl14", img_size: int = 896, num_betas: int = 10,
-                    xat_depth: int = 2, xat_num_heads: int = 8, seed: int = 0,
-                    det_bias: float = -4.0) -> dict:
-    """Random-init weights with trained-like scales.  `det_bias` shifts the detection logit so that only a
-    few cells per image pass the 0.3 threshold."""
-    cfg = BACKBONES[backbone]
-    D, depth = cfg["embed_dim"], cfg["depth"]
-    C = D + CAMERA_EMBED_DIM
-    res = img_size // PATCH
-    g = _gen(seed)
-    sd = {}
-
+def _makers(sd, g):
     def lin(name, out_f, in_f, std=0.02, bias=True, bias_std=0.02):
         sd[name + ".weight"] = _randn(g, out_f, in_f, std=std)
         if bias:
@@ -62,7 +51,14 @@ def make_state_dict(backbone: str = "dinov2_vitl14", img_size: int = 896, num_be
         sd[name + ".weight"] = 1.0 + _randn(g, dim, std=0.1)
         sd[name + ".bias"] = _randn(g, dim, std=0.05)
 
-    e = "backbone.encoder."
+    return lin, ln
+
+
+def _backbone_weights(sd, g, backbone, e):
+    """DINOv2 hub-model weights under the prefix `e` (the random stream is consumed in a fixed order)."""
+    cfg = BACKBONES[backbone]
+    D, depth = cfg["embed_dim"], cfg["depth"]
+    lin, ln = _makers(sd, g)
     sd[e + "cls_token"] = _randn(g, 1, 1, D, std=0.02)
     sd[e + "pos_embed"] = _randn(g, 1, 1 + 37 * 37, D, std=0.02)
     sd[e + "mask_token"] = torch.zeros(1, D)
@@ -79,6 +75,21 @@ def make_state_dict(backbone: str = "dinov2_vitl14", img_size: int = 896, num_be
         lin(b + "mlp.fc2", D, 4 * D)
         sd[b + "ls2.gamma"] = 0.05 + 0.95 * torch.rand(D, generator=g)
     ln(e + "norm", D)
+
+
+def make_state_dict(backbone: str = "dinov2_vitl14", img_size: int = 896, num_betas: int = 10,
+                    xat_depth: int = 2, xat_num_heads: int = 8, seed: int = 0,
+                    det_bias: float = -4.0) -> dict:
+    """Random-init weights with trained-like scales.  `det_bias` shifts the detection logit so that only a
+    few cells per image pass the 0.3 threshold."""
+    cfg = BACKBONES[backbone]
+    D = cfg["embed_dim"]
+    C = D + CAMERA_EMBED_DIM
+    res = img_size // PATCH
+    g = _gen(seed)
+    sd = {}
+    lin, ln = _makers(sd, g)
+    _backbone_weights(sd, g, backbone, "backbone.encoder.")
 
     lin("mlp_classif.0", D, D)
     lin("mlp_classif.2", 1, D, std=0.07)
@@ -249,3 +260,148 @@ def make_forced_idx(batch: int, res: int, persons_per_image, seed: int = 0):
         xs += (cells % res).tolist()
     t = lambda v: torch.tensor(v, dtype=torch.int64)
     return (t(bs), t(ys), t(xs), torch.zeros(len(bs), dtype=torch.int64))
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Anny variant (reference multi_hmr_anny/): state dict of `Multi_HMR` and an Anny-like body model
+# ------------------------------------------------------------------------------------------------------------------
+ANNY_NUM_JOINTS = 163
+ANNY_NUM_BETAS = 11
+ANNY_PHENOTYPES = ["gender", "age", "muscle", "weight", "height", "proportions", "cupsize", "firmness",
+                   "african", "asian", "caucasian"]
+ANNY_HEAD_BONE = 9
+
+
+def sincos_pos_embed_2d(dim: int, grid: int) -> torch.Tensor:
+    """[grid*grid, dim] fixed 2-D sine-cosine table (MAE / CroCo convention): the first half of the channels encodes
+    the row index, the second half the column index; each half is [sin(pos w) | cos(pos w)] with
+    w_i = 10000^(-i / (dim/4)).  Row n = y * grid + x.  Computed in float64, stored as float32."""
+    q = dim // 4
+    omega = 1.0 / 10000 ** (torch.arange(q, dtype=torch.float64) / q)
+    ys, xs = torch.meshgrid(torch.arange(grid, dtype=torch.float64), torch.arange(grid, dtype=torch.float64),
+                            indexing="ij")
+
+    def enc(pos):
+        a = pos.reshape(-1, 1) * omega[None]
+        return torch.cat([torch.sin(a), torch.cos(a)], 1)
+
+    return torch.cat([enc(ys), enc(xs)], 1).float()
+
+
+def make_anny_state_dict(backbone: str = "dinov2_vitl14", img_size: int = 672, xat_dim: int = 512,
+                         xat_depth: int = 8, xat_heads: int = 16, xat_mlp_dim: int = 2048, seed: int = 0,
+                         det_bias: float = -4.0, fov_deg: float = 60.0, dist_m: float = 3.5) -> dict:
+    """`Multi_HMR.state_dict()` keys of an Anny checkpoint (encoder.backbone.*, encoder.mlp_det / mlp_fov_unique,
+    dec_to_token, decoder.transformer.layers.*, mlp_offset / pose / shape / dist, useful_rotmat, init_body_pose,
+    dec_pos_emb, encoder.fov_max, eye).  The output biases put the regressed field of view near `fov_deg` and the
+    distances near `dist_m`; `det_bias` shifts the detection logit as in make_state_dict."""
+    cfg = BACKBONES[backbone]
+    D = cfg["embed_dim"]
+    res = img_size // PATCH
+    J = ANNY_NUM_JOINTS
+    g = _gen(seed + 1000)
+    sd = {}
+    lin, ln = _makers(sd, g)
+    _backbone_weights(sd, g, backbone, "encoder.backbone.")
+    lin("encoder.mlp_det.0", D, D)
+    lin("encoder.mlp_det.2", 1, D, std=0.07)
+    sd["encoder.mlp_det.2.bias"] = torch.full((1,), float(det_bias))
+    lin("encoder.mlp_fov_unique.0", D, D)
+    lin("encoder.mlp_fov_unique.2", 1, D, std=0.02)
+    s = fov_deg / 180.0
+    sd["encoder.mlp_fov_unique.2.bias"] = torch.full((1,), math.log(s / (1.0 - s)))
+    sd["encoder.fov_max"] = torch.tensor([math.pi])
+    sd["dec_pos_emb"] = sincos_pos_embed_2d(xat_dim, res)
+    lin("dec_to_token", xat_dim, D)
+    inner = xat_heads * 32
+    for l in range(xat_depth):
+        p = f"decoder.transformer.layers.{l}."
+        ln(p + "0.norm", xat_dim)
+        lin(p + "0.fn.to_qkv", 3 * inner, xat_dim, bias=False, std=0.03)
+        lin(p + "0.fn.to_out.0", xat_dim, inner)
+        ln(p + "1.norm", xat_dim)
+        lin(p + "1.fn.to_kv", 2 * inner, xat_dim, bias=False, std=0.03)
+        lin(p + "1.fn.to_q", inner, xat_dim, bias=False, std=0.03)
+        lin(p + "1.fn.to_out.0", xat_dim, inner)
+        ln(p + "2.norm", xat_dim)
+        lin(p + "2.fn.net.0", xat_mlp_dim, xat_dim)
+        lin(p + "2.fn.net.3", xat_dim, xat_mlp_dim)
+    lin("mlp_offset.0", xat_dim, xat_dim)
+    lin("mlp_offset.2", 2, xat_dim, std=0.02)
+    lin("mlp_pose.0", xat_dim, xat_dim + 6 * J)
+    lin("mlp_pose.2", 6 * J, xat_dim, std=0.005)
+    lin("mlp_shape.0", xat_dim, xat_dim)
+    lin("mlp_shape.2", ANNY_NUM_BETAS, xat_dim, std=0.05)
+    lin("mlp_dist.0", xat_dim, xat_dim)
+    lin("mlp_dist.2", 1, xat_dim, std=0.01)
+    focal = (img_size / 2) / math.tan(math.radians(fov_deg) / 2)
+    sd["mlp_dist.2.bias"] = torch.full((1,), math.log(focal / dist_m))
+    sd["useful_rotmat"] = (torch.rand(1, J, generator=g) < 0.6).float()
+    # 6-D initial rotations in the layout rot6d.reshape(3, 2) reads (columns = the two basis vectors): a
+    # seeded root rotation, identities elsewhere
+    R0 = _rotation(_randn(g, 3, std=0.8))
+    init = torch.eye(3).reshape(1, 3, 3).repeat(J, 1, 1)
+    init[0] = R0
+    sd["init_body_pose"] = init[:, :, :2].flatten(1).reshape(1, -1)
+    sd["eye"] = torch.eye(3).unsqueeze(0)
+    return sd
+
+
+def _rotation(rv: torch.Tensor) -> torch.Tensor:
+    ang = rv.norm().clamp_min(1e-8)
+    ax = rv / ang
+    Kx = torch.tensor([[0.0, -ax[2], ax[1]], [ax[2], 0.0, -ax[0]], [-ax[1], ax[0], 0.0]])
+    return torch.eye(3) + torch.sin(ang) * Kx + (1 - torch.cos(ang)) * (Kx @ Kx)
+
+
+class AnnyLikeBodyModel(torch.nn.Module):
+    """A deterministic stand-in for the `anny` package's full-body model with the interface Multi_HMR uses
+    (multi_hmr_anny/multi_hmr.py:70-77, :169-182): `bone_labels` (163, with 'head'), `phenotype_labels`, `faces`,
+    `set_skinning_method`, and `forward(pose_parameters=[P,163,4,4], phenotype_kwargs={name: [P]})` returning
+    `vertices` [P,V,3], `bone_poses` [P,163,4,4] and `blendshape_coeffs` [P,6].  Its arithmetic is a plain
+    phenotype blendshape + forward kinematics + linear blend skinning on seeded data; it is NOT the Anny model."""
+
+    SHAPE_KEYS = ("age", "gender", "weight", "height", "muscle", "proportions")
+
+    def __init__(self, num_verts: int = 14000, seed: int = 0):
+        super().__init__()
+        g = _gen(seed + 2000)
+        J, V = ANNY_NUM_JOINTS, num_verts
+        parents = [-1] + [int(torch.randint(0, j, (1,), generator=g)) for j in range(1, J)]
+        self.register_buffer("parents", torch.tensor(parents, dtype=torch.int64))
+        self.register_buffer("joints_rest", _randn(g, J, 3) * torch.tensor([0.2, 0.5, 0.1]))
+        self.register_buffer("joint_dirs", _randn(g, len(self.SHAPE_KEYS), J, 3, std=0.02))
+        self.register_buffer("v_template", _randn(g, V, 3) * torch.tensor([0.25, 0.6, 0.12]))
+        self.register_buffer("shape_dirs", _randn(g, len(self.SHAPE_KEYS), V, 3, std=0.03))
+        ids = torch.randint(0, J, (V, 4), generator=g)
+        w = torch.rand(V, 4, generator=g) + 0.05
+        W = torch.zeros(V, J)
+        W.scatter_add_(1, ids, w / w.sum(1, keepdim=True))
+        self.register_buffer("weights", W)
+        self.faces = torch.randint(0, V, (2 * V, 3), generator=g)
+        self.bone_labels = [f"bone_{j:03d}" for j in range(J)]
+        self.bone_labels[ANNY_HEAD_BONE] = "head"
+        self.phenotype_labels = list(ANNY_PHENOTYPES)
+        self.skinning_method = "lbs"
+
+    def set_skinning_method(self, name):
+        assert name == "lbs"
+        self.skinning_method = name
+
+    def forward(self, pose_parameters, phenotype_kwargs):
+        P = pose_parameters.shape[0]
+        c = torch.stack([phenotype_kwargs[k] for k in self.SHAPE_KEYS], 1) - 0.5          # [P, 6]
+        Jr = self.joints_rest[None] + torch.einsum("pk,kjc->pjc", c, self.joint_dirs)     # [P, J, 3]
+        vs = self.v_template[None] + torch.einsum("pk,kvc->pvc", c, self.shape_dirs)      # [P, V, 3]
+        G = [None] * ANNY_NUM_JOINTS
+        for j in range(ANNY_NUM_JOINTS):
+            T = pose_parameters[:, j].clone()
+            p = int(self.parents[j])
+            T[:, :3, 3] = Jr[:, j] - (Jr[:, p] if p >= 0 else 0.0)
+            G[j] = T if p < 0 else G[p] @ T
+        G = torch.stack(G, 1)                                                             # [P, J, 4, 4]
+        A = G.clone()
+        A[:, :, :3, 3] = G[:, :, :3, 3] - torch.einsum("pjab,pjb->pja", G[:, :, :3, :3], Jr)
+        Tv = torch.einsum("vj,pjab->pvab", self.weights, A)                               # [P, V, 4, 4]
+        verts = torch.einsum("pvab,pvb->pva", Tv[..., :3, :3], vs) + Tv[..., :3, 3]
+        return {"vertices": verts, "bone_poses": G, "blendshape_coeffs": c.reshape(P, -1)}
