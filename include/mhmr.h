@@ -78,6 +78,72 @@ int mhmr_op_attention(const void* qkv, int64_t ld_qkv, void* out, int64_t ldo, i
  * host derives from that function the output is bit-identical, and the upload is 4x smaller.  W % 4 == 0. */
 int mhmr_op_normalize_u8(const void* img_u8, const float* lut, float* out, int B, int H, int W, void* stream);
 
+/* Person-decoder kernels (the per-person path after the backbone), each the engine's own launcher behind a thin
+ * validating entry.  All pointers are device pointers; `count` is a device int32 holding the person count
+ * (<= max_persons), read on the device as in the engine: grids are sized for max_persons and exit early, and rows
+ * >= count are not written.  fp32 throughout. */
+
+/* out[p, n] = resid[p, n] + act(LN(x[p, :K]) . W[n, :K] + bias[n]) for p < count; the skinny Linear of the HPH and
+ * the regressors.  LN (ln_g, ln_b, eps; both or neither, K % 4 == 0) is applied to the input row, act 0 none,
+ * 1 ReLU, 2 erf GELU; bias, LN and resid are nullable, out may equal resid (in-place residual update).
+ * W pitch ldw >= K rounded up to 4, multiple of 4; its padding columns are multiplied by zero, so must be finite.
+ * ldx % 4 == 0: 128-bit loads (ldx >= K rounded to 4); otherwise scalar loads.  cols: 16 or 32 output columns per
+ * CTA (2 or 4 per warp), 0 lets the device's SM count decide as the engine does. */
+int mhmr_op_skinny_linear(const float* x, int ldx, const int* count, int max_persons, int K, const float* W, int ldw,
+                          const float* bias, int Nout, const float* ln_g, const float* ln_b, float ln_eps, int act,
+                          const float* resid, int ldr, float* out, int ldo, int cols, void* stream);
+
+/* HPH self-attention among the persons of each image (cross_attn_transformer.py:129-159, heads of 32,
+ * softmax(q k^T / sqrt(32)) v): qkv [P, ld] = q | k | v column blocks of heads * 32; persons sorted by image,
+ * det_b[p] their image, img_off[b] .. img_off[b + 1] the persons of image b. */
+int mhmr_op_hph_self_attn(const float* qkv, int ld, const int* det_b, const int* img_off, const int* count,
+                          int max_persons, int heads, float* out, int ldo, void* stream);
+
+/* HPH cross-attention (cross_attn_transformer.py:185-205): person p attends to the N rows of image det_b[p] of
+ * KV [B * N, ldkv], keys at columns k_col + h * 32, values at v_col + h * 32 (multiples of 4). */
+int mhmr_op_hph_cross_attn(const float* q, int ldq, const float* KV, int64_t ldkv, int k_col, int v_col,
+                           const int* det_b, const int* count, int max_persons, int heads, int N, float* out, int ldo,
+                           void* stream);
+
+/* Detection (model.py:145-149, :612-638): scores_out = scores * (maxpool_k(scores) == scores) (k in [1, 15]; padding
+ * (k - 1) / 2, 1 for k = 2, 2 for k = 4), then the cells with scores_out >= thresh in (b, y, x) order: the first
+ * max_persons of them in det_b / det_y / det_x / det_score, their true number in count, min(count, max_persons) in
+ * count_clamped, and img_off[b] (B + 1 entries) = first kept person of image b. */
+int mhmr_op_detect(const float* scores, int B, int res, int nms_k, float thresh, int max_persons, float* scores_out,
+                   int* det_b, int* det_y, int* det_x, float* det_score, int* count, int* count_clamped, int* img_off,
+                   void* stream);
+
+/* SMPL-X per-person outputs (utils/humans.py:12-22, model.py:189-203, :272-275, :291, blocks/smpl_layer.py:123):
+ * dec [P, ld_dec] = pose6 (318) | betas (num_betas) | cam (3) | expression (10); K [B, 3, 3] (inverted inside);
+ * focal_norm = img_size / (2 tan 30 deg).  Writes rotmat [P, 53, 3, 3], rotvec [P, 53, 3], shape, expr, dist_pp,
+ * dist, loc [P, 2], transl [P, 3], K_det [P, 3, 3].  Allocates a temporary and synchronises the stream. */
+int mhmr_op_person_post(const float* dec, int ld_dec, int num_betas, const float* offset, const float* K, int B,
+                        const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
+                        float focal_norm, float* rotmat, float* rotvec, float* shape, float* expr, float* dist_pp,
+                        float* dist, float* loc, float* transl, float* K_det, void* stream);
+
+/* Anny camera and per-person outputs (encoder.py:50-56, multi_hmr.py:133-175): from hid [B, D] (the hidden layer of
+ * mlp_fov_unique) fov [B], K_regressed and K_use [B, 3, 3] (K if given, else K_regressed); then per person the 6D
+ * rows rot6d [P, ld6] (J joints) -> rotmat [P, J, 3, 3] blended with the identity by useful [J], rotmat_homo
+ * [P, J, 4, 4], rotvec, dist = K_use[0,0] / max(exp(dist_pp), 1e-5), loc, transl, K_det, and shape [P, num_betas]
+ * replaced by its sigmoid in place.  Allocates a temporary and synchronises the stream. */
+int mhmr_op_anny_person_post(const float* hid, int D, const float* w2, const float* b2, const float* fov_max,
+                             const float* K, int B, int img_size, float* fov, float* K_regressed, float* K_use,
+                             const float* rot6d, int ld6, int J, const float* useful, float* shape, int num_betas,
+                             const float* offset, const float* dist_pp, const int* det_b, const int* det_y,
+                             const int* det_x, const int* count, int max_persons, float* rotmat, float* rotmat_homo,
+                             float* rotvec, float* dist, float* loc, float* transl, float* K_det, void* stream);
+
+/* Central-stream refinement (DESIGN.md §3) of `count` rows x [max_persons, D] in place, through `depth` dinov2
+ * blocks: x += ls1 * (Wproj . O16[l][rowidx[p]] + bproj);  x += ls2 * (Wfc2 . gelu(Wfc1 . LN2(x) + bfc1) + bfc2)
+ * (LayerNorm eps 1e-6).  Weights stacked per layer: Wproj [depth, D, D], Wfc1 [depth, 4D, D], Wfc2 [depth, D, 4D],
+ * vectors [depth, D] (bfc1 [depth, 4D]); O16 fp16 [depth, rows_o16, D].  D % 4 == 0.  Bit-reproducible.
+ * Allocates its temporaries and synchronises the stream. */
+int mhmr_op_refine_chain(int depth, int D, const int* count, int max_persons, const float* Wproj, const float* bproj,
+                         const float* ls1, const float* ln2_g, const float* ln2_b, const float* Wfc1, const float* bfc1,
+                         const float* Wfc2, const float* bfc2, const float* ls2, const void* O16, int64_t rows_o16,
+                         const int* rowidx, float* x, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Engine: the whole `Model.forward(x, K)` path (reference model.py:205-349) behind one handle
  * ---------------------------------------------------------------------------------------------- */

@@ -3,7 +3,13 @@
 #include "gemm_tc.cuh"
 #include "kernels.cuh"
 
+#include <vector>
+
 using namespace mhmr;
+
+namespace {
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+}  // namespace
 
 extern "C" {
 
@@ -89,6 +95,143 @@ int mhmr_op_attention(const void* qkv, int64_t ld_qkv, void* out, int64_t ldo, i
 int mhmr_op_normalize_u8(const void* img_u8, const float* lut, float* out, int B, int H, int W, void* stream) {
   MHMR_REQUIRE(img_u8 != nullptr && lut != nullptr && out != nullptr, "null argument");
   return normalize_u8(static_cast<const uint8_t*>(img_u8), lut, out, B, H, W, static_cast<cudaStream_t>(stream));
+}
+
+// ---- person-decoder kernels (head.cu, refine.cu): the launchers the engine calls, unchanged ----------------------
+
+int mhmr_op_skinny_linear(const float* x, int ldx, const int* count, int max_persons, int K, const float* W, int ldw,
+                          const float* bias, int Nout, const float* ln_g, const float* ln_b, float ln_eps, int act,
+                          const float* resid, int ldr, float* out, int ldo, int cols, void* stream) {
+  MHMR_REQUIRE(x && count && W && out, "null argument");
+  MHMR_REQUIRE(max_persons >= 0 && K >= 1 && Nout >= 1 && act >= 0 && act <= 2, "skinny_linear: bad sizes or act");
+  MHMR_REQUIRE(ldo >= Nout && (resid == nullptr || ldr >= Nout), "skinny_linear: output pitches must cover Nout");
+  MHMR_REQUIRE((ln_g == nullptr) == (ln_b == nullptr), "skinny_linear: LayerNorm needs both ln_g and ln_b");
+  MHMR_REQUIRE(aligned16(W) && (ldx % 4 != 0 || aligned16(x)) && (ln_g == nullptr || (aligned16(ln_g) && aligned16(ln_b))),
+               "skinny_linear: W, LayerNorm vectors and x (when ldx % 4 == 0) must be 16-byte aligned");
+  if (max_persons == 0) return MHMR_OK;
+  return skinny_linear_ex(x, ldx, cols, count, max_persons, K, W, ldw, bias, Nout, ln_g, ln_b, ln_eps, act, resid, ldr,
+                          out, ldo, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_hph_self_attn(const float* qkv, int ld, const int* det_b, const int* img_off, const int* count,
+                          int max_persons, int heads, float* out, int ldo, void* stream) {
+  MHMR_REQUIRE(qkv && det_b && img_off && count && out, "null argument");
+  MHMR_REQUIRE(max_persons >= 0 && heads >= 1 && ld >= 3 * 32 * heads && ldo >= 32 * heads,
+               "hph_self_attn: pitches must cover 3 * heads * 32 (qkv) and heads * 32 (out)");
+  if (max_persons == 0) return MHMR_OK;
+  return hph_self_attn(qkv, ld, det_b, img_off, count, max_persons, heads, out, ldo, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_hph_cross_attn(const float* q, int ldq, const float* KV, int64_t ldkv, int k_col, int v_col,
+                           const int* det_b, const int* count, int max_persons, int heads, int N, float* out, int ldo,
+                           void* stream) {
+  MHMR_REQUIRE(q && KV && det_b && count && out, "null argument");
+  MHMR_REQUIRE(max_persons >= 0 && heads >= 1 && N >= 1 && ldq >= 32 * heads && ldo >= 32 * heads && k_col >= 0 &&
+                   v_col >= 0 && k_col + 32 * heads <= ldkv && v_col + 32 * heads <= ldkv,
+               "hph_cross_attn: bad sizes or column offsets");
+  MHMR_REQUIRE(aligned16(KV), "hph_cross_attn: KV must be 16-byte aligned");
+  if (max_persons == 0) return MHMR_OK;
+  return hph_cross_attn(q, ldq, KV, ldkv, k_col, v_col, det_b, count, max_persons, heads, N, out, ldo,
+                        static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_detect(const float* scores, int B, int res, int nms_k, float thresh, int max_persons, float* scores_out,
+                   int* det_b, int* det_y, int* det_x, float* det_score, int* count, int* count_clamped, int* img_off,
+                   void* stream) {
+  MHMR_REQUIRE(scores && scores_out && det_b && det_y && det_x && det_score && count && count_clamped && img_off,
+               "null argument");
+  MHMR_REQUIRE(scores != scores_out, "detect: scores_out must not alias scores (neighbours are read while writing)");
+  MHMR_REQUIRE(B >= 1 && res >= 1 && max_persons >= 0, "detect: bad sizes");
+  return nms_compact(scores, scores_out, B, res, nms_k, thresh, max_persons, det_b, det_y, det_x, det_score, count,
+                     count_clamped, img_off, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_person_post(const float* dec, int ld_dec, int num_betas, const float* offset, const float* K, int B,
+                        const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
+                        float focal_norm, float* rotmat, float* rotvec, float* shape, float* expr, float* dist_pp,
+                        float* dist, float* loc, float* transl, float* K_det, void* stream) {
+  MHMR_REQUIRE(dec && offset && K && det_b && det_y && det_x && count && rotmat && rotvec && shape && expr && dist_pp &&
+                   dist && loc && transl && K_det, "null argument");
+  MHMR_REQUIRE(B >= 1 && max_persons >= 0 && num_betas >= 1 && num_betas <= 32 && ld_dec >= 318 + num_betas + 13,
+               "person_post: bad sizes (num_betas in [1, 32], decoder row = 318 + num_betas + 3 + 10)");
+  if (max_persons == 0) return MHMR_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  float* Kinv = nullptr;
+  auto run = [&]() -> int {
+    MHMR_CUDA_CHECK(cudaMalloc(&Kinv, static_cast<size_t>(B) * 9 * sizeof(float)));
+    int r = invert_K(K, Kinv, B, st);
+    if (r != MHMR_OK) return r;
+    return person_post(dec, ld_dec, num_betas, offset, K, Kinv, det_b, det_y, det_x, count, max_persons, focal_norm,
+                       rotmat, rotvec, shape, expr, dist_pp, dist, loc, transl, K_det, st);
+  };
+  const int rc = run();
+  cudaStreamSynchronize(st);
+  cudaFree(Kinv);
+  return rc;
+}
+
+int mhmr_op_anny_person_post(const float* hid, int D, const float* w2, const float* b2, const float* fov_max,
+                             const float* K, int B, int img_size, float* fov, float* K_regressed, float* K_use,
+                             const float* rot6d, int ld6, int J, const float* useful, float* shape, int num_betas,
+                             const float* offset, const float* dist_pp, const int* det_b, const int* det_y,
+                             const int* det_x, const int* count, int max_persons, float* rotmat, float* rotmat_homo,
+                             float* rotvec, float* dist, float* loc, float* transl, float* K_det, void* stream) {
+  MHMR_REQUIRE(hid && w2 && b2 && fov_max && fov && K_regressed && K_use && rot6d && useful && shape && offset &&
+                   dist_pp && det_b && det_y && det_x && count && rotmat && rotmat_homo && rotvec && dist && loc &&
+                   transl && K_det, "null argument");
+  MHMR_REQUIRE(B >= 1 && D >= 1 && img_size >= 1 && J >= 1 && ld6 >= 6 * J && num_betas >= 0 && max_persons >= 0,
+               "anny_person_post: bad sizes");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  float* Kinv = nullptr;
+  auto run = [&]() -> int {
+    MHMR_CUDA_CHECK(cudaMalloc(&Kinv, static_cast<size_t>(B) * 9 * sizeof(float)));
+    int r = anny_camera(hid, D, w2, b2, fov_max, K, B, img_size, fov, K_regressed, K_use, Kinv, st);
+    if (r != MHMR_OK || max_persons == 0) return r;
+    return anny_person_post(rot6d, ld6, J, useful, shape, num_betas, offset, dist_pp, K_use, Kinv, det_b, det_y, det_x,
+                            count, max_persons, rotmat, rotmat_homo, rotvec, dist, loc, transl, K_det, st);
+  };
+  const int rc = run();
+  cudaStreamSynchronize(st);
+  cudaFree(Kinv);
+  return rc;
+}
+
+int mhmr_op_refine_chain(int depth, int D, const int* count, int max_persons, const float* Wproj, const float* bproj,
+                         const float* ls1, const float* ln2_g, const float* ln2_b, const float* Wfc1, const float* bfc1,
+                         const float* Wfc2, const float* bfc2, const float* ls2, const void* O16, int64_t rows_o16,
+                         const int* rowidx, float* x, void* stream) {
+  MHMR_REQUIRE(count && Wproj && bproj && ls1 && ln2_g && ln2_b && Wfc1 && bfc1 && Wfc2 && bfc2 && ls2 && O16 && rowidx &&
+                   x, "null argument");
+  MHMR_REQUIRE(depth >= 1 && D >= 4 && D % 4 == 0 && max_persons >= 0 && rows_o16 >= 1, "refine_chain: bad sizes");
+  // the chain stages 8 hidden rows of 4D floats plus a 8 x 256 reduction buffer in (at most 200 KB of) shared memory
+  MHMR_REQUIRE((8 * 4 * D + 8 * 256) * 4 <= 200 * 1024, "refine_chain: D must be at most 1536");
+  MHMR_REQUIRE(aligned16(x) && aligned16(O16) && aligned16(Wproj) && aligned16(Wfc1) && aligned16(Wfc2) &&
+                   aligned16(ln2_g) && aligned16(ln2_b), "refine_chain: x, O16, weights and ln2 must be 16-byte aligned");
+  if (max_persons == 0) return MHMR_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t DD = static_cast<int64_t>(D) * D;
+  std::vector<RefineLayer> rl(depth);
+  for (int l = 0; l < depth; ++l)
+    rl[l] = RefineLayer{static_cast<const __half*>(O16) + l * rows_o16 * D, Wproj + l * DD, bproj + l * D, ls1 + l * D,
+                        ln2_g + l * D, ln2_b + l * D, Wfc1 + l * 4 * DD, bfc1 + l * 4 * D, Wfc2 + l * 4 * DD,
+                        bfc2 + l * D, ls2 + l * D};
+  RefineLayer* layers = nullptr;
+  float *term = nullptr, *h = nullptr;
+  unsigned int* barrier = nullptr;
+  auto run = [&]() -> int {
+    MHMR_CUDA_CHECK(cudaMalloc(&layers, rl.size() * sizeof(RefineLayer)));
+    MHMR_CUDA_CHECK(cudaMalloc(&term, static_cast<size_t>(depth) * max_persons * D * sizeof(float)));
+    MHMR_CUDA_CHECK(cudaMalloc(&h, static_cast<size_t>(max_persons) * 4 * D * sizeof(float)));
+    MHMR_CUDA_CHECK(cudaMalloc(&barrier, sizeof(unsigned int)));
+    MHMR_CUDA_CHECK(cudaMemcpyAsync(layers, rl.data(), rl.size() * sizeof(RefineLayer), cudaMemcpyHostToDevice, st));
+    int r = refine_proj_terms(layers, depth, rowidx, count, D, max_persons, term, st);
+    if (r != MHMR_OK) return r;
+    return refine_mlp_chain(layers, depth, count, D, max_persons, term, x, h, barrier, st);
+  };
+  const int rc = run();
+  cudaStreamSynchronize(st);
+  cudaFree(layers); cudaFree(term); cudaFree(h); cudaFree(barrier);
+  return rc;
 }
 
 }  // extern "C"

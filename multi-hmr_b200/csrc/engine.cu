@@ -657,9 +657,8 @@ int refine_streams(mhmr_engine* e, const ImgSrc& x, const int* det_b, const int*
   LAUNCH(MHMR_CAT_REFINE, refine_prepare(x.f32, x.u8, x.lut, e->cfg.img_size, e->rowadd, D, det_b, det_y, det_x, count, Pm, e->res,
                                          n_cls, e->cls_pos, n_cls > 0 ? rows : nullptr, e->r_rowidx, e->r_patch, 592, e->r_x, st));
   const int* rc = n_cls > 0 ? rows : count;
-  SkinnyExtra none;
-  LAUNCH(MHMR_CAT_REFINE, skinny_linear_ex(e->r_patch, 592, none, rc, Rm, 588, e->Wpatch32, 588, nullptr, D, nullptr,
-                                           nullptr, 0.f, 0, e->r_x, D, e->r_x, D, st));
+  LAUNCH(MHMR_CAT_REFINE, skinny_linear(e->r_patch, 592, rc, Rm, 588, e->Wpatch32, 588, nullptr, D, nullptr, nullptr, 0.f, 0,
+                                        e->r_x, D, e->r_x, D, st));
   LAUNCH(MHMR_CAT_REFINE, refine_proj_terms(e->r_layers, e->depth, e->r_rowidx, rc, D, Rm, e->r_term, st));
   LAUNCH(MHMR_CAT_REFINE, refine_mlp_chain(e->r_layers, e->depth, rc, D, Rm, e->r_term, e->r_x, e->r_h, e->r_barrier, st));
   return MHMR_OK;

@@ -332,10 +332,9 @@ __global__ void kv_add_rows_kernel(float* __restrict__ KV, int64_t ldkv, const f
 }
 
 // ----------------------------------------------------------------------------------------------
-// Skinny linear: out[p, n] = resid[p, n] + gamma[n] * act( LN?(x[p, :]) . W[n, :] + bias[n] ),  p < *count.
-// fp32 weights streamed once per chunk of 8 persons (from L2 after the first chunk).  The input rows are
-// either fp32 rows of `x` or fp16 rows `x16[rowidx[p], :]` gathered from a token matrix (central-stream
-// refinement: rows of the attention output of the backbone's bulk pass).
+// Skinny linear: out[p, n] = resid[p, n] + act( LN?(x[p, :]) . W[n, :] + bias[n] ),  p < *count.
+// fp32 weights streamed once per chunk of 8 persons (from L2 after the first chunk).  out may be resid (the
+// residual updates of the HPH): each element is read and then written by the same thread.
 //   grid = (ceil(Nout / (8 CPW)), ceil(max_persons / 8)), block = 256: 8 warps x CPW output columns each.
 //   The 8 input rows are staged K-tile by K-tile (1024 floats per person, 32 KB static smem, 128-bit loads, LayerNorm
 //   applied on the way in from per-row statistics computed once) so that several CTAs share an SM whatever K is;
@@ -349,12 +348,10 @@ constexpr int kSkinnyKT = 1024;
 
 template <int CPW>
 __global__ void __launch_bounds__(256)
-skinny_linear_kernel(const float* __restrict__ x, int ldx, const __half* __restrict__ x16, int64_t ldx16,
-                     const int* __restrict__ rowidx, const int* __restrict__ count, int K,
+skinny_linear_kernel(const float* __restrict__ x, int ldx, const int* __restrict__ count, int K,
                      const float* __restrict__ W, int ldw, const float* __restrict__ bias, int Nout,
                      const float* __restrict__ ln_g, const float* __restrict__ ln_b, float ln_eps, int act,
-                     const float* __restrict__ gamma, const float* __restrict__ resid, int ldr,
-                     float* __restrict__ out, int ldo) {
+                     const float* resid, int ldr, float* out, int ldo) {
   __shared__ __align__(16) float xs[kSkinnyPT][kSkinnyKT];
   __shared__ float stats[kSkinnyPT][2];
   constexpr int COLS = 8 * CPW;
@@ -400,7 +397,7 @@ skinny_linear_kernel(const float* __restrict__ x, int ldx, const __half* __restr
   for (int c = 0; c < CPW; ++c)
 #pragma unroll
     for (int j = 0; j < kSkinnyPT; ++j) acc[c][j] = 0.f;
-  const bool vec_x = (x16 != nullptr) || ((ldx & 3) == 0);  // 128-bit loads need 16-byte aligned rows
+  const bool vec_x = (ldx & 3) == 0;  // 128-bit loads need 16-byte aligned rows
 
   for (int k0 = 0; k0 < Kp; k0 += kSkinnyKT) {
     const int kt = min(kSkinnyKT, Kp - k0);  // multiple of 4
@@ -410,21 +407,14 @@ skinny_linear_kernel(const float* __restrict__ x, int ldx, const __half* __restr
       const int j = idx / q4, q = idx - j * q4, k = k0 + 4 * q;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (j < np) {
-        if (x16 != nullptr) {
-          const uint2 pk = *reinterpret_cast<const uint2*>(x16 + static_cast<int64_t>(rowidx[p0 + j]) * ldx16 + k);
-          const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&pk.x));
-          const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&pk.y));
-          v = make_float4(a.x, a.y, b.x, b.y);
+        const float* src = x + static_cast<int64_t>(p0 + j) * ldx + k;
+        if (vec_x) {
+          v = *reinterpret_cast<const float4*>(src);
         } else {
-          const float* src = x + static_cast<int64_t>(p0 + j) * ldx + k;
-          if (vec_x) {
-            v = *reinterpret_cast<const float4*>(src);
-          } else {
-            v.x = src[0];
-            if (k + 1 < K) v.y = src[1];
-            if (k + 2 < K) v.z = src[2];
-            if (k + 3 < K) v.w = src[3];
-          }
+          v.x = src[0];
+          if (k + 1 < K) v.y = src[1];
+          if (k + 2 < K) v.z = src[2];
+          if (k + 3 < K) v.w = src[3];
         }
         if (ln_g != nullptr) {
           const float mean = stats[j][0], rstd = stats[j][1];
@@ -494,7 +484,6 @@ skinny_linear_kernel(const float* __restrict__ x, int ldx, const __half* __restr
     if (bias != nullptr) v += bias[n];
     if (act == 1) v = fmaxf(v, 0.f);
     if (act == 2) v = gelu_erf(v);
-    if (gamma != nullptr) v *= gamma[n];
     if (resid != nullptr) v += resid[static_cast<int64_t>(p0 + j) * ldr + n];
     out[static_cast<int64_t>(p0 + j) * ldo + n] = v;
   }
@@ -817,19 +806,18 @@ int kv_add_rows(float* KV, int64_t ldkv, const float* dKV, int ncols, const int*
   return MHMR_OK;
 }
 
-int skinny_linear_ex(const float* x, int ldx, const SkinnyExtra& ex, const int* count, int max_persons, int K,
-                     const float* W, int ldw, const float* bias, int Nout, const float* ln_g, const float* ln_b,
-                     float ln_eps, int act, const float* resid, int ldr, float* out, int ldo, cudaStream_t st) {
+int skinny_linear_ex(const float* x, int ldx, int cols, const int* count, int max_persons, int K, const float* W, int ldw,
+                     const float* bias, int Nout, const float* ln_g, const float* ln_b, float ln_eps, int act,
+                     const float* resid, int ldr, float* out, int ldo, cudaStream_t st) {
   const int Kp = (K + 3) & ~3;
   MHMR_REQUIRE(ldw % 4 == 0 && ldw >= Kp, "skinny_linear: weight pitch must be >= K rounded to 4");
-  MHMR_REQUIRE((x != nullptr) != (ex.x16 != nullptr), "skinny_linear: exactly one of x / x16");
-  MHMR_REQUIRE(ex.x16 == nullptr || (ex.rowidx != nullptr && ex.ldx16 % 4 == 0 && K % 4 == 0),
-               "skinny_linear: x16 needs row indices, a pitch and K that are multiples of 4");
-  MHMR_REQUIRE(x == nullptr || (ldx % 4 != 0) || ldx >= Kp, "skinny_linear: input pitch must cover K rounded to 4");
-  MHMR_REQUIRE(ln_g == nullptr || (x != nullptr && K % 4 == 0), "skinny_linear: LayerNorm needs fp32 rows, K % 4 == 0");
+  MHMR_REQUIRE(x != nullptr && ldx >= K && (ldx % 4 != 0 || ldx >= Kp),
+               "skinny_linear: input pitch must cover K (rounded to 4 when it is a multiple of 4)");
+  MHMR_REQUIRE(ln_g == nullptr || K % 4 == 0, "skinny_linear: LayerNorm needs K % 4 == 0");
+  MHMR_REQUIRE(cols == 0 || cols == 16 || cols == 32, "skinny_linear: cols must be 0 (pick), 16 or 32");
   // columns per warp: 4 (32 per CTA) by default, 2 when that leaves fewer CTAs than SMs for one 8-person chunk
-  int cpw = (ex.cols == 16) ? 2 : 4;
-  if (ex.cols <= 0 && (Nout + 31) / 32 < device_sm_count()) cpw = 2;
+  int cpw = (cols == 16) ? 2 : 4;
+  if (cols == 0 && (Nout + 31) / 32 < device_sm_count()) cpw = 2;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((Nout + 8 * cpw - 1) / (8 * cpw), (max_persons + kSkinnyPT - 1) / kSkinnyPT);
   cfg.blockDim = dim3(256);
@@ -841,11 +829,11 @@ int skinny_linear_ex(const float* x, int ldx, const SkinnyExtra& ex, const int* 
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
   if (cpw == 4) {
-    MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, skinny_linear_kernel<4>, x, ldx, ex.x16, ex.ldx16, ex.rowidx, count, K, W, ldw,
-                                       bias, Nout, ln_g, ln_b, ln_eps, act, ex.gamma, resid, ldr, out, ldo));
+    MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, skinny_linear_kernel<4>, x, ldx, count, K, W, ldw, bias, Nout, ln_g, ln_b,
+                                       ln_eps, act, resid, ldr, out, ldo));
   } else {
-    MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, skinny_linear_kernel<2>, x, ldx, ex.x16, ex.ldx16, ex.rowidx, count, K, W, ldw,
-                                       bias, Nout, ln_g, ln_b, ln_eps, act, ex.gamma, resid, ldr, out, ldo));
+    MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, skinny_linear_kernel<2>, x, ldx, count, K, W, ldw, bias, Nout, ln_g, ln_b,
+                                       ln_eps, act, resid, ldr, out, ldo));
   }
   return MHMR_OK;
 }
@@ -853,9 +841,8 @@ int skinny_linear_ex(const float* x, int ldx, const SkinnyExtra& ex, const int* 
 int skinny_linear(const float* x, int ldx, const int* count, int max_persons, int K, const float* W, int ldw,
                   const float* bias, int Nout, const float* ln_g, const float* ln_b, float ln_eps, int act,
                   const float* resid, int ldr, float* out, int ldo, cudaStream_t st) {
-  SkinnyExtra ex;
-  return skinny_linear_ex(x, ldx, ex, count, max_persons, K, W, ldw, bias, Nout, ln_g, ln_b, ln_eps, act, resid, ldr,
-                          out, ldo, st);
+  return skinny_linear_ex(x, ldx, 0, count, max_persons, K, W, ldw, bias, Nout, ln_g, ln_b, ln_eps, act, resid, ldr, out,
+                          ldo, st);
 }
 
 int hph_self_attn(const float* qkv, int ld, const int* det_b, const int* img_off, const int* count,

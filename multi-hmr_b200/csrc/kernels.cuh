@@ -61,17 +61,10 @@ int kv_add_rows(float* KV, int64_t ldkv, const float* dKV, int ncols, const int*
 int skinny_linear(const float* x, int ldx, const int* count, int max_persons, int K, const float* W, int ldw,
                   const float* bias, int Nout, const float* ln_g, const float* ln_b, float ln_eps, int act,
                   const float* resid, int ldr, float* out, int ldo, cudaStream_t st);
-// extras of the skinny linear: fp16 gathered input rows, LayerScale, columns per CTA (0 = pick for occupancy)
-struct SkinnyExtra {
-  const __half* x16 = nullptr;
-  int64_t ldx16 = 0;
-  const int* rowidx = nullptr;
-  const float* gamma = nullptr;
-  int cols = 0;
-};
-int skinny_linear_ex(const float* x, int ldx, const SkinnyExtra& ex, const int* count, int max_persons, int K,
-                     const float* W, int ldw, const float* bias, int Nout, const float* ln_g, const float* ln_b,
-                     float ln_eps, int act, const float* resid, int ldr, float* out, int ldo, cudaStream_t st);
+// cols: columns per CTA, 16 or 32 (2 or 4 per warp); 0 picks 16 when 32 would leave SMs idle for one person chunk
+int skinny_linear_ex(const float* x, int ldx, int cols, const int* count, int max_persons, int K, const float* W, int ldw,
+                     const float* bias, int Nout, const float* ln_g, const float* ln_b, float ln_eps, int act,
+                     const float* resid, int ldr, float* out, int ldo, cudaStream_t st);
 // ---- refine.cu: central-stream refinement (DESIGN.md §3) -----------------------------------------
 struct RefineLayer {
   const __half* O16;  // this block's attention output of the bulk pass [B*T, D]

@@ -151,7 +151,7 @@ constexpr int kChainThreads = 512;
 template <typename Epi>
 __device__ __forceinline__ void cta_linear(const float* __restrict__ W, int64_t ldw, int Nout, int K, int n0, int ngroups,
                                            const float* xs, int ldxs, float* red, int warp, int lane, Epi epi) {
-  const int slice = ((K / 8) + 3) & ~3;           // K slice of a warp (multiple of 4)
+  const int slice = ((K + 31) / 32) * 4;          // K slice of a warp: a multiple of 4, 8 slices cover K
   const int kw = warp & 7, team = warp >> 3;
   const int kbeg = kw * slice, kend = min(K, kbeg + slice);
   for (int g = team; g < ngroups; g += kChainThreads / 256) {

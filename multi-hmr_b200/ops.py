@@ -8,7 +8,7 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from ._lib import c_int, c_int64, check, ptr, stream_ptr
+from ._lib import c_float, c_int, c_int64, check, ptr, stream_ptr
 
 EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RELU_F16, EPI_LS_RESID_F32, EPI_ROWADD_F32, EPI_BIAS_F32 = range(6)
 
@@ -78,3 +78,145 @@ def attention(qkv, B, T, D, out=None):
                                c_int(T), c_int(D), stream_ptr())
     check(rc, "mhmr_op_attention")
     return out
+
+
+# ---- person-decoder kernels: `count` is a device int32 tensor [1] (<= max_persons), read on the device -----------
+def _f32(*ts):
+    for t in ts:
+        assert t is None or (t.dtype == torch.float32 and (t.dim() == 1 or t.stride(-1) == 1)), "fp32 rows expected"
+
+
+def _i32(*ts):
+    for t in ts:
+        assert t.dtype == torch.int32 and t.is_contiguous(), "int32 contiguous tensor expected"
+
+
+def skinny_linear(x, count, max_persons, K, w, out, bias=None, ln=None, act=0, resid=None, cols=0):
+    """out[p, :N] = resid[p] + act(LN(x[p, :K]) @ w[:, :K]^T + bias) for p < count, N = w.shape[0]; row pitches are
+    the tensors' strides.  ln = (gamma, beta, eps) or None; act 0 none, 1 ReLU, 2 erf GELU; out may be resid;
+    cols 16 / 32 columns per CTA, 0 = the engine's choice."""
+    _cuda(x, count, w, out, bias, resid)
+    _f32(x, w, out, bias, resid)
+    _i32(count)
+    g, b, eps = ln if ln is not None else (None, None, 0.0)
+    rc = _lib.load().mhmr_op_skinny_linear(
+        ptr(x), c_int(x.stride(0)), ptr(count), c_int(max_persons), c_int(K), ptr(w), c_int(w.stride(0)), ptr(bias),
+        c_int(w.shape[0]), ptr(g), ptr(b), c_float(eps), c_int(act), ptr(resid),
+        c_int(resid.stride(0) if resid is not None else 0), ptr(out), c_int(out.stride(0)), c_int(cols), stream_ptr())
+    check(rc, "mhmr_op_skinny_linear")
+    return out
+
+
+def hph_self_attn(qkv, det_b, img_off, count, max_persons, heads, out=None):
+    """qkv [P, >= 3 * heads * 32] -> out [P, heads * 32]: attention among the persons of each image."""
+    _cuda(qkv, det_b, img_off, count)
+    _f32(qkv)
+    _i32(det_b, img_off, count)
+    if out is None:
+        out = torch.zeros(max_persons, heads * 32, device=qkv.device)
+    rc = _lib.load().mhmr_op_hph_self_attn(ptr(qkv), c_int(qkv.stride(0)), ptr(det_b), ptr(img_off), ptr(count),
+                                           c_int(max_persons), c_int(heads), ptr(out), c_int(out.stride(0)), stream_ptr())
+    check(rc, "mhmr_op_hph_self_attn")
+    return out
+
+
+def hph_cross_attn(q, kv, k_col, v_col, det_b, count, max_persons, heads, N, out=None):
+    """q [P, >= heads * 32], kv [B * N, ldkv] -> out [P, heads * 32]: person p attends to image det_b[p]'s rows."""
+    _cuda(q, kv, det_b, count)
+    _f32(q, kv)
+    _i32(det_b, count)
+    if out is None:
+        out = torch.zeros(max_persons, heads * 32, device=q.device)
+    rc = _lib.load().mhmr_op_hph_cross_attn(ptr(q), c_int(q.stride(0)), ptr(kv), c_int64(kv.stride(0)), c_int(k_col),
+                                            c_int(v_col), ptr(det_b), ptr(count), c_int(max_persons), c_int(heads),
+                                            c_int(N), ptr(out), c_int(out.stride(0)), stream_ptr())
+    check(rc, "mhmr_op_hph_cross_attn")
+    return out
+
+
+def detect(scores, nms_k, thresh, max_persons):
+    """scores [B, res, res] fp32 -> dict(scores_out, det_b, det_y, det_x, det_score, count, count_clamped, img_off)."""
+    _cuda(scores)
+    assert scores.dtype == torch.float32 and scores.is_contiguous() and scores.dim() == 3
+    B, res, _ = scores.shape
+    dev = scores.device
+    cap = max(max_persons, 1)
+    o = {"scores_out": torch.empty_like(scores), "det_b": torch.full((cap,), -1, dtype=torch.int32, device=dev),
+         "det_y": torch.full((cap,), -1, dtype=torch.int32, device=dev),
+         "det_x": torch.full((cap,), -1, dtype=torch.int32, device=dev),
+         "det_score": torch.full((cap,), -1.0, device=dev), "count": torch.full((1,), -1, dtype=torch.int32, device=dev),
+         "count_clamped": torch.full((1,), -1, dtype=torch.int32, device=dev),
+         "img_off": torch.full((B + 1,), -1, dtype=torch.int32, device=dev)}
+    rc = _lib.load().mhmr_op_detect(ptr(scores), c_int(B), c_int(res), c_int(nms_k), c_float(thresh), c_int(max_persons),
+                                    *(ptr(o[k]) for k in ("scores_out", "det_b", "det_y", "det_x", "det_score", "count",
+                                                          "count_clamped", "img_off")), stream_ptr())
+    check(rc, "mhmr_op_detect")
+    return o
+
+
+def _zeros(dev, *shape):
+    return torch.zeros(*shape, device=dev)
+
+
+def person_post(dec, num_betas, offset, K, det_b, det_y, det_x, count, max_persons, focal_norm):
+    """SMPL-X per-person outputs from the decoder rows dec [P, >= 331 + num_betas]; returns a dict of [max_persons, ...]
+    tensors (rows >= count stay zero)."""
+    _cuda(dec, offset, K, det_b, det_y, det_x, count)
+    _f32(dec, offset, K)
+    _i32(det_b, det_y, det_x, count)
+    assert offset.is_contiguous() and K.is_contiguous()
+    Pm, dev = max_persons, dec.device
+    o = {"rotmat": _zeros(dev, Pm, 53, 3, 3), "rotvec": _zeros(dev, Pm, 53, 3), "shape": _zeros(dev, Pm, num_betas),
+         "expression": _zeros(dev, Pm, 10), "dist_pp": _zeros(dev, Pm), "dist": _zeros(dev, Pm),
+         "loc": _zeros(dev, Pm, 2), "transl": _zeros(dev, Pm, 3), "K_det": _zeros(dev, Pm, 3, 3)}
+    rc = _lib.load().mhmr_op_person_post(
+        ptr(dec), c_int(dec.stride(0)), c_int(num_betas), ptr(offset), ptr(K),
+        c_int(K.shape[0]), ptr(det_b), ptr(det_y), ptr(det_x), ptr(count), c_int(Pm), c_float(focal_norm),
+        *(ptr(o[k]) for k in ("rotmat", "rotvec", "shape", "expression", "dist_pp", "dist", "loc", "transl", "K_det")),
+        stream_ptr())
+    check(rc, "mhmr_op_person_post")
+    return o
+
+
+def anny_person_post(hid, w2, b2, fov_max, K, img_size, rot6d, J, useful, shape, offset, dist_pp, det_b, det_y, det_x,
+                     count, max_persons):
+    """Anny camera (hid [B, D] -> fov, K_regressed, K_use; K None = regressed) and per-person outputs from rot6d
+    [P, >= 6 J]; `shape` [P, num_betas] is replaced by its sigmoid in place.  Returns a dict."""
+    _cuda(hid, w2, b2, fov_max, K, rot6d, useful, shape, offset, dist_pp, det_b, det_y, det_x, count)
+    _f32(hid, w2, b2, fov_max, K, rot6d, useful, shape, offset, dist_pp)
+    _i32(det_b, det_y, det_x, count)
+    assert hid.is_contiguous() and shape.is_contiguous() and offset.is_contiguous() and dist_pp.is_contiguous()
+    assert K is None or K.is_contiguous()
+    B, D = hid.shape
+    Pm, dev = max_persons, hid.device
+    o = {"fov": _zeros(dev, B), "K_regressed": _zeros(dev, B, 3, 3), "K_use": _zeros(dev, B, 3, 3),
+         "rotmat": _zeros(dev, Pm, J, 3, 3), "rotmat_homo": _zeros(dev, Pm, J, 4, 4), "rotvec": _zeros(dev, Pm, J, 3),
+         "dist": _zeros(dev, Pm), "loc": _zeros(dev, Pm, 2), "transl": _zeros(dev, Pm, 3), "K_det": _zeros(dev, Pm, 3, 3)}
+    rc = _lib.load().mhmr_op_anny_person_post(
+        ptr(hid), c_int(D), ptr(w2), ptr(b2), ptr(fov_max), ptr(K), c_int(B),
+        c_int(img_size), ptr(o["fov"]), ptr(o["K_regressed"]), ptr(o["K_use"]), ptr(rot6d), c_int(rot6d.stride(0)),
+        c_int(J), ptr(useful), ptr(shape), c_int(shape.shape[1]), ptr(offset), ptr(dist_pp),
+        ptr(det_b), ptr(det_y), ptr(det_x), ptr(count), c_int(Pm),
+        *(ptr(o[k]) for k in ("rotmat", "rotmat_homo", "rotvec", "dist", "loc", "transl", "K_det")), stream_ptr())
+    check(rc, "mhmr_op_anny_person_post")
+    o["shape"] = shape
+    return o
+
+
+def refine_chain(layers, o16, rowidx, count, x):
+    """Central-stream refinement of x [max_persons, D] in place through len(layers) dinov2 blocks.  `layers` maps
+    Wproj, bproj, ls1, ln2_g, ln2_b, Wfc1, bfc1, Wfc2, bfc2, ls2 to fp32 tensors stacked over the blocks; o16 is the
+    fp16 attention output [depth, R, D] of the bulk pass, rowidx [max_persons] int32 its row per person."""
+    keys = ("Wproj", "bproj", "ls1", "ln2_g", "ln2_b", "Wfc1", "bfc1", "Wfc2", "bfc2", "ls2")
+    _cuda(o16, rowidx, count, x, *(layers[k] for k in keys))
+    _f32(x, *(layers[k] for k in keys))
+    _i32(rowidx, count)
+    assert o16.dtype == torch.float16 and o16.is_contiguous() and x.is_contiguous()
+    assert all(layers[k].is_contiguous() for k in keys)
+    depth, R, D = o16.shape
+    assert x.shape[1] == D and rowidx.shape[0] >= x.shape[0]
+    rc = _lib.load().mhmr_op_refine_chain(c_int(depth), c_int(D), ptr(count), c_int(x.shape[0]),
+                                          *(ptr(layers[k]) for k in keys), ptr(o16), c_int64(R), ptr(rowidx), ptr(x),
+                                          stream_ptr())
+    check(rc, "mhmr_op_refine_chain")
+    return x
