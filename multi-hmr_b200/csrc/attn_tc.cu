@@ -6,7 +6,7 @@
 //   grid  = one CTA per (image, head, 128-row query tile); query tile fastest, so that the CTAs running at the
 //           same time share the K / V of few (image, head) pairs in L2.
 //   CTA   = 384 threads = 3 warpgroups: warpgroup 0 loads Q once and streams K / V tiles of 128 keys through a
-//           ring of smem stages (TMA, one elected lane of warp 0); warpgroups 1 and 2 each own 64 query rows.
+//           ring of 4 smem stages (TMA, one elected lane of warp 0); warpgroups 1 and 2 each own 64 query rows.
 //   smem  = Q (16 KB) | kStages x (K 16 KB | V 16 KB), 128B swizzle, one TMA box per tile.
 //   S = Q K^T : wgmma m64n128k16, A = Q (smem, K-major), B = K tile (smem, K-major); S in registers.
 //   O += P V  : wgmma m64n64k16, A = P (registers: the fp16 S fragments ARE the A fragments of the next MMA),
@@ -14,9 +14,17 @@
 // Online softmax in fp32 in the exp2 domain; each thread holds 2 rows x 32 columns of S, the row max and sum
 // are reduced over the 4 lanes that share a row.
 //
-// Ragged sequence (T = N + 1 is 1 mod 128 for every Multi-HMR resolution): keys beyond T in the last tile are
-// masked to -inf (the rows there belong to the next image or are zero-filled by TMA); query rows beyond T are
+// The consumer warpgroups overlap tensor-core work with the softmax twice over: each issues S_{j} = Q K_j^T
+// together with O += P_{j-1} V_{j-1} and runs the softmax of S_j while that PV is in flight, and the two take
+// turns issuing their wgmmas (named barriers), so one's softmax runs under the other's MMAs.
+//
+// Ragged sequence (T = N + 1 is 1 mod 128 at 224, 448, 672 and 896 px, 17 mod 128 at 280 and 1288 px): keys
+// beyond T in the last tile are masked to -inf (the rows there belong to the next image or are zero-filled by
+// TMA); a last tile of at most 32 keys runs 32 keys wide (S by m64n32, PV by 2 k-steps). Query rows beyond T are
 // computed and not stored.
+//
+// Grid at ViT-L (16 heads) on 132 SMs: 896 px batch 8 (T = 4097) 4224 CTAs = 32.0 waves; 672 px batch 4
+// (T = 2305) 1216 CTAs = 9.2 waves; 1288 px batch 2 (T = 8465) 2144 CTAs = 16.2 waves.
 #include "kernels.cuh"
 
 namespace mhmr {
@@ -27,7 +35,7 @@ constexpr int kHeadDim = 64;
 constexpr int kBlockQ = 128;
 constexpr int kBlockKV = 128;
 constexpr int kTileBytes = 128 * kHeadDim * 2;  // 16 KB: Q, K or V tile
-constexpr int kStages = 3;
+constexpr int kStages = 4;
 constexpr int kAttnThreads = 384;
 constexpr int kRegsProducer = 40, kRegsConsumer = 232;
 // Q + K/V ring + 1 KB alignment pad + barriers
@@ -43,6 +51,75 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
+// S = Q K^T over the first kN keys (128 or 32) of a K tile; the caller fences and commits.
+template <int kN>
+__device__ __forceinline__ void issue_qk(float (&sc)[64], uint64_t q_desc, uint64_t k_desc) {
+#pragma unroll
+  for (int k = 0; k < kHeadDim / 16; ++k) {
+    if constexpr (kN == 128)
+      wgmma_m64n128_ss(sc, q_desc + 2u * k, k_desc + 2u * k, k > 0 ? 1u : 0u);
+    else
+      wgmma_m64n32_ss(*reinterpret_cast<float(*)[16]>(sc), q_desc + 2u * k, k_desc + 2u * k, k > 0 ? 1u : 0u);
+  }
+}
+
+// O += P V over the first 16 kK keys of a V tile (128 keys x 64 dims, N contiguous: MN-major, 8-key groups 1024 B
+// apart, 16 keys per step); the caller fences and commits.
+template <int kK>
+__device__ __forceinline__ void issue_pv(float (&o)[32], const uint32_t (&p)[8][4], uint64_t v_desc) {
+#pragma unroll
+  for (int kk = 0; kk < kK; ++kk) wgmma_m64n64_rs_bt(o, p[kk], v_desc + 128u * kk);
+}
+
+// One online-softmax step over the first kN columns of S, of which the first `valid` are keys of this image:
+// S <- exp2(S scale_log2 - m_new) in place, m_run / l_run updated, alpha = the factor the old O is scaled by.
+template <int kN>
+__device__ __forceinline__ void softmax_step(float (&sc)[64], int valid, float scale_log2, int lane,
+                                             float (&m_run)[2], float (&l_run)[2], float (&alpha)[2]) {
+  if (valid < kN) {
+#pragma unroll
+    for (int i = 0; i < kN / 2; ++i)
+      if (8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= valid) sc[i] = -INFINITY;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int g = 0; g < kN / 8; ++g) mx = fmaxf(mx, fmaxf(sc[4 * g + 2 * h], sc[4 * g + 2 * h + 1]));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float m_new = fmaxf(m_run[h], mx * scale_log2);
+    alpha[h] = ex2(m_run[h] - m_new);  // 0 on the first tile
+    m_run[h] = m_new;
+    float sum = 0.f;
+#pragma unroll
+    for (int g = 0; g < kN / 8; ++g) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int i = 4 * g + 2 * h + e;
+        sc[i] = ex2(fmaf(sc[i], scale_log2, -m_new));
+        sum += sc[i];
+      }
+    }
+    l_run[h] = l_run[h] * alpha[h] + sum;  // partial over this lane's columns; reduced over the quad at the end
+  }
+}
+
+// P as fp16 A fragments, one set of 4 registers per 16 keys
+template <int kK>
+__device__ __forceinline__ void pack_p(const float (&sc)[64], uint32_t (&p)[8][4]) {
+#pragma unroll
+  for (int kk = 0; kk < kK; ++kk) {
+    p[kk][0] = pack_half2(sc[8 * kk + 0], sc[8 * kk + 1]);
+    p[kk][1] = pack_half2(sc[8 * kk + 2], sc[8 * kk + 3]);
+    p[kk][2] = pack_half2(sc[8 * kk + 4], sc[8 * kk + 5]);
+    p[kk][3] = pack_half2(sc[8 * kk + 6], sc[8 * kk + 7]);
+  }
+}
+
+// kLastN = 32 runs the last key tile (at most 32 keys of this image, n_kv >= 2) 32 keys wide: S by m64n32 and
+// PV by 2 k-steps instead of 8; kLastN = 128 runs every tile full width.
+template <int kLastN>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ out, int64_t ldo, int T, int D,
                 int heads, int n_qt, float scale_log2) {
@@ -114,50 +191,53 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ 
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float sc[64], alpha[2];
+  uint32_t p[8][4];
+  const int valid_last = T - (n_kv - 1) * kBlockKV;
+  auto k_desc = [&](int j) { return make_sw128_desc(smem_u32(sKV + 2 * (j % kStages) * kTileBytes), 16, 1024); };
+  auto v_desc = [&](int j) {
+    return make_sw128_desc(smem_u32(sKV + (2 * (j % kStages) + 1) * kTileBytes), 1024, 1024);
+  };
+  // Ping-pong: the two consumer warpgroups take turns issuing their wgmmas. Named barrier 1 + cw opens the turn
+  // of warpgroup cw; the other warpgroup arrives on it once it has issued its own, so the softmax of one warpgroup
+  // runs while the tensor cores work on the other's MMAs. Each warpgroup issues n_kv + 1 times; warpgroup 1 opens
+  // the first turn of warpgroup 0 and skips its own last hand-over, which leaves both barriers balanced.
+  const uint32_t my_turn = 1 + cw, other_turn = 2 - cw;
+  if (cw == 1) named_bar_arrive(other_turn, 256);
   mbar_wait(q_full, 0);
 
-  for (int j = 0; j < n_kv; ++j) {
-    const int s = j % kStages;
-    mbar_wait(&kv_full[s], (j / kStages) & 1);
-    const uint32_t sk = smem_u32(sKV + 2 * s * kTileBytes);
-    const uint64_t k_desc = make_sw128_desc(sk, 16, 1024);
-    float sc[64];
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < kHeadDim / 16; ++k) wgmma_m64n128_ss(sc, q_desc + 2u * k, k_desc + 2u * k, k > 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(sc);
+  // Within a warpgroup, S_j = Q K_j^T is issued together with O += P_{j-1} V_{j-1}; the softmax of S_j runs while
+  // that PV is in flight, and O is rescaled by alpha_j once it lands, before P_j V_j is issued: the same
+  // per-row arithmetic as a sequential S, softmax, PV loop.
+  mbar_wait(&kv_full[0], 0);
+  named_bar_sync(my_turn, 256);
+  wgmma_fence();
+  issue_qk<128>(sc, q_desc, k_desc(0));
+  wgmma_commit();
+  named_bar_arrive(other_turn, 256);
+  wgmma_wait<0>();
+  wgmma_fence_regs(sc);
+  softmax_step<128>(sc, n_kv == 1 ? valid_last : kBlockKV, scale_log2, lane, m_run, l_run, alpha);
+  pack_p<8>(sc, p);  // O is still 0: no rescale
 
-    if (j == n_kv - 1) {  // keys beyond T
-      const int valid = T - j * kBlockKV;
-#pragma unroll
-      for (int i = 0; i < 64; ++i)
-        if (8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= valid) sc[i] = -INFINITY;
-    }
-    float alpha[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int g = 0; g < 16; ++g) mx = fmaxf(mx, fmaxf(sc[4 * g + 2 * h], sc[4 * g + 2 * h + 1]));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      const float m_new = fmaxf(m_run[h], mx * scale_log2);
-      alpha[h] = ex2(m_run[h] - m_new);  // 0 on the first tile
-      m_run[h] = m_new;
-      float sum = 0.f;
-#pragma unroll
-      for (int g = 0; g < 16; ++g) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int i = 4 * g + 2 * h + e;
-          sc[i] = ex2(fmaf(sc[i], scale_log2, -m_new));
-          sum += sc[i];
-        }
-      }
-      l_run[h] = l_run[h] * alpha[h] + sum;  // partial over this lane's columns; reduced over the quad at the end
-    }
+  // key tile j >= 1, the first kN keys of it (the wgmma shapes are fixed at compile time: a runtime choice
+  // between them would make ptxas serialize every wgmma of the kernel)
+  auto step = [&](int j, auto width) {
+    constexpr int kN = decltype(width)::value;
+    mbar_wait(&kv_full[j % kStages], (j / kStages) & 1);
+    named_bar_sync(my_turn, 256);
+    wgmma_fence();
+    issue_qk<kN>(sc, q_desc, k_desc(j));
+    wgmma_commit();
+    issue_pv<8>(o, p, v_desc(j - 1));
+    wgmma_commit();
+    named_bar_arrive(other_turn, 256);
+    wgmma_wait<1>();  // S_j
+    wgmma_fence_regs(sc);
+    softmax_step<kN>(sc, j == n_kv - 1 ? valid_last : kBlockKV, scale_log2, lane, m_run, l_run, alpha);
+    wgmma_wait<0>();  // P_{j-1} V_{j-1}: stage j - 1 is no longer read
+    wgmma_fence_regs(o);
+    if (release_lane) mbar_arrive(&kv_empty[(j - 1) % kStages]);
 #pragma unroll
     for (int g = 0; g < 8; ++g) {
       o[4 * g + 0] *= alpha[0];
@@ -165,25 +245,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ 
       o[4 * g + 2] *= alpha[1];
       o[4 * g + 3] *= alpha[1];
     }
-    // P as fp16 A fragments, one set of 4 registers per 16 keys
-    uint32_t p[8][4];
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      p[kk][0] = pack_half2(sc[8 * kk + 0], sc[8 * kk + 1]);
-      p[kk][1] = pack_half2(sc[8 * kk + 2], sc[8 * kk + 3]);
-      p[kk][2] = pack_half2(sc[8 * kk + 4], sc[8 * kk + 5]);
-      p[kk][3] = pack_half2(sc[8 * kk + 6], sc[8 * kk + 7]);
-    }
-    // V tile: 128 keys (K) x 64 dims (N), N contiguous: MN-major, 8-key groups 1024 B apart, 16 keys per step
-    const uint64_t v_desc = make_sw128_desc(sk + kTileBytes, 1024, 1024);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) wgmma_m64n64_rs_bt(o, p[kk], v_desc + 128u * kk);
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(o);
-    if (release_lane) mbar_arrive(&kv_empty[s]);
-  }
+    pack_p<kN / 16>(sc, p);
+  };
+  constexpr bool kNarrow = kLastN < kBlockKV;  // then n_kv >= 2 (attention_forward)
+  for (int j = 1; j < n_kv - (kNarrow ? 1 : 0); ++j) step(j, std::integral_constant<int, kBlockKV>{});
+  if constexpr (kNarrow) step(n_kv - 1, std::integral_constant<int, kLastN>{});
+
+  named_bar_sync(my_turn, 256);
+  wgmma_fence();
+  issue_pv<kLastN / 16>(o, p, v_desc(n_kv - 1));
+  wgmma_commit();
+  if (cw == 0) named_bar_arrive(other_turn, 256);
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
+  if (release_lane) mbar_arrive(&kv_empty[(n_kv - 1) % kStages]);
 
   // epilogue: O / l -> fp16 -> out[img*T + q, head*64 + :]
 #pragma unroll
@@ -217,10 +292,15 @@ int attention_forward(const __half* qkv, int64_t ld_qkv, __half* out, int64_t ld
   if (rc != MHMR_OK) return rc;
   const int heads = D / kHeadDim;
   const int n_qt = (T + kBlockQ - 1) / kBlockQ;
+  const int n_kv = (T + kBlockKV - 1) / kBlockKV;
   static PerDeviceOnce once;
   if (once.first()) {
-    MHMR_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
+    MHMR_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kAttnSmemBytes));
+    MHMR_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kAttnSmemBytes));
   }
+  const bool narrow_tail = n_kv >= 2 && T - (n_kv - 1) * kBlockKV <= 32;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(B * heads * n_qt);
   cfg.blockDim = dim3(kAttnThreads);
@@ -232,7 +312,8 @@ int attention_forward(const __half* qkv, int64_t ld_qkv, __half* out, int64_t ld
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
   const float scale_log2 = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e)
-  MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, attn_fwd_kernel, tm, out, ldo, T, D, heads, n_qt, scale_log2));
+  MHMR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, narrow_tail ? attn_fwd_kernel<32> : attn_fwd_kernel<128>, tm, out, ldo,
+                                     T, D, heads, n_qt, scale_log2));
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }

@@ -228,6 +228,14 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Named CTA barriers (ids 1..15; 0 is __syncthreads) over `count` threads, a multiple of 32: sync blocks until
+// `count` threads have arrived, arrive counts this warp in and goes on.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 // Keeps the compiler from moving accumulator accesses across an in-flight wgmma.
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
@@ -246,6 +254,16 @@ __device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t da, uin
       "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
       "%32, %33, p, 1, 1, 0, 0;\n\t}"
       : MHMR_WG_D8(0), MHMR_WG_D8(8), MHMR_WG_D8(16), MHMR_WG_D8(24)
+      : "l"(da), "l"(db), "r"(acc));
+}
+// D[64 x 32] (+)= A[smem] * B[smem]^T, fp16 operands, both K-major, fp32 accumulate.
+__device__ __forceinline__ void wgmma_m64n32_ss(float (&d)[16], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n\t}"
+      : MHMR_WG_D8(0), MHMR_WG_D8(8)
       : "l"(da), "l"(db), "r"(acc));
 }
 // D[64 x 128] (+)= A[smem] * B[smem]^T, fp16 operands, both K-major, fp32 accumulate.
