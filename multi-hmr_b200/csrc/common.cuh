@@ -188,11 +188,13 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// Arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+// Arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster.  No cluster-scope release
+// (that form compiles to a CTA- and a GPU-scope MEMBAR): a waiter in the other CTA must not rely on it to see
+// this thread's earlier memory writes.
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 // 2-D tile load global -> shared of every CTA in `cta_mask`, at the same offsets; each destination CTA's
 // barrier at `bar`'s offset receives the bytes.

@@ -1,7 +1,8 @@
 // wgmma + TMA persistent GEMM (see gemm_tc.cuh for the contract).
 //
 // CTA = 384 threads = 3 warpgroups, one CTA per SM, persistent over output tiles (128 x BN):
-//   warpgroup 0   : TMA producer (warp 0, one elected lane)   global -> 128B-swizzled smem ring
+//   warpgroup 0   : TMA producer (warp 0, one elected lane)   global -> 128B-swizzled smem ring of 3 stages of
+//                   48 KB at BN = 256 (5 of 32 KB at BN = 128)
 //   warpgroups 1-2: consumers; warpgroup 1 + c computes columns [c BN/2, (c+1) BN/2) of the tile with
 //                   wgmma m64 x (BN/2) x k16 (fp32 accumulators in registers), then runs the fused epilogue
 //                   (gemm_epilogue.cuh) on them.
@@ -12,6 +13,11 @@
 // block_n 512: a cluster of two CTAs computes a 256 x 256 tile.  Each CTA stages its own 128 rows of A and
 // loads half of the 256-row weight tile, multicast into both CTAs, so the weight traffic from L2 per CTA
 // halves.  A smem stage is refilled only once the consumers of BOTH CTAs have released it.
+//
+// A consumer warpgroup releases a stage once the wgmma_wait after the next k block's issue shows the stage's
+// wgmmas complete.  The release is a plain mbarrier arrive on its own CTA's barrier and a remote arrive on the
+// peer's, with no memory fence: a .release.cluster arrive compiles to a CTA- and a GPU-scope MEMBAR, which also
+// waits for the releasing lane's outstanding epilogue stores, and the whole warpgroup waits for that lane.
 #include "gemm_tc.cuh"
 #include "gemm_epilogue.cuh"
 
@@ -121,13 +127,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int w = warp & 3;         // rows 32w..32w+31 of the tile
     const bool release_lane = (threadIdx.x & 127) == 0;
     float* scratch = scratch_base + (warp - 4) * (kScratchBytes / 4);
+    // Frees stage s in every CTA of the cluster.  No fence: this warpgroup's wgmma reads of the stage are
+    // complete at the wgmma_wait that precedes every release, and the refill is a TMA (async-proxy) write that
+    // the producer issues only after its empty_bar wait has observed the arrives.
     auto release = [&](uint32_t s) {
       if (release_lane) {
+        mbar_arrive(&empty_bar[s]);
         if constexpr (CL > 1) {
 #pragma unroll
-          for (int c = 0; c < CL; ++c) mbar_arrive_cluster(&empty_bar[s], static_cast<uint32_t>(c));
-        } else {
-          mbar_arrive(&empty_bar[s]);
+          for (int c = 0; c < CL; ++c)
+            if (c != static_cast<int>(rank)) mbar_arrive_remote(&empty_bar[s], static_cast<uint32_t>(c));
         }
       }
     };
