@@ -144,6 +144,79 @@ int mhmr_op_refine_chain(int depth, int D, const int* count, int max_persons, co
                          const float* Wfc2, const float* bfc2, const float* ls2, const void* O16, int64_t rows_o16,
                          const int* rowidx, float* x, void* stream);
 
+/* Backbone entry, folded LayerNorm and the gathers of the heads: the engine's own launchers behind thin validating
+ * entries, arguments checked before any launch.  Device pointers; fp16 buffers are passed as void*.  Entries with a
+ * person capacity read the count from the device int32 `count` like the person-decoder entries above, and return
+ * without a launch for a capacity of 0. */
+
+/* Patch rows of the 14x14/14 patch-embed conv: A[b*N + gy*(S/14) + gx, c*196 + ky*14 + kx] = fp16 of pixel
+ * (c, gy*14 + ky, gx*14 + kx) of image b, from img fp32 [B,3,S,S] or img_u8 [B,S,S,3] through lut [3][256] (exactly
+ * one source).  Columns 588 .. ldA-1 are not written. */
+int mhmr_op_im2col_patch14(const float* img, const void* img_u8, const float* lut, int B, int S, void* A, int ldA,
+                           void* stream);
+/* LayerNorm of M rows of width D (multiple of 128, <= 1024): X fp32 [M, D], or the two-term fp16 stream X = hi plane,
+ * Xlo = lo plane.  out16 (fp16, pitch ld16) and out32 (fp32, pitch ld32) are each nullable, not both.  rows_in > 0:
+ * row g*rows_in + t is dropped when t < skip, else written to row g*(rows_in - skip) + t - skip (the final norm drops
+ * the cls row). */
+int mhmr_op_layernorm(const void* X, const void* Xlo, const float* gamma, const float* beta, void* out16, int64_t ld16,
+                      float* out32, int64_t ld32, int M, int D, float eps, int rows_in, int skip, void* stream);
+/* Entry of the folded-LayerNorm chain: X fp32 [M, D] -> xhi = fp16(X), xlo = fp16(X - xhi) (pitch ld16), and
+ * stats [M, slots] (sum, sum of squares) pairs: slot 0 the whole row, slots >= 1 zero. */
+int mhmr_op_split_rowstats(const float* X, void* xhi, void* xlo, int64_t ld16, float* stats, int slots, int M, int D,
+                           void* stream);
+/* Load-time folding of a LayerNorm into the Linear after it: W16[n,k] = fp16(W[n,k] ln_g[k] - mean_k(W[n,:] ln_g)),
+ * bias2[n] = bias[n] + sum_k ln_b[k] W[n,k]; W fp32 [N, K], W16 fp16 [N, K]. */
+int mhmr_op_fold_ln_linear(const float* W, const float* bias, const float* ln_g, const float* ln_b, void* W16,
+                           float* bias2, int N, int K, void* stream);
+/* The GEMM of mhmr_op_gemm_f16 with the engine's internal epilogues (kinds 6-9):
+ *   6  LS_RESID_SPLIT  x = (x16 + xlo) + gamma * (acc + bias) written back as two fp16 planes (pitch ldx16), and per
+ *                      row the (sum, sum of squares) of the new x over the N/stat_slots columns of each slot into
+ *                      stats [M, stat_slots]; stat_slots = 2 * ceil(N / tile), tile 128 (block_n 128) or 256
+ *   7  LN_BIAS_F16     out16 = rstd * acc + bias, rstd = 1/sqrt(max(q/K - (s/K)^2, 0) + 1e-6) from the slot sums of
+ *                      stats
+ *                      [M, stat_slots] (stat_slots even, <= 8)
+ *   8  LN_GELU_F16     out16 = gelu_erf(rstd * acc + bias)
+ *   9  ROWADD_F16      out16 = acc + rowadd[m % rows_in] */
+int mhmr_op_gemm_internal(const void* A, int64_t lda, const void* W, int64_t ldw, int M, int N, int K, int epilogue,
+                          const float* bias, const float* gamma, void* x16, void* xlo, int64_t ldx16, float* stats,
+                          int stat_slots, const float* rowadd, int rows_in, void* out, int64_t ldo, int block_n,
+                          void* stream);
+/* Camera rays of every token (model.py:160-187): Kinv [B, 3, 3] = K^-1, then ctx[b*res*res + n, col0 + j] = fp16 of
+ * feature j < 99 of cell n (the (row, col) grid passed as (x, y)), zero for 99 <= j < pad_cols (<= 128). */
+int mhmr_op_camera_ctx(const float* K, int B, const float* freqs, float* Kinv, void* ctx, int64_t ld, int res, int col0,
+                       int pad_cols, void* stream);
+/* scores[r] = sigmoid(hid[r, :D] . w + b[0]) for r < M, hid fp16 (pitch ld); clamped to [1e-4, 1 - 1e-4] when clamp
+ * is set; logits (nullable) receives the dot product plus bias. */
+int mhmr_op_rowdot_sigmoid(const void* hid, int64_t ld, const float* w, const float* b, float* scores, float* logits,
+                           int clamp, int M, int D, void* stream);
+/* Per person: zc [P, D] = feature row of the cell (z32 [B*res*res, D]), or LayerNorm(xr[p]; norm_g, norm_b, 1e-6) when
+ * xr is given; query [P, ldq] = cat(zc, camera feature) + cq_x[y] + cq_y[x]; vals [P, ldq] = cv_x[y] + cv_y[x]
+ * (tables [res, D + 99]); columns D + 99 .. ldq-1 of query and vals are zero. */
+int mhmr_op_person_gather(const float* z32, const float* xr, const float* norm_g, const float* norm_b, const float* Kinv,
+                          const float* freqs, const float* cq_x, const float* cq_y, const float* cv_x, const float* cv_y,
+                          const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
+                          int res, int D, float* zc, float* query, float* vals, int ldq, void* stream);
+/* Inputs of the central-stream refinement: rows [0, n_cls) are the cls rows of images 0..n_cls-1 (rowidx b*(N+1),
+ * zero patch, xr = cls_pos), row n_cls + p is person p (rowidx b*(N+1) + 1 + cell, its 588 pixels in (c, ky, kx)
+ * order from img fp32 or img_u8 + lut, xr = rowadd[cell]); patch pitch ldp; rows_out (nullable) = n_cls + count. */
+int mhmr_op_refine_prepare(const float* img, const void* img_u8, const float* lut, int S, const float* rowadd, int D,
+                           const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
+                           int n_cls, const float* cls_pos, int* rows_out, int* rowidx, float* patch, int ldp, float* xr,
+                           void* stream);
+/* KV[b*res*res + y*res + x, :ncols] += dKV[p, :ncols] once per distinct cell of the persons p < count (model.py:517). */
+int mhmr_op_kv_add_rows(float* KV, int64_t ldkv, const float* dKV, int ncols, const int* det_b, const int* det_y,
+                        const int* det_x, const int* count, int max_persons, int res, void* stream);
+/* out[b, :D] = row b*T of the residual stream: X fp32, or the two-term split X = hi, Xlo = lo (fp16); pitch ld. */
+int mhmr_op_cls_gather(const void* X, const void* Xlo, int64_t ld, int T, int B, int D, float* out, void* stream);
+/* Anny decoder inputs per person: zc [P, D] as in mhmr_op_person_gather, xa [P, dim] = pos[cell]. */
+int mhmr_op_anny_gather(const float* z32, const float* xr, const float* norm_g, const float* norm_b, const float* pos,
+                        const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons, int res,
+                        int D, int dim, float* zc, float* xa, void* stream);
+/* Placement of P bodies (mhmr_anny_place with the centre bone given): v3d in place and j3d from bone_poses, both
+ * shifted by transl - bone(center); v2d (nullable), j2d projected with K_det; transl_pelvis = j3d[:, 0]. */
+int mhmr_op_anny_place(const float* bone_poses, const float* transl, const float* K_det, int center, int P, int V, int J,
+                       float* v3d, float* j3d, float* v2d, float* j2d, float* transl_pelvis, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Engine: the whole `Model.forward(x, K)` path (reference model.py:205-349) behind one handle
  * ---------------------------------------------------------------------------------------------- */

@@ -234,4 +234,165 @@ int mhmr_op_refine_chain(int depth, int D, const int* count, int max_persons, co
   return rc;
 }
 
+// ---- backbone entry, folded LayerNorm and the gathers of the heads (vit_misc.cu, gemm_tc.cu, head.cu) --------------
+
+int mhmr_op_im2col_patch14(const float* img, const void* img_u8, const float* lut, int B, int S, void* A, int ldA,
+                           void* stream) {
+  MHMR_REQUIRE(A != nullptr && (img != nullptr) != (img_u8 != nullptr) && (img_u8 == nullptr) == (lut == nullptr),
+               "im2col: exactly one image source (fp32 CHW, or uint8 HWC with its table)");
+  MHMR_REQUIRE(B >= 1 && S >= 14 && S % 14 == 0 && ldA >= 588, "im2col: bad geometry");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (img_u8 != nullptr)
+    return im2col_u8_patch14(static_cast<const uint8_t*>(img_u8), lut, static_cast<__half*>(A), B, S, ldA, st);
+  return im2col_patch14(img, static_cast<__half*>(A), B, S, ldA, st);
+}
+
+int mhmr_op_layernorm(const void* X, const void* Xlo, const float* gamma, const float* beta, void* out16, int64_t ld16,
+                      float* out32, int64_t ld32, int M, int D, float eps, int rows_in, int skip, void* stream) {
+  MHMR_REQUIRE(X && gamma && beta && (out16 || out32), "null argument");
+  MHMR_REQUIRE(M >= 0 && D >= 128 && D % 128 == 0 && D <= 1024, "layernorm: D must be a multiple of 128 (<= 1024)");
+  MHMR_REQUIRE(rows_in == 0 ? skip == 0 : (rows_in > 0 && skip >= 0 && skip < rows_in && M % rows_in == 0),
+               "layernorm: rows_in must divide M and exceed skip");
+  MHMR_REQUIRE((out16 == nullptr || (ld16 >= D && ld16 % 4 == 0)) && (out32 == nullptr || (ld32 >= D && ld32 % 4 == 0)),
+               "layernorm: output pitches must cover D and be multiples of 4");
+  MHMR_REQUIRE(aligned16(X) && aligned16(gamma) && aligned16(beta) && (Xlo == nullptr || aligned16(Xlo)) &&
+                   (out16 == nullptr || aligned16(out16)) && (out32 == nullptr || aligned16(out32)),
+               "layernorm: every buffer must be 16-byte aligned");
+  if (M == 0) return MHMR_OK;
+  return layernorm_split(X, static_cast<const __half*>(Xlo), gamma, beta, static_cast<__half*>(out16), ld16, out32,
+                         ld32, M, D, eps, rows_in, skip, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_split_rowstats(const float* X, void* xhi, void* xlo, int64_t ld16, float* stats, int slots, int M, int D,
+                           void* stream) {
+  MHMR_REQUIRE(X && xhi && xlo && stats, "null argument");
+  MHMR_REQUIRE(M >= 0 && D >= 128 && D % 128 == 0 && D <= 1024 && slots >= 1 && slots <= 32 && ld16 >= D &&
+                   ld16 % 4 == 0, "split_rowstats: bad sizes");
+  MHMR_REQUIRE(aligned16(X) && aligned16(xhi) && aligned16(xlo) && (reinterpret_cast<uintptr_t>(stats) & 7u) == 0,
+               "split_rowstats: X and the planes must be 16-byte aligned, stats 8-byte aligned");
+  if (M == 0) return MHMR_OK;
+  return split_rowstats(X, static_cast<__half*>(xhi), static_cast<__half*>(xlo), ld16, reinterpret_cast<float2*>(stats),
+                        slots, M, D, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_fold_ln_linear(const float* W, const float* bias, const float* ln_g, const float* ln_b, void* W16,
+                           float* bias2, int N, int K, void* stream) {
+  MHMR_REQUIRE(W && bias && ln_g && ln_b && W16 && bias2, "null argument");
+  MHMR_REQUIRE(N >= 1 && K >= 1, "fold_ln_linear: bad sizes");
+  return fold_ln_linear(W, bias, ln_g, ln_b, static_cast<__half*>(W16), bias2, N, K, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_gemm_internal(const void* A, int64_t lda, const void* W, int64_t ldw, int M, int N, int K, int epilogue,
+                          const float* bias, const float* gamma, void* x16, void* xlo, int64_t ldx16, float* stats,
+                          int stat_slots, const float* rowadd, int rows_in, void* out, int64_t ldo, int block_n,
+                          void* stream) {
+  MHMR_REQUIRE(epilogue >= EPI_NUM_PUBLIC_KINDS && epilogue < EPI_NUM_KINDS,
+               "gemm_internal: epilogue must be an internal kind (6..9)");
+  MHMR_REQUIRE(epilogue != EPI_LS_RESID_SPLIT || (ldx16 >= N && aligned16(x16) && aligned16(xlo)),
+               "gemm_internal: the split planes must cover N columns and be 16-byte aligned");
+  MHMR_REQUIRE(epilogue == EPI_LS_RESID_SPLIT || (ldo >= N && aligned16(out)),
+               "gemm_internal: the output must cover N columns and be 16-byte aligned");
+  MHMR_REQUIRE(stats == nullptr || aligned16(stats), "gemm_internal: stats must be 16-byte aligned");
+  MHMR_REQUIRE(rowadd == nullptr || aligned16(rowadd), "gemm_internal: rowadd must be 16-byte aligned");
+  GemmEpi ep;
+  ep.bias = bias;
+  ep.gamma = gamma;
+  ep.rowadd = rowadd;
+  ep.rows_in = rows_in;
+  ep.out = out;
+  ep.ldo = ldo;
+  ep.x16 = static_cast<__half*>(x16);
+  ep.xlo = static_cast<__half*>(xlo);
+  ep.ldx16 = ldx16;
+  ep.stats = reinterpret_cast<float2*>(stats);
+  ep.stat_slots = stat_slots;
+  GemmPlan plan;
+  int rc = gemm_plan_init(&plan, static_cast<const __half*>(A), lda, static_cast<const __half*>(W), ldw, M, N, K,
+                          epilogue, ep, block_n);
+  if (rc != MHMR_OK) return rc;
+  return gemm_plan_run(&plan, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_camera_ctx(const float* K, int B, const float* freqs, float* Kinv, void* ctx, int64_t ld, int res, int col0,
+                       int pad_cols, void* stream) {
+  MHMR_REQUIRE(K && freqs && Kinv && ctx, "null argument");
+  MHMR_REQUIRE(B >= 1 && res >= 1 && col0 >= 0 && pad_cols >= 99 && pad_cols <= 128 && ld >= col0 + pad_cols,
+               "camera_ctx: bad sizes (pad_cols in [99, 128], ld >= col0 + pad_cols)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int rc = invert_K(K, Kinv, B, st);
+  if (rc != MHMR_OK) return rc;
+  return ctx_fourier(Kinv, freqs, static_cast<__half*>(ctx), ld, B, res, col0, pad_cols, st);
+}
+
+int mhmr_op_rowdot_sigmoid(const void* hid, int64_t ld, const float* w, const float* b, float* scores, float* logits,
+                           int clamp, int M, int D, void* stream) {
+  MHMR_REQUIRE(hid && w && b && scores, "null argument");
+  MHMR_REQUIRE(M >= 0 && D >= 8 && D % 8 == 0 && ld >= D && ld % 8 == 0, "rowdot_sigmoid: bad sizes");
+  MHMR_REQUIRE(aligned16(hid) && aligned16(w), "rowdot_sigmoid: hid and w must be 16-byte aligned");
+  if (M == 0) return MHMR_OK;
+  return rowdot_sigmoid(static_cast<const __half*>(hid), ld, w, b, scores, logits, clamp != 0, M, D,
+                        static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_person_gather(const float* z32, const float* xr, const float* norm_g, const float* norm_b, const float* Kinv,
+                          const float* freqs, const float* cq_x, const float* cq_y, const float* cv_x, const float* cv_y,
+                          const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
+                          int res, int D, float* zc, float* query, float* vals, int ldq, void* stream) {
+  MHMR_REQUIRE(max_persons >= 0 && res >= 1 && D >= 1 && ldq >= D + 99, "person_gather: bad sizes (ldq >= D + 99)");
+  if (max_persons == 0) return MHMR_OK;
+  MHMR_REQUIRE(z32 && Kinv && freqs && cq_x && cq_y && cv_x && cv_y && det_b && det_y && det_x && count && zc && query &&
+                   vals, "null argument");
+  MHMR_REQUIRE(xr == nullptr || (norm_g && norm_b), "person_gather: the refined rows need the final norm");
+  return person_gather(z32, xr, norm_g, norm_b, Kinv, freqs, cq_x, cq_y, cv_x, cv_y, det_b, det_y, det_x, count,
+                       max_persons, res, D, zc, query, vals, ldq, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_refine_prepare(const float* img, const void* img_u8, const float* lut, int S, const float* rowadd, int D,
+                           const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
+                           int n_cls, const float* cls_pos, int* rows_out, int* rowidx, float* patch, int ldp, float* xr,
+                           void* stream) {
+  MHMR_REQUIRE(S >= 14 && S % 14 == 0 && D >= 1 && max_persons >= 0 && n_cls >= 0, "refine_prepare: bad sizes");
+  if (n_cls + max_persons == 0) return MHMR_OK;
+  MHMR_REQUIRE(rowadd && det_b && det_y && det_x && count && rowidx && patch && xr, "null argument");
+  MHMR_REQUIRE(img_u8 == nullptr || lut != nullptr, "refine_prepare: the uint8 image needs its table");
+  return refine_prepare(img, static_cast<const uint8_t*>(img_u8), lut, S, rowadd, D, det_b, det_y, det_x, count,
+                        max_persons, S / 14, n_cls, cls_pos, rows_out, rowidx, patch, ldp, xr,
+                        static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_kv_add_rows(float* KV, int64_t ldkv, const float* dKV, int ncols, const int* det_b, const int* det_y,
+                        const int* det_x, const int* count, int max_persons, int res, void* stream) {
+  MHMR_REQUIRE(max_persons >= 0 && res >= 1 && ncols >= 1 && ldkv >= ncols, "kv_add_rows: bad sizes");
+  if (max_persons == 0) return MHMR_OK;
+  MHMR_REQUIRE(KV && dKV && det_b && det_y && det_x && count, "null argument");
+  return kv_add_rows(KV, ldkv, dKV, ncols, det_b, det_y, det_x, count, max_persons, res,
+                     static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_cls_gather(const void* X, const void* Xlo, int64_t ld, int T, int B, int D, float* out, void* stream) {
+  MHMR_REQUIRE(X && out, "null argument");
+  MHMR_REQUIRE(B >= 1 && T >= 1 && D >= 1 && ld >= D, "cls_gather: bad sizes");
+  return cls_gather(X, static_cast<const __half*>(Xlo), ld, T, B, D, out, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_anny_gather(const float* z32, const float* xr, const float* norm_g, const float* norm_b, const float* pos,
+                        const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons, int res,
+                        int D, int dim, float* zc, float* xa, void* stream) {
+  MHMR_REQUIRE(max_persons >= 0 && res >= 1 && D >= 1 && dim >= 1, "anny_gather: bad sizes");
+  if (max_persons == 0) return MHMR_OK;
+  MHMR_REQUIRE(z32 && pos && det_b && det_y && det_x && count && zc && xa, "null argument");
+  MHMR_REQUIRE(xr == nullptr || (norm_g && norm_b), "anny_gather: the refined rows need the final norm");
+  return anny_gather(z32, xr, norm_g, norm_b, pos, det_b, det_y, det_x, count, max_persons, res, D, dim, zc, xa,
+                     static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_anny_place(const float* bone_poses, const float* transl, const float* K_det, int center, int P, int V, int J,
+                       float* v3d, float* j3d, float* v2d, float* j2d, float* transl_pelvis, void* stream) {
+  MHMR_REQUIRE(P >= 0 && P <= 65535 && V >= 0 && J >= 1 && center >= 0 && center < J, "anny_place: bad sizes");
+  if (P == 0) return MHMR_OK;
+  MHMR_REQUIRE(bone_poses && transl && K_det && (V == 0 || v3d) && j3d && j2d && transl_pelvis, "null argument");
+  return anny_place(bone_poses, transl, K_det, center, P, V, J, v3d, j3d, v2d, j2d, transl_pelvis,
+                    static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

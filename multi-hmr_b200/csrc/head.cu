@@ -321,13 +321,20 @@ refine_prepare_kernel(const float* __restrict__ img, const uint8_t* __restrict__
 }
 
 // KV[b*N + cell(p), :] += dKV[p, :]   (context += learned values at detected cells, model.py:517)
+// The reference's `xx[idx] += values` is a non-accumulating index_put: a cell that several (forced) persons share
+// receives the values once.  Their dKV rows are equal (the values depend on the cell only), so only the first person
+// of a cell adds; the others leave, and no row is updated by two CTAs.
 __global__ void kv_add_rows_kernel(float* __restrict__ KV, int64_t ldkv, const float* __restrict__ dKV,
                                    int ncols, const int* __restrict__ det_b, const int* __restrict__ det_y,
                                    const int* __restrict__ det_x, const int* __restrict__ count, int res) {
   const int p = blockIdx.x;
   if (p >= *count) return;
+  const int b = det_b[p], y = det_y[p], x = det_x[p];
+  int dup = 0;
+  for (int q = threadIdx.x; q < p; q += blockDim.x) dup |= (det_b[q] == b && det_y[q] == y && det_x[q] == x);
+  if (__syncthreads_or(dup)) return;
   const int N = res * res;
-  float* row = KV + (static_cast<int64_t>(det_b[p]) * N + det_y[p] * res + det_x[p]) * ldkv;
+  float* row = KV + (static_cast<int64_t>(b) * N + y * res + x) * ldkv;
   for (int c = threadIdx.x; c < ncols; c += blockDim.x) row[c] += dKV[static_cast<int64_t>(p) * ncols + c];
 }
 

@@ -56,6 +56,7 @@ int person_gather(const float* z32, const float* xr, const float* norm_g, const 
 int refine_prepare(const float* img, const uint8_t* img_u8, const float* lut, int S, const float* rowadd, int D, const int* det_b, const int* det_y,
                    const int* det_x, const int* count, int max_persons, int res, int n_cls, const float* cls_pos,
                    int* rows_out, int* rowidx, float* patch, int ldp, float* xr, cudaStream_t st);
+// each distinct cell once: persons that share a cell with an earlier person add nothing (their dKV rows are equal)
 int kv_add_rows(float* KV, int64_t ldkv, const float* dKV, int ncols, const int* det_b, const int* det_y,
                 const int* det_x, const int* count, int max_persons, int res, cudaStream_t st);
 int skinny_linear(const float* x, int ldx, const int* count, int max_persons, int K, const float* W, int ldw,

@@ -220,3 +220,189 @@ def refine_chain(layers, o16, rowidx, count, x):
                                           stream_ptr())
     check(rc, "mhmr_op_refine_chain")
     return x
+
+
+# ---- backbone entry, folded LayerNorm and the gathers of the heads -------------------------------------------------
+EPI_LS_RESID_SPLIT, EPI_LN_BIAS_F16, EPI_LN_GELU_F16, EPI_ROWADD_F16 = range(6, 10)
+
+
+def _contig(*ts):
+    for t in ts:
+        assert t is None or t.is_contiguous(), "contiguous tensor expected"
+
+
+def im2col_patch14(img, A, lut=None):
+    """Patch rows of the patch-embed GEMM into A [B*(S/14)^2, ldA] fp16 (columns >= 588 untouched): img fp32
+    [B, 3, S, S], or uint8 [B, S, S, 3] with its [3, 256] table `lut`."""
+    _cuda(img, A, lut)
+    _contig(img, lut)
+    assert A.dtype == torch.float16 and A.stride(1) == 1
+    u8 = img.dtype == torch.uint8
+    assert (lut is not None) == u8 and (img.dtype == torch.float32 or u8)
+    B, S = img.shape[0], img.shape[2] if u8 else img.shape[3]
+    rc = _lib.load().mhmr_op_im2col_patch14(ptr(None if u8 else img), ptr(img if u8 else None), ptr(lut), c_int(B),
+                                            c_int(S), ptr(A), c_int(A.stride(0)), stream_ptr())
+    check(rc, "mhmr_op_im2col_patch14")
+    return A
+
+
+def layernorm(x, gamma, beta, out16=None, out32=None, eps=1e-6, rows_in=0, skip=0, xlo=None):
+    """LayerNorm of the rows of x [M, D] (fp32, or the fp16 hi plane with `xlo` the lo plane) into out16 and / or
+    out32 (row pitches = their strides); rows_in > 0 drops rows t < skip of every group of rows_in."""
+    _cuda(x, xlo, gamma, beta, out16, out32)
+    _contig(x, xlo, gamma, beta)
+    assert (xlo is None and x.dtype == torch.float32) or (x.dtype == xlo.dtype == torch.float16)
+    for o in (out16, out32):
+        assert o is None or o.stride(1) == 1
+    M, D = x.shape
+    rc = _lib.load().mhmr_op_layernorm(ptr(x), ptr(xlo), ptr(gamma), ptr(beta), ptr(out16),
+                                       c_int64(out16.stride(0) if out16 is not None else 0), ptr(out32),
+                                       c_int64(out32.stride(0) if out32 is not None else 0), c_int(M), c_int(D),
+                                       c_float(eps), c_int(rows_in), c_int(skip), stream_ptr())
+    check(rc, "mhmr_op_layernorm")
+
+
+def split_rowstats(x, hi, lo, stats):
+    """x fp32 [M, D] -> hi, lo fp16 [M, >= D] (x = hi + lo) and stats fp32 [M, slots, 2] (slot 0 = (sum, sumsq))."""
+    _cuda(x, hi, lo, stats)
+    _contig(x, stats)
+    assert hi.dtype == lo.dtype == torch.float16 and hi.stride() == lo.stride() and hi.stride(1) == 1
+    M, D = x.shape
+    rc = _lib.load().mhmr_op_split_rowstats(ptr(x), ptr(hi), ptr(lo), c_int64(hi.stride(0)), ptr(stats),
+                                            c_int(stats.shape[1]), c_int(M), c_int(D), stream_ptr())
+    check(rc, "mhmr_op_split_rowstats")
+
+
+def fold_ln_linear(w, bias, ln_g, ln_b):
+    """Folds LayerNorm(ln_g, ln_b) into the Linear (w [N, K], bias): returns (W16 fp16 [N, K], bias2 fp32 [N])."""
+    _cuda(w, bias, ln_g, ln_b)
+    _contig(w, bias, ln_g, ln_b)
+    N, K = w.shape
+    w16 = torch.empty(N, K, device=w.device, dtype=torch.float16)
+    b2 = torch.empty(N, device=w.device)
+    rc = _lib.load().mhmr_op_fold_ln_linear(ptr(w), ptr(bias), ptr(ln_g), ptr(ln_b), ptr(w16), ptr(b2), c_int(N),
+                                            c_int(K), stream_ptr())
+    check(rc, "mhmr_op_fold_ln_linear")
+    return w16, b2
+
+
+def gemm_internal(a, w, epilogue, block_n, out=None, bias=None, gamma=None, hi=None, lo=None, stats=None, rowadd=None,
+                  rows_in=0):
+    """The GEMM a [M, K] @ w [N, K]^T with an internal epilogue (6 split residual update of (hi, lo) + stats, 7 / 8
+    folded-LN consumer from stats, 9 fp16 row add); stats fp32 [M, slots, 2]."""
+    _cuda(a, w, out, bias, gamma, hi, lo, stats, rowadd)
+    _contig(stats, rowadd, bias, gamma)
+    assert a.dtype == w.dtype == torch.float16 and a.stride(1) == 1 and w.stride(1) == 1
+    assert out is None or (out.dtype == torch.float16 and out.stride(1) == 1)
+    assert hi is None or (hi.dtype == lo.dtype == torch.float16 and hi.stride() == lo.stride() and hi.stride(1) == 1)
+    M, K = a.shape
+    N = w.shape[0]
+    rc = _lib.load().mhmr_op_gemm_internal(
+        ptr(a), c_int64(a.stride(0)), ptr(w), c_int64(w.stride(0)), c_int(M), c_int(N), c_int(K), c_int(epilogue),
+        ptr(bias), ptr(gamma), ptr(hi), ptr(lo), c_int64(hi.stride(0) if hi is not None else 0), ptr(stats),
+        c_int(stats.shape[1] if stats is not None else 0), ptr(rowadd), c_int(rows_in), ptr(out),
+        c_int64(out.stride(0) if out is not None else 0), c_int(block_n), stream_ptr())
+    check(rc, "mhmr_op_gemm_internal")
+    return out
+
+
+def camera_ctx(K, freqs, ctx, res, col0, pad_cols):
+    """K^-1 (returned, [B, 3, 3]) and the fp16 camera features of every cell into ctx[:, col0 : col0 + pad_cols]."""
+    _cuda(K, freqs, ctx)
+    _contig(K, freqs)
+    assert ctx.dtype == torch.float16 and ctx.stride(1) == 1
+    B = K.shape[0]
+    kinv = torch.empty(B, 3, 3, device=K.device)
+    rc = _lib.load().mhmr_op_camera_ctx(ptr(K), c_int(B), ptr(freqs), ptr(kinv), ptr(ctx), c_int64(ctx.stride(0)),
+                                        c_int(res), c_int(col0), c_int(pad_cols), stream_ptr())
+    check(rc, "mhmr_op_camera_ctx")
+    return kinv
+
+
+def rowdot_sigmoid(hid, D, w, b, scores, logits=None, clamp=True):
+    """scores[r] = sigmoid(hid[r, :D] . w + b) (clamped to [1e-4, 1 - 1e-4] with `clamp`) for r < scores.numel()."""
+    _cuda(hid, w, b, scores, logits)
+    _contig(w, b, scores, logits)
+    assert hid.dtype == torch.float16 and hid.stride(1) == 1
+    rc = _lib.load().mhmr_op_rowdot_sigmoid(ptr(hid), c_int64(hid.stride(0)), ptr(w), ptr(b), ptr(scores), ptr(logits),
+                                            c_int(1 if clamp else 0), c_int(scores.numel()), c_int(D), stream_ptr())
+    check(rc, "mhmr_op_rowdot_sigmoid")
+
+
+def person_gather(z32, kinv, freqs, cq_x, cq_y, cv_x, cv_y, det_b, det_y, det_x, count, max_persons, res, zc, query,
+                  vals, xr=None, norm=(None, None)):
+    """Per-person feature rows zc [Pm, D], queries and values [Pm, ldq] (pitch = query's stride)."""
+    _cuda(z32, kinv, freqs, cq_x, cq_y, cv_x, cv_y, zc, query, vals, xr, *norm)
+    _f32(z32, kinv, cq_x, cq_y, cv_x, cv_y, zc, query, vals, xr)
+    _contig(z32, kinv, freqs, cq_x, cq_y, cv_x, cv_y, zc, xr, *norm)
+    _i32(det_b, det_y, det_x, count)
+    assert query.stride() == vals.stride()
+    D = z32.shape[-1]
+    rc = _lib.load().mhmr_op_person_gather(
+        ptr(z32), ptr(xr), ptr(norm[0]), ptr(norm[1]), ptr(kinv), ptr(freqs), ptr(cq_x), ptr(cq_y), ptr(cv_x),
+        ptr(cv_y), ptr(det_b), ptr(det_y), ptr(det_x), ptr(count), c_int(max_persons), c_int(res), c_int(D), ptr(zc),
+        ptr(query), ptr(vals), c_int(query.stride(0)), stream_ptr())
+    check(rc, "mhmr_op_person_gather")
+
+
+def refine_prepare(img, rowadd, det_b, det_y, det_x, count, max_persons, rowidx, patch, xr, lut=None, n_cls=0,
+                   cls_pos=None, rows_out=None):
+    """Refinement inputs of n_cls cls rows and max_persons person rows: rowidx int32, patch fp32 [R, ldp], xr [R, D];
+    img fp32 [B, 3, S, S] or uint8 [B, S, S, 3] with `lut`."""
+    _cuda(img, rowadd, lut, cls_pos, rowidx, patch, xr, rows_out)
+    _contig(img, rowadd, lut, cls_pos, rowidx, xr)
+    _i32(det_b, det_y, det_x, count)
+    assert patch.stride(1) == 1
+    u8 = img.dtype == torch.uint8
+    S = img.shape[2] if u8 else img.shape[3]
+    rc = _lib.load().mhmr_op_refine_prepare(
+        ptr(None if u8 else img), ptr(img if u8 else None), ptr(lut), c_int(S), ptr(rowadd), c_int(xr.shape[1]),
+        ptr(det_b), ptr(det_y), ptr(det_x), ptr(count), c_int(max_persons), c_int(n_cls), ptr(cls_pos), ptr(rows_out),
+        ptr(rowidx), ptr(patch), c_int(patch.stride(0)), ptr(xr), stream_ptr())
+    check(rc, "mhmr_op_refine_prepare")
+
+
+def kv_add_rows(kv, dkv, det_b, det_y, det_x, count, max_persons, res):
+    """kv[b*res*res + cell, :ncols] += dkv[p] once per distinct cell of the persons p < count (in place)."""
+    _cuda(kv, dkv, det_b, det_y, det_x, count)
+    _f32(kv, dkv)
+    _contig(dkv)
+    _i32(det_b, det_y, det_x, count)
+    rc = _lib.load().mhmr_op_kv_add_rows(ptr(kv), c_int64(kv.stride(0)), ptr(dkv), c_int(dkv.shape[1]), ptr(det_b),
+                                         ptr(det_y), ptr(det_x), ptr(count), c_int(max_persons), c_int(res),
+                                         stream_ptr())
+    check(rc, "mhmr_op_kv_add_rows")
+
+
+def cls_gather(x, T, B, D, xlo=None):
+    """Rows b*T (b < B) of the residual stream x [B*T, ld] (fp32, or the fp16 hi plane with `xlo`) -> fp32 [B, D]."""
+    _cuda(x, xlo)
+    assert x.stride(1) == 1 and (xlo is None or xlo.stride() == x.stride())
+    out = torch.empty(B, D, device=x.device)
+    rc = _lib.load().mhmr_op_cls_gather(ptr(x), ptr(xlo), c_int64(x.stride(0)), c_int(T), c_int(B), c_int(D), ptr(out),
+                                        stream_ptr())
+    check(rc, "mhmr_op_cls_gather")
+    return out
+
+
+def anny_gather(z32, pos, det_b, det_y, det_x, count, max_persons, res, zc, xa, xr=None, norm=(None, None)):
+    """Anny decoder inputs: zc [Pm, D] (bulk row, or the final norm of xr), xa [Pm, dim] = pos[cell]."""
+    _cuda(z32, pos, zc, xa, xr, *norm)
+    _contig(z32, pos, zc, xa, xr, *norm)
+    _i32(det_b, det_y, det_x, count)
+    rc = _lib.load().mhmr_op_anny_gather(ptr(z32), ptr(xr), ptr(norm[0]), ptr(norm[1]), ptr(pos), ptr(det_b),
+                                         ptr(det_y), ptr(det_x), ptr(count), c_int(max_persons), c_int(res),
+                                         c_int(z32.shape[-1]), c_int(xa.shape[1]), ptr(zc), ptr(xa), stream_ptr())
+    check(rc, "mhmr_op_anny_gather")
+
+
+def anny_place(bone_poses, transl, K_det, center, v3d, j3d, j2d, transl_pelvis, v2d=None):
+    """Places P bodies: v3d [P, V, 3] in place, j3d [P, J, 3] from bone_poses [P, J, 4, 4], v2d / j2d, transl_pelvis."""
+    _cuda(bone_poses, transl, K_det, v3d, j3d, j2d, transl_pelvis, v2d)
+    _contig(bone_poses, transl, K_det, v3d, j3d, j2d, transl_pelvis, v2d)
+    P, J = bone_poses.shape[:2]
+    V = v3d.shape[1]
+    rc = _lib.load().mhmr_op_anny_place(ptr(bone_poses), ptr(transl), ptr(K_det), c_int(center), c_int(P), c_int(V),
+                                        c_int(J), ptr(v3d), ptr(j3d), ptr(v2d), ptr(j2d), ptr(transl_pelvis),
+                                        stream_ptr())
+    check(rc, "mhmr_op_anny_place")

@@ -139,6 +139,39 @@ def test_num_betas_11_layer(cuda_device):
     assert not bad, bad
 
 
+def test_forced_persons_sharing_a_cell(cuda_device):
+    """Two forced persons on the same cell (b, y, x): the reference adds the learned values to that context cell with a
+    non-accumulating index_put (model.py:517), so the cell holds ctx + v once, not ctx + 2v."""
+    from multihmr_b200 import synth
+    from multihmr_b200.model import Model
+
+    backbone, S, B, seed = "dinov2_vits14", 224, 2, 43
+    sd = synth.make_state_dict(backbone, S, seed=seed)
+    # value embeddings 5x their synthetic scale: adding them once or twice at the shared cell then moves every person
+    # output of image 1 by 3.5e-3 (dist) to 1.5e-2 (v3d), well outside the 1e-3 tolerance (checked below)
+    h = "x_attention_head."
+    for n in ("cross_values_x", "cross_values_y"):
+        sd[h + n] = 5.0 * sd[h + n]
+    bm = synth.make_body_model(seed)
+    x, K = synth.make_images(B, S, seed), synth.make_cameras(B, S, jitter=True, seed=seed)
+    t = lambda v: torch.tensor(v, dtype=torch.int64)
+    idx = (t([0, 0, 1, 1]), t([3, 10, 5, 5]), t([4, 2, 7, 7]), t([0, 0, 0, 0]))  # image 1: both persons on (5, 7)
+    keys = ["rotmat", "shape", "expression", "dist", "v3d", "j3d", "transl"]
+    ref = _oracle_cpu(sd, bm, backbone, S, x, K, idx=idx, is_training=True)
+    # sensitivity: image 1 holds only the shared cell, so doubling the value tables is ctx + 2v there
+    sd2 = dict(sd)
+    for n in ("cross_values_x", "cross_values_y"):
+        sd2[h + n] = 2.0 * sd[h + n]
+    twice = _oracle_cpu(sd2, bm, backbone, S, x, K, idx=idx, is_training=True)
+    caught = pu.compare({k: twice[k][2:] for k in keys}, {k: ref[k][2:] for k in keys}, keys)
+    assert [k for k, _, _ in caught] == keys, caught
+    m = Model(backbone=backbone, img_size=S, max_batch=B, max_persons=8, body_model=bm)
+    m.load_state_dict(sd)
+    out = m(x, idx=idx, K=K, is_training=True)
+    bad = pu.compare(out, {k: v.float() for k, v in ref.items()}, keys, verbose=True)
+    assert not bad, bad
+
+
 def test_nms_off_threshold_list_and_partial_batch(cuda_device):
     """nms_kernel_size=1 (forward_model's default, demo.py:110), det_thresh given as a list
     (model.py:614-615), and a batch smaller than max_batch."""
