@@ -395,6 +395,50 @@ int mhmr_eval_match_2d(const float* pred_j2d, const float* gt_j2d, const uint8_t
 int mhmr_eval_points_error(const float* pred, const float* pred_center, const float* gt, const float* gt_center,
                            const int32_t* pairs, const int32_t* n_pairs, int max_pairs, int n_points, float* err_mm,
                            float* pa_err_mm, void* stream);
+/* Sparse regression of matched pairs, centre first (train.py:375-384, :406-415):
+ *     out[m, i] = A[r] . (X[s] - center[s]) - (root >= 0 ? A[root] . (X[s] - center[s]) : 0)
+ * with s = pairs[2m + side], r = rows[i] (rows NULL: r = i and R_out = R), for m < *n_pairs (m < max_pairs <= 48).
+ * Device data is not range-checked here: rows[i] and root must lie in [0, R), pairs / n_pairs must come from
+ * mhmr_eval_match_2d (or index X and center), CSR columns must lie in [0, N).
+ * A [R, N] in CSR form (rowptr [R+1], col, val; rows need not sum to 1), X [*, N, 3], center [*, 3] nullable,
+ * out [max_pairs, R_out, 3].  K [*, 3, 3] and out2d [max_pairs, R_out, 2] (both or neither) add the perspective
+ * projection of the outputs (utils/camera.py:14-27).  Serves the SMPL-X -> SMPL transfer (smplx2smpl.pkl), the H36M
+ * joints of 3DPW (J_regressor_h36m, rows H36M_TO_J14, root 0) and the EHF joints (J_regressor @ vertices). */
+int mhmr_eval_regress(const int32_t* rowptr, const int32_t* col, const float* val, int R, int N, const int32_t* rows,
+                      int R_out, int root, const float* X, const float* center, const int32_t* pairs, int side,
+                      const int32_t* n_pairs, int max_pairs, const float* K, float* out, float* out2d, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Ground-truth body models (Trainer.prepare_gt, train.py:58-134): the raw `smplx` forward with `transl`, as
+ * smplx.create(SMPLX_DIR, 'smpl', gender=...) and smplx.create(..., 'smplx', gender='neutral', use_pca=False,
+ * flat_hand_mean=True, num_betas=11) compute it (train.py:41-43).  Independent of the engine handle.
+ *   MHMR_BODY_SMPL   24 joints, 207 pose features; joints = 24 LBS + 21 vertex-picked = 45; no expression
+ *   MHMR_BODY_SMPLX  55 joints, 486 pose features, 10 expression coefficients; 55 + 21 + 51 landmarks = 127
+ * ---------------------------------------------------------------------------------------------- */
+#define MHMR_BODY_SMPL 0
+#define MHMR_BODY_SMPLX 1
+typedef struct mhmr_body mhmr_body;
+/* Arrays (host or device, fp32 / int32; the handle keeps its own folded copies): v_template [V,3], shapedirs
+ * [V,3,num_betas], expr_dirs [V,3,10] (SMPL-X), posedirs [9(NJ-1), 3V], J_regressor [NJ,V], lbs_weights [V,NJ],
+ * parents [NJ] (parents[0] = -1, parents[j] < j), extra_joints_idxs [21] (smplx.vertex_ids order), lmk_tri [51*3] and
+ * lmk_bary [51*3] (SMPL-X).  Every array is first copied into device memory (cudaMemcpyDefault), so host and device
+ * pointers are both accepted.  Sizes (9 (NJ-1) + num_betas + expression <= 512) and table ranges are checked before
+ * any kernel is launched; synchronises `stream`. */
+int mhmr_body_create(int kind, int num_verts, int num_betas, int max_persons, const float* v_template,
+                     const float* shapedirs, const float* expr_dirs, const float* posedirs, const float* J_regressor,
+                     const float* lbs_weights, const int32_t* parents, const int32_t* extra_joints_idxs,
+                     const int32_t* lmk_tri, const float* lmk_bary, void* stream, mhmr_body** out);
+int mhmr_body_destroy(mhmr_body* h);
+/* Any output pointer may be NULL.  num_joints_out = joints per person of mhmr_body_forward (45 or 127). */
+int mhmr_body_info(const mhmr_body* h, int* num_verts, int* num_joints_out, int* num_pose_joints, int* num_betas,
+                   int* num_expression);
+/* P <= max_persons persons, device pointers: full_pose [P,NJ,3] in smplx order (SMPL: global, body 23; SMPL-X:
+ * global, body 21, jaw, leye, reye, lhand 15, rhand 15), betas [P,num_betas], expression [P,10] (SMPL-X; NULL for
+ * SMPL), transl [P,3], K [P,3,3].  Outputs v3d [P,V,3], v2d [P,V,2] (nullable), j3d / j2d [P,num_joints_out,3 / 2],
+ * transl_pelvis [P,3] = j3d[:, 0]; vertices and joints include transl, j2d = perspective_projection(j3d, K). */
+int mhmr_body_forward(mhmr_body* h, int P, const float* full_pose, const float* betas, const float* expression,
+                      const float* transl, const float* K, float* v3d, float* v2d, float* j3d, float* j2d,
+                      float* transl_pelvis, void* stream);
 
 /* Kernel launches enqueued by the last mhmr_forward (bench.py's `gpu_launches`). */
 int mhmr_last_launch_count(mhmr_engine* h);

@@ -97,6 +97,100 @@ def body_model_from_smplx_npz(path: str, num_betas: int = 10) -> dict:
     }
 
 
+# smplx.vertex_ids.vertex_ids['smplh'] in the order of smplx.vertex_joint_selector.VertexJointSelector: face (nose,
+# reye, leye, rear, lear), feet (LBigToe, LSmallToe, LHeel, RBigToe, RSmallToe, RHeel), then the finger tips of the
+# left and the right hand (thumb, index, middle, ring, pinky).  [3P-memory]: recalled from the smplx package, which is
+# not installed here; re-verify against smplx/vertex_ids.py before relying on SMPL joints 24..44.
+SMPL_EXTRA_JOINTS_IDXS = [332, 6260, 2800, 4071, 583, 3216, 3226, 3387, 6617, 6624, 6787,
+                          2746, 2319, 2445, 2556, 2673, 6191, 5782, 5905, 6016, 6133]
+
+# Classes a body-model pickle may name: numpy / scipy containers, and chumpy's array wrapper, which is replaced by the
+# ndarray it holds (chumpy is not a dependency).  Anything else is refused.
+_PICKLE_NUMPY = {("numpy", "ndarray"), ("numpy", "dtype"), ("numpy.core.multiarray", "_reconstruct"),
+                 ("numpy._core.multiarray", "_reconstruct"), ("numpy.core.multiarray", "scalar"),
+                 ("numpy._core.multiarray", "scalar"), ("copyreg", "_reconstructor"), ("copy_reg", "_reconstructor"),
+                 ("builtins", "object"), ("__builtin__", "object"), ("_codecs", "encode"),
+                 ("builtins", "set"), ("__builtin__", "set"), ("builtins", "frozenset"), ("__builtin__", "frozenset")}
+_PICKLE_SCIPY = {"csc_matrix", "csr_matrix"}
+
+
+class _ChumpyArray:
+    """Stand-in for a pickled chumpy object: keeps its state; `_unchumpy` swaps it for the ndarray it wraps."""
+
+    def __init__(self, *args, **kwargs):
+        pass
+
+    def __setstate__(self, state):
+        self.__dict__.update(state if isinstance(state, dict) else {})
+
+
+class _BodyModelUnpickler:
+    @staticmethod
+    def make(fh):
+        import pickle
+
+        class U(pickle.Unpickler):
+            def find_class(self, module, name):
+                if (module, name) in _PICKLE_NUMPY:
+                    return super().find_class(module, name)
+                if module.split(".")[0] == "scipy" and module.startswith("scipy.sparse") and name in _PICKLE_SCIPY:
+                    return super().find_class(module, name)
+                if module.split(".")[0] == "chumpy":
+                    return _ChumpyArray
+                raise pickle.UnpicklingError(f"refusing to unpickle {module}.{name}")
+
+        return U(fh, encoding="latin1")
+
+
+def _unchumpy(obj):
+    if isinstance(obj, _ChumpyArray):
+        if "x" not in obj.__dict__:
+            raise ValueError("chumpy object without a stored value ('x')")
+        return np.asarray(_unchumpy(obj.__dict__["x"]))
+    if isinstance(obj, dict):
+        return {k: _unchumpy(v) for k, v in obj.items()}
+    return obj
+
+
+def load_body_model_pickle(path: str) -> dict:
+    """A body-model pickle (SMPL_*.pkl, smplx2smpl.pkl) through a restricted unpickler: numpy and scipy.sparse
+    containers only, chumpy arrays mapped to their ndarray (the layout SMPL's python-2 pickles use: chumpy.ch.Ch with
+    its value in 'x' -- [3P-memory], re-verify against chumpy/ch.py)."""
+    with open(path, "rb") as fh:
+        return _unchumpy(_BodyModelUnpickler.make(fh).load())
+
+
+def body_model_from_smpl_pkl(path: str, num_betas: int = 10) -> dict:
+    """Reads `SMPL_{MALE,FEMALE}.pkl` the way `smplx.create(SMPLX_DIR, 'smpl', gender=...)` does (train.py:42-43):
+    shapedirs[..., :num_betas], posedirs [V,3,207] -> [207, 3V], J_regressor densified, kinematic parents from
+    kintree_table[0], the 21 vertex-picked joints of smplx.vertex_ids['smplh']."""
+    d = load_body_model_pickle(path)
+    t = lambda a, dt=torch.float32: torch.as_tensor(np.asarray(a)).to(dt)
+    jr = d["J_regressor"]
+    jr = jr.toarray() if hasattr(jr, "toarray") else np.asarray(jr)
+    pd = np.asarray(d["posedirs"])
+    parents = t(np.asarray(d["kintree_table"])[0].astype(np.int64), torch.int64)
+    parents[0] = -1
+    return {
+        "v_template": t(d["v_template"]), "shapedirs": t(d["shapedirs"])[..., :num_betas],
+        "posedirs": t(pd.reshape(-1, pd.shape[-1]).T.copy()), "J_regressor": t(jr), "parents": parents,
+        "lbs_weights": t(d["weights"]), "faces": t(np.asarray(d["f"]).astype(np.int64), torch.int64),
+        "extra_joints_idxs": torch.tensor(SMPL_EXTRA_JOINTS_IDXS, dtype=torch.int64),
+        "num_verts": int(np.asarray(d["v_template"]).shape[0]),
+    }
+
+
+def load_smplx2smpl(path: str) -> np.ndarray:
+    """`smplx2smpl.pkl['matrix']` [6890, 10475] as fp32 (train.py:44-45)."""
+    m = load_body_model_pickle(path)["matrix"]
+    return np.asarray(m.toarray() if hasattr(m, "toarray") else m, dtype=np.float32)
+
+
+def load_j_regressor_h36m(path: str) -> np.ndarray:
+    """`J_regressor_h36m.npy` [17, 6890] (train.py:400)."""
+    return np.load(path).astype(np.float32)
+
+
 def load_model(model_name, device=torch.device("cuda"), max_batch=8, max_persons=None, body_model=None):
     """Open a checkpoint, build the engine from its saved arguments, load the weights (demo.py:70-106).
     No download is attempted (this build has no network): a missing file is an error.  A checkpoint whose name

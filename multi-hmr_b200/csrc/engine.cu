@@ -428,13 +428,13 @@ int finalize_body(mhmr_engine* e, cudaStream_t st) {
   TRY(repack_f32(sd, nb, 0, sfull, L, 0, 3 * V, nb, false, st));
   TRY(repack_f32(ed, 10, 0, sfull, L, nb, 3 * V, 10, false, st));
   TRY(e->alloc(&PDX, static_cast<size_t>(486 + L) * bm.ldp));
-  TRY(smplx_build_pdx(pd, sfull, L, V, bm.ldp, PDX, st));
+  TRY(smplx_build_pdx(pd, sfull, 486, L, V, bm.ldp, PDX, st));
   TRY(e->alloc(&vtp, bm.ldp));
   MHMR_CUDA_CHECK(cudaMemcpyAsync(vtp, vt, 3ll * V * 4, cudaMemcpyDeviceToDevice, st));
   TRY(e->alloc(&Jt, 55 * 3));
-  TRY(smplx_fold_jreg(jr, vt, V, 3, Jt, st));
+  TRY(smplx_fold_jreg(jr, vt, 55, V, 3, Jt, st));
   TRY(e->alloc(&Jd, static_cast<size_t>(55) * 3 * L));
-  TRY(smplx_fold_jreg(jr, sfull, V, 3 * L, Jd, st));
+  TRY(smplx_fold_jreg(jr, sfull, 55, V, 3 * L, Jd, st));
   // skinning weights padded to whole 72-vertex tiles (the vertex kernel bulk-copies one tile per CTA)
   const int tv = smplx_tile_verts();
   const int Vpad = (V + tv - 1) / tv * tv;

@@ -111,35 +111,43 @@ int anny_place(const float* bone_poses, const float* transl, const float* K_det,
 // ---- smplx_lbs.cu ----------------------------------------------------------------------------
 struct SmplxDeviceModel {
   int V = 0;            // vertices
-  int L = 0;            // num_betas + 10 shape/expression coefficients
+  int L = 0;            // num_betas + expression coefficients (10 for SMPL-X, 0 for SMPL)
   int num_betas = 10;
   int center_idx = 15;  // person_center joint ('head')
+  int num_joints = 55;  // kinematic joints (SMPL-X 55, SMPL 24)
+  int pose_feat = 486;  // pose-corrective features = 9 (num_joints - 1)
+  int n_lmk = 51;       // static face landmarks appended to the joints (SMPL: 0)
   int ldp = 0;          // PDX / vt row pitch: 3V rounded up to 4
-  const float* PDX = nullptr;          // [486 + L, ldp]
+  const float* PDX = nullptr;          // [pose_feat + L, ldp]
   const float* vt = nullptr;           // [ldp] v_template flattened
-  const float* lbs_weights_padded = nullptr;  // [ceil(V/72)*72, 55], zero rows beyond V
+  const float* lbs_weights_padded = nullptr;  // [ceil(V/72)*72, num_joints], zero rows beyond V
   CUtensorMap tmPDX;                   // TMA descriptor of PDX (boxes of 16 rows x 220 columns)
-  const float* Jt = nullptr;           // [55, 3]   J_regressor . v_template
-  const float* Jdirs = nullptr;        // [55*3, L] J_regressor . shapedirs
-  const int* parents = nullptr;        // [55]
+  const float* Jt = nullptr;           // [num_joints, 3]   J_regressor . v_template
+  const float* Jdirs = nullptr;        // [num_joints*3, L] J_regressor . shapedirs
+  const int* parents = nullptr;        // [num_joints]
   const int* extra_idx = nullptr;      // [21] vertex-picked joints
-  const int* lmk_tri = nullptr;        // [51, 3] vertex ids of the landmark faces
-  const float* lmk_bary = nullptr;     // [51, 3]
+  const int* lmk_tri = nullptr;        // [n_lmk, 3] vertex ids of the landmark faces
+  const float* lmk_bary = nullptr;     // [n_lmk, 3]
 };
 struct SmplxScratch {
-  float* cf = nullptr;      // [max_persons, 486 + L]
-  float* Amat = nullptr;    // [max_persons, 55, 12]
+  float* cf = nullptr;      // [max_persons, pose_feat + L]
+  float* Amat = nullptr;    // [max_persons, num_joints, 12]
   float* xf = nullptr;      // [max_persons, 16]
-  float* jposed = nullptr;  // [max_persons, 55, 3]
+  float* jposed = nullptr;  // [max_persons, num_joints, 3]
 };
 int smplx_make_tmap(SmplxDeviceModel* bm);
 int smplx_tile_verts();
-int smplx_build_pdx(const float* posedirs, const float* sdirs_full, int L, int V, int ldp, float* PDX,
+int smplx_build_pdx(const float* posedirs, const float* sdirs_full, int PF, int L, int V, int ldp, float* PDX,
                     cudaStream_t st);
-int smplx_fold_jreg(const float* Jr, const float* M, int V, int Q, float* out, cudaStream_t st);
+int smplx_fold_jreg(const float* Jr, const float* M, int NJ, int V, int Q, float* out, cudaStream_t st);
 int smplx_forward(const SmplxDeviceModel& bm, const float* rotvec, const float* shape, const float* expr,
                   const float* transl, const float* K_det, const int* count, int max_persons,
                   SmplxScratch& ws, float* v3d, float* v2d, float* j3d, float* j2d, float* transl_pelvis,
                   cudaStream_t st);
+// The raw body model (smplx.SMPL / smplx.SMPLX forward with transl): full_pose [P, num_joints, 3] in smplx order,
+// betas [P, num_betas], expr [P, L - num_betas] (nullable when that is 0), transl [P, 3], K [P, 3, 3] for j2d / v2d.
+int body_forward_raw(const SmplxDeviceModel& bm, const float* full_pose, const float* betas, const float* expr,
+                     const float* transl, const float* K, const int* count, int max_persons, SmplxScratch& ws,
+                     float* v3d, float* v2d, float* j3d, float* j2d, float* transl_pelvis, cudaStream_t st);
 
 }  // namespace mhmr

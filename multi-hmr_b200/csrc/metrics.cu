@@ -6,6 +6,8 @@
 //   mhmr_eval_points_error  per matched pair: mean point error in mm (PVE / MPJPE, train.py:387,419) and the same
 //                           after the Procrustes similarity alignment (PA-PVE / PA-MPJPE, train.py:391-393,
 //                           roma.rigid_points_registration(compute_scaling=True))
+//   mhmr_eval_regress       per matched pair: a sparse regressor applied to the centred points (SMPL-X -> SMPL
+//                           transfer, train.py:383-384; H36M joints, :406-415; EHF joints, :73)
 // The matched pairs stay on the device between the two calls (no host round trip inside one image's evaluation).
 // Latency-bound kernels on a few persons: one CTA for the matching, one CTA per matched pair for the errors.
 #include "kernels.cuh"
@@ -264,9 +266,78 @@ points_error_kernel(const float* __restrict__ pred, const float* __restrict__ pr
   if (threadIdx.x == 0) pa_err_mm[m] = static_cast<float>(pe / n * 1000.0);
 }
 
+// One warp per output row i of pair m: y_r = sum_k A[r, k] (X[src, k] - c[src]) for r = rows[i] (or i), minus y_root when
+// root >= 0; src = pairs[2m + side].  Optional projection out2d[m, i] = (K[src] . (y / y_z))[:2] (utils/camera.py:14-27).
+__device__ __forceinline__ void regress_row(const int* __restrict__ rowptr, const int* __restrict__ col,
+                                            const float* __restrict__ val, int r, const float* __restrict__ X,
+                                            const float c[3], int lane, float y[3]) {
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+  for (int e = rowptr[r] + lane; e < rowptr[r + 1]; e += 32) {
+    const int k = col[e];
+    const float w = val[e];
+    a0 = fmaf(w, X[3 * k] - c[0], a0);
+    a1 = fmaf(w, X[3 * k + 1] - c[1], a1);
+    a2 = fmaf(w, X[3 * k + 2] - c[2], a2);
+  }
+  y[0] = warp_sum(a0);
+  y[1] = warp_sum(a1);
+  y[2] = warp_sum(a2);
+}
+
+__global__ void __launch_bounds__(256)
+regress_pairs_kernel(const int* __restrict__ rowptr, const int* __restrict__ col, const float* __restrict__ val,
+                     const int* __restrict__ rows, int R_out, int root, int N, const float* __restrict__ X,
+                     const float* __restrict__ center, const int* __restrict__ pairs, int side,
+                     const int* __restrict__ n_pairs, const float* __restrict__ K, float* __restrict__ out,
+                     float* __restrict__ out2d) {
+  const int m = blockIdx.y;
+  if (m >= *n_pairs) return;
+  const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (i >= R_out) return;
+  const int src = pairs[2 * m + side];
+  const float* Xs = X + static_cast<int64_t>(src) * N * 3;
+  float c[3] = {0.f, 0.f, 0.f};
+  if (center != nullptr) for (int q = 0; q < 3; ++q) c[q] = center[src * 3 + q];
+  float y[3];
+  regress_row(rowptr, col, val, rows != nullptr ? rows[i] : i, Xs, c, lane, y);
+  if (root >= 0) {
+    float y0[3];
+    regress_row(rowptr, col, val, root, Xs, c, lane, y0);
+    for (int q = 0; q < 3; ++q) y[q] -= y0[q];
+  }
+  if (lane != 0) return;
+  float* o = out + (static_cast<int64_t>(m) * R_out + i) * 3;
+  o[0] = y[0]; o[1] = y[1]; o[2] = y[2];
+  if (out2d != nullptr) {
+    const float* Kd = K + src * 9;
+    const float u = y[0] / y[2], w = y[1] / y[2], one = y[2] / y[2];
+    out2d[(static_cast<int64_t>(m) * R_out + i) * 2] = Kd[0] * u + Kd[1] * w + Kd[2] * one;
+    out2d[(static_cast<int64_t>(m) * R_out + i) * 2 + 1] = Kd[3] * u + Kd[4] * w + Kd[5] * one;
+  }
+}
+
 }  // namespace
 
 extern "C" {
+
+int mhmr_eval_regress(const int32_t* rowptr, const int32_t* col, const float* val, int R, int N, const int32_t* rows,
+                      int R_out, int root, const float* X, const float* center, const int32_t* pairs, int side,
+                      const int32_t* n_pairs, int max_pairs, const float* K, float* out, float* out2d, void* stream) {
+  MHMR_REQUIRE(rowptr != nullptr && col != nullptr && val != nullptr && X != nullptr && pairs != nullptr &&
+                   n_pairs != nullptr && out != nullptr, "null argument");
+  MHMR_REQUIRE(R >= 1 && N >= 1 && R_out >= 1, "empty regressor");
+  MHMR_REQUIRE(rows != nullptr || R_out == R, "without a row list every row of A is an output row");
+  MHMR_REQUIRE(root >= -1 && root < R, "root row out of range");
+  MHMR_REQUIRE(side == 0 || side == 1, "side selects the prediction (0) or ground-truth (1) column of pairs");
+  MHMR_REQUIRE(max_pairs >= 1 && max_pairs <= kMaxPersons, "regression handles up to 48 pairs per image");
+  MHMR_REQUIRE((out2d == nullptr) == (K == nullptr), "K and out2d go together");
+  const dim3 grid((R_out + 7) / 8, max_pairs);
+  regress_pairs_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      rowptr, col, val, rows, R_out, root, N, X, center, pairs, side, n_pairs, K, out, out2d);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
+}
+
 
 int mhmr_eval_match_2d(const float* pred_j2d, const float* gt_j2d, const uint8_t* valid_mask, int P, int G, int J,
                        float iou_thresh, int32_t* pairs, int32_t* n_pairs, int32_t* pred_to_gt, int32_t* gt_to_pred,

@@ -32,31 +32,37 @@ __device__ __forceinline__ int full_pose_source(int j) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Per person: Rodrigues x55, pose features, joints, kinematic chain, skinning transforms, root placement.
+// Per person: Rodrigues xNJ, pose features, joints, kinematic chain, skinning transforms, placement.
+// kRaw = false: the engine's SMPL-X layer -- rotvec [P, 53, 3] in the reference's order, global orient and eyes zero
+//   inside the body model, root placed by R (x - pelvis) - center (blocks/smpl_layer.py:88-140).
+// kRaw = true: the raw `smplx` body model as Trainer.prepare_gt calls it (train.py:76-109) -- rotvec is the full
+//   pose [P, NJ, 3] in smplx order with the global rotation inside the chain, as `lbs` does; placement is the
+//   identity (R = I, pelvis = 0, centre = 0), so the vertex / joints kernels add `transl` and nothing else.
 // ------------------------------------------------------------------------------------------------
+template <int NJ, int PF, bool kRaw>
 __global__ void __launch_bounds__(64)
-smplx_prep_kernel(const float* __restrict__ rotvec, const float* __restrict__ shape,
-                  const float* __restrict__ expr, const float* __restrict__ transl,
-                  const float* __restrict__ Jt, const float* __restrict__ Jdirs,
-                  const int* __restrict__ parents, const int* __restrict__ count, int num_betas,
-                  int center_idx, int KT, float* __restrict__ cf, float* __restrict__ Amat,
-                  float* __restrict__ xf, float* __restrict__ jposed) {
+body_prep_kernel(const float* __restrict__ rotvec, const float* __restrict__ shape,
+                 const float* __restrict__ expr, int n_expr, const float* __restrict__ Jt,
+                 const float* __restrict__ Jdirs, const int* __restrict__ parents, const int* __restrict__ count,
+                 int num_betas, int center_idx, int KT, float* __restrict__ cf, float* __restrict__ Amat,
+                 float* __restrict__ xf, float* __restrict__ jposed) {
+  static_assert(NJ <= 64 && PF == (NJ - 1) * 9, "one thread per joint; pose features = 9 (NJ - 1)");
   const int p = blockIdx.x;
   if (p >= *count) return;
-  __shared__ float Rs[kNJ][9];
-  __shared__ float Js[kNJ][3];
-  __shared__ float Gs[kNJ][12];
+  __shared__ float Rs[NJ][9];
+  __shared__ float Js[NJ][3];
+  __shared__ float Gs[NJ][12];
   __shared__ float beta[32];
   const int j = threadIdx.x;
-  const int L = num_betas + 10;
+  const int L = num_betas + n_expr;
   if (j < num_betas) beta[j] = shape[p * num_betas + j];
-  if (j >= 32 && j < 42) beta[num_betas + (j - 32)] = expr[p * 10 + (j - 32)];
+  if (j >= 32 && j < 32 + n_expr) beta[num_betas + (j - 32)] = expr[p * n_expr + (j - 32)];
   __syncthreads();
-  if (j < kNJ) {
+  if (j < NJ) {
     float rx = 0.f, ry = 0.f, rz = 0.f;
-    const int src = full_pose_source(j);
+    const int src = kRaw ? j : full_pose_source(j);
     if (src >= 0) {
-      const float* rv = rotvec + (static_cast<int64_t>(p) * 53 + src) * 3;
+      const float* rv = rotvec + (static_cast<int64_t>(p) * (kRaw ? NJ : 53) + src) * 3;
       rx = rv[0]; ry = rv[1]; rz = rv[2];
     }
     // smplx.lbs.batch_rodrigues: angle = || r + 1e-8 ||, axis = r / angle
@@ -86,9 +92,9 @@ smplx_prep_kernel(const float* __restrict__ rotvec, const float* __restrict__ sh
       Js[j][r] = v;
     }
   }
-  if (j < L) cf[static_cast<int64_t>(p) * KT + kPoseFeat + j] = beta[j];
+  if (j < L) cf[static_cast<int64_t>(p) * KT + PF + j] = beta[j];
   __syncthreads();
-  if (j < kNJ) {
+  if (j < NJ) {
     // kinematic chain (smplx.lbs.batch_rigid_transform): G_j = prod over the ancestors (root first) of
     // [R_i | J_i - J_parent(i)].  Every joint walks its own ancestor list (depth <= 16) independently
     // instead of one thread serialising the 55 joints; the product order equals the reference's.
@@ -124,18 +130,20 @@ smplx_prep_kernel(const float* __restrict__ rotvec, const float* __restrict__ sh
     for (int q = 0; q < 12; ++q) Gs[j][q] = G[q];
   }
   __syncthreads();
-  if (j < kNJ) {
+  if (j < NJ) {
     // A_j = G_j with translation G_t - G_R J_j; posed joint = G_t
-    float* A = Amat + (static_cast<int64_t>(p) * kNJ + j) * 12;
+    float* A = Amat + (static_cast<int64_t>(p) * NJ + j) * 12;
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
       const float g0 = Gs[j][r * 4], g1 = Gs[j][r * 4 + 1], g2 = Gs[j][r * 4 + 2];
       A[r * 4 + 0] = g0; A[r * 4 + 1] = g1; A[r * 4 + 2] = g2;
       A[r * 4 + 3] = Gs[j][r * 4 + 3] - (g0 * Js[j][0] + g1 * Js[j][1] + g2 * Js[j][2]);
-      jposed[(static_cast<int64_t>(p) * kNJ + j) * 3 + r] = Gs[j][r * 4 + 3];
+      jposed[(static_cast<int64_t>(p) * NJ + j) * 3 + r] = Gs[j][r * 4 + 3];
     }
   }
-  if (j == 63) {
+  if (kRaw) {
+    if (j < 16) xf[static_cast<int64_t>(p) * 16 + j] = (j == 0 || j == 4 || j == 8) ? 1.f : 0.f;
+  } else if (j == 63) {
     // root placement (blocks/smpl_layer.py:107-140): R = roma.rotvec_to_rotmat(pose[:,0]),
     // x -> R (x - pelvis) - center + transl, center = R (J[center_idx] - pelvis)
     const float* rv = rotvec + static_cast<int64_t>(p) * 53 * 3;
@@ -175,7 +183,7 @@ smplx_prep_kernel(const float* __restrict__ rotvec, const float* __restrict__ sh
 // One CTA per SM (72 vertices = 216 coordinate columns).  A producer warp streams this CTA's column slab
 // of PDX through a 6-stage shared-memory ring with TMA (16 rows x 220 columns per box; the 220-float pitch
 // makes the consumers' 128-bit reads conflict-free) and bulk-copies the skinning-weight tile; 432 consumer
-// threads = 54 column groups x 8 row lanes accumulate 16 persons per streamed row, so the 64 MB matrix
+// threads = 54 column groups x 8 row lanes accumulate PB = 16 persons per streamed row, so the 64 MB matrix
 // is read from HBM exactly once per forward with ~80 KB in flight per SM, decoupled from the FMA work.
 // ------------------------------------------------------------------------------------------------
 constexpr int kTV = 72;            // vertices per CTA
@@ -185,7 +193,6 @@ constexpr int kRL = 8;             // row lanes (adjacent lanes of a warp)
 constexpr int kChunkRows = 16;     // PDX rows per TMA box
 constexpr int kPitch = 220;        // floats per staged row (box inner size; 880 B)
 constexpr int kStagesV = 6;
-constexpr int kPB = 16;            // persons per pass
 constexpr int kConsumers = kCG * kRL;              // 432
 constexpr int kConsumerWarps = (kConsumers + 31) / 32;  // 14
 constexpr int kVertThreads = kConsumerWarps * 32 + 32;  // + producer warp = 480
@@ -193,22 +200,26 @@ constexpr int kKTMax = 512;        // >= 486 + 21, multiple of kChunkRows
 constexpr int kCfPitch = 20;       // floats per coefficient row (16 persons + pad: conflict-free)
 constexpr int kStageFloats = kChunkRows * kPitch;
 
+// PB persons per pass (a multiple of kRL): 16 for SMPL-X; the SMPL instance takes 8, whose 32 accumulators per
+// consumer thread fit the 128-register budget without spilling.
+template <int NJ, int PB>
 struct VertSmem {
   float stage[kStagesV][kStageFloats];   // 6 x 14080 B (TMA destinations: 128-byte aligned)
-  float Ws[kTV][kNJ];                    // skinning-weight tile (bulk copy destination, 16-byte aligned)
+  float Ws[kTV][NJ];                    // skinning-weight tile (bulk copy destination, 16-byte aligned)
   float pfs[kKTMax][kCfPitch];
-  float As[kPB][kNJ * 12];
-  float xf[kPB][16];
-  float tr[kPB][4];
-  float Kd[kPB][12];
-  float vps[kPB][kTC];
-  float outs[kPB][kTC];
-  float outs2[kPB][kTV * 2];
+  float As[PB][NJ * 12];
+  float xf[PB][16];
+  float tr[PB][4];
+  float Kd[PB][12];
+  float vps[PB][kTC];
+  float outs[PB][kTC];
+  float outs2[PB][kTV * 2];
   uint64_t full_bar[kStagesV];
   uint64_t empty_bar[kStagesV];
   uint64_t w_bar;
 };
 
+template <int NJ, int PB>
 __global__ void __launch_bounds__(kVertThreads, 1)
 smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const float* __restrict__ vt,
                     const float* __restrict__ Wl_padded, const float* __restrict__ cf,
@@ -218,7 +229,8 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
                     float* __restrict__ v2d) {
   extern __shared__ uint8_t vsmem_raw[];
   // 128-byte alignment by pointer arithmetic (keeps the shared address space: LDS/STS, not generic LD/ST)
-  VertSmem& sm = *reinterpret_cast<VertSmem*>(vsmem_raw + ((128u - (smem_u32(vsmem_raw) & 127u)) & 127u));
+  static_assert(PB % kRL == 0 && PB <= 16, "whole persons per row lane; pfs rows hold 16");
+  VertSmem<NJ, PB>& sm = *reinterpret_cast<VertSmem<NJ, PB>*>(vsmem_raw + ((128u - (smem_u32(vsmem_raw) & 127u)) & 127u));
   const int P = *count;
   if (P <= 0) return;
   const int tid = threadIdx.x;
@@ -228,7 +240,7 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
   const int nv = min(kTV, V - v0);
   const int ncol = nv * 3;
   const int n_chunks = (KT + kChunkRows - 1) / kChunkRows;
-  const int n_pass = (P + kPB - 1) / kPB;
+  const int n_pass = (P + PB - 1) / PB;
   const bool is_producer = (warp == kConsumerWarps);
 
   if (tid == 0) {
@@ -245,11 +257,11 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
     if (lane == 0) {
       tma_prefetch_desc(&tmPDX);
       // skinning-weight tile: rows v0..v0+71 of the padded [ceil(V/72)*72, 55] matrix are contiguous
-      mbar_arrive_expect_tx(&sm.w_bar, kTV * kNJ * 4);
+      mbar_arrive_expect_tx(&sm.w_bar, kTV * NJ * 4);
       asm volatile(
           "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
               smem_u32(&sm.Ws[0][0])),
-          "l"(Wl_padded + static_cast<int64_t>(v0) * kNJ), "r"(kTV * kNJ * 4), "r"(smem_u32(&sm.w_bar))
+          "l"(Wl_padded + static_cast<int64_t>(v0) * NJ), "r"(kTV * NJ * 4), "r"(smem_u32(&sm.w_bar))
           : "memory");
       // fill the ring right away: the first kStagesV boxes need no hand-shake, so the HBM stream starts
       // while the other warps are still staging the per-person coefficients
@@ -267,18 +279,18 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
   uint32_t it = 0;
 
   for (int pass = 0; pass < n_pass; ++pass) {
-    const int pb0 = pass * kPB;
-    const int np = min(kPB, P - pb0);
+    const int pb0 = pass * PB;
+    const int np = min(PB, P - pb0);
     __syncthreads();  // previous pass finished with the per-person buffers
-    for (int i = tid; i < kKTMax * kPB; i += kVertThreads) {
-      const int k = i / kPB, j = i - k * kPB;
+    for (int i = tid; i < kKTMax * PB; i += kVertThreads) {
+      const int k = i / PB, j = i - k * PB;
       sm.pfs[k][j] = (j < np && k < KT) ? cf[static_cast<int64_t>(pb0 + j) * KT + k] : 0.f;
     }
-    for (int i = tid; i < kPB * kNJ * 12; i += kVertThreads) {
-      const int j = i / (kNJ * 12), q = i - j * (kNJ * 12);
-      sm.As[j][q] = (j < np) ? Amat[static_cast<int64_t>(pb0 + j) * kNJ * 12 + q] : 0.f;
+    for (int i = tid; i < PB * NJ * 12; i += kVertThreads) {
+      const int j = i / (NJ * 12), q = i - j * (NJ * 12);
+      sm.As[j][q] = (j < np) ? Amat[static_cast<int64_t>(pb0 + j) * NJ * 12 + q] : 0.f;
     }
-    for (int i = tid; i < kPB * 16; i += kVertThreads) {
+    for (int i = tid; i < PB * 16; i += kVertThreads) {
       const int j = i >> 4, q = i & 15;
       sm.xf[j][q] = (j < np) ? xf[static_cast<int64_t>(pb0 + j) * 16 + q] : 0.f;
       if (q < 4) sm.tr[j][q] = (j < np && q < 3) ? transl[(pb0 + j) * 3 + q] : 0.f;
@@ -288,11 +300,11 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
 
     if (!is_producer) {
       // ---- consume the streamed rows: acc[i][j] += cf[j][k] * PDX[k][col + i]
-      float acc[4][kPB];
+      float acc[4][PB];
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < kPB; ++j) acc[i][j] = 0.f;
+        for (int j = 0; j < PB; ++j) acc[i][j] = 0.f;
       for (int c = 0; c < n_chunks; ++c, ++it) {
         const uint32_t s = it % kStagesV, ph = (it / kStagesV) & 1u;
         mbar_wait(&sm.full_bar[s], ph);
@@ -302,7 +314,7 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
           const int k = c * kChunkRows + row;  // rows >= KT are zero-filled by TMA, pfs rows are zero
           const float4 w = *reinterpret_cast<const float4*>(&sm.stage[s][row * kPitch + cg * 4]);
 #pragma unroll
-          for (int q = 0; q < kPB / 4; ++q) {
+          for (int q = 0; q < PB / 4; ++q) {
             const float4 cc = *reinterpret_cast<const float4*>(&sm.pfs[k][q * 4]);
             const float cj[4] = {cc.x, cc.y, cc.z, cc.w};
 #pragma unroll
@@ -321,7 +333,7 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < kPB; ++j) {
+        for (int j = 0; j < PB; ++j) {
           float v = acc[i][j];
           v += __shfl_xor_sync(0xffffffffu, v, 1);
           v += __shfl_xor_sync(0xffffffffu, v, 2);
@@ -330,8 +342,8 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
         }
       if (active) {
 #pragma unroll
-        for (int j = 0; j < kPB; ++j) {
-          if ((j >> 1) == r) {
+        for (int j = 0; j < PB; ++j) {
+          if (j / (PB / kRL) == r) {
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const int cc = cg * 4 + i;
@@ -355,11 +367,11 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
     __syncthreads();
 
     // ---- skinning + root placement + projection, one (vertex, person) pair per thread-iteration
-    for (int i = tid; i < kTV * kPB; i += kVertThreads) {
+    for (int i = tid; i < kTV * PB; i += kVertThreads) {
       const int j = i / kTV, v = i - j * kTV;
       if (v >= nv || j >= np) continue;
       float4 T0 = make_float4(0.f, 0.f, 0.f, 0.f), T1 = T0, T2 = T0;
-      for (int jj = 0; jj < kNJ; ++jj) {
+      for (int jj = 0; jj < NJ; ++jj) {
         const float w = sm.Ws[v][jj];
         const float4* A = reinterpret_cast<const float4*>(&sm.As[j][jj * 12]);
         const float4 a0 = A[0], a1 = A[1], a2 = A[2];
@@ -387,12 +399,12 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
       sm.outs2[j][v * 2 + 1] = Kd[3] * u + Kd[4] * w_ + Kd[5] * one;
     }
     __syncthreads();
-    for (int i = tid; i < kPB * kTC; i += kVertThreads) {
+    for (int i = tid; i < PB * kTC; i += kVertThreads) {
       const int j = i / kTC, c = i - j * kTC;
       if (j < np && c < ncol) v3d[(static_cast<int64_t>(pb0 + j) * V) * 3 + col0 + c] = sm.outs[j][c];
     }
     if (v2d != nullptr) {
-      for (int i = tid; i < kPB * kTV * 2; i += kVertThreads) {
+      for (int i = tid; i < PB * kTV * 2; i += kVertThreads) {
         const int j = i / (kTV * 2), c = i - j * (kTV * 2);
         if (j < np && c < nv * 2) v2d[(static_cast<int64_t>(pb0 + j) * V) * 2 + v0 * 2 + c] = sm.outs2[j][c];
       }
@@ -401,9 +413,10 @@ smplx_vertex_kernel(const __grid_constant__ CUtensorMap tmPDX, int KT, const flo
 }
 
 // ------------------------------------------------------------------------------------------------
-// Joints: 55 posed LBS joints + 21 vertex-picked joints + 51 barycentric face landmarks = 127
-// (smplx.SMPLX.forward), placed in camera space like the vertices; 2-D projection; transl_pelvis.
+// Joints: NJ posed LBS joints + 21 vertex-picked joints + NL barycentric face landmarks (smplx.SMPLX.forward:
+// 55 + 21 + 51 = 127; smplx.SMPL.forward: 24 + 21 + 0 = 45), placed like the vertices; 2-D projection; transl_pelvis.
 // ------------------------------------------------------------------------------------------------
+template <int NJ, int NL>
 __global__ void __launch_bounds__(128)
 smplx_joints_kernel(const float* __restrict__ jposed, const float* __restrict__ xf,
                     const float* __restrict__ transl, const float* __restrict__ K_det,
@@ -414,21 +427,23 @@ smplx_joints_kernel(const float* __restrict__ jposed, const float* __restrict__ 
   const int p = blockIdx.x;
   if (p >= *count) return;
   const int j = threadIdx.x;
-  if (j >= 127) return;
+  constexpr int kJ = NJ + 21 + NL;
+  static_assert(kJ <= 128, "one thread per joint");
+  if (j >= kJ) return;
   float o[3];
   const float* vp = v3d + static_cast<int64_t>(p) * V * 3;
-  if (j < kNJ) {
+  if (j < NJ) {
     const float* X = xf + static_cast<int64_t>(p) * 16;
-    const float* q = jposed + (static_cast<int64_t>(p) * kNJ + j) * 3;
+    const float* q = jposed + (static_cast<int64_t>(p) * NJ + j) * 3;
     const float dx = q[0] - X[9], dy = q[1] - X[10], dz = q[2] - X[11];
 #pragma unroll
     for (int r = 0; r < 3; ++r)
       o[r] = ((X[r * 3] * dx + X[r * 3 + 1] * dy + X[r * 3 + 2] * dz) - X[12 + r]) + transl[p * 3 + r];
-  } else if (j < kNJ + 21) {
-    const int v = extra_idx[j - kNJ];
+  } else if (j < NJ + 21) {
+    const int v = extra_idx[j - NJ];
     o[0] = vp[v * 3]; o[1] = vp[v * 3 + 1]; o[2] = vp[v * 3 + 2];
   } else {
-    const int l = j - kNJ - 21;
+    const int l = j - NJ - 21;
     o[0] = o[1] = o[2] = 0.f;
 #pragma unroll
     for (int f = 0; f < 3; ++f) {
@@ -439,27 +454,27 @@ smplx_joints_kernel(const float* __restrict__ jposed, const float* __restrict__ 
       o[2] = fmaf(b, vp[v * 3 + 2], o[2]);
     }
   }
-  float* jo = j3d + (static_cast<int64_t>(p) * 127 + j) * 3;
+  float* jo = j3d + (static_cast<int64_t>(p) * kJ + j) * 3;
   jo[0] = o[0]; jo[1] = o[1]; jo[2] = o[2];
   if (j == 0) {
     transl_pelvis[p * 3] = o[0]; transl_pelvis[p * 3 + 1] = o[1]; transl_pelvis[p * 3 + 2] = o[2];
   }
   const float* Kd = K_det + p * 9;
   const float u = o[0] / o[2], w = o[1] / o[2], one = o[2] / o[2];
-  j2d[(static_cast<int64_t>(p) * 127 + j) * 2] = Kd[0] * u + Kd[1] * w + Kd[2] * one;
-  j2d[(static_cast<int64_t>(p) * 127 + j) * 2 + 1] = Kd[3] * u + Kd[4] * w + Kd[5] * one;
+  j2d[(static_cast<int64_t>(p) * kJ + j) * 2] = Kd[0] * u + Kd[1] * w + Kd[2] * one;
+  j2d[(static_cast<int64_t>(p) * kJ + j) * 2 + 1] = Kd[3] * u + Kd[4] * w + Kd[5] * one;
 }
 
 // ------------------------------------------------------------------------------------------------
 // Load-time folding / repacking kernels
 // ------------------------------------------------------------------------------------------------
-// PDX[k, c]: k < 486 -> posedirs[k, c]; k >= 486 -> shapedirs_full[c, k - 486]  (shapedirs_full [3V, L])
-__global__ void build_pdx_kernel(const float* __restrict__ posedirs, const float* __restrict__ sdirs, int L,
+// PDX[k, c]: k < PF -> posedirs[k, c]; k >= PF -> shapedirs_full[c, k - PF]  (shapedirs_full [3V, L])
+__global__ void build_pdx_kernel(const float* __restrict__ posedirs, const float* __restrict__ sdirs, int PF, int L,
                                  int V3, int ldp, float* __restrict__ PDX) {
   const int k = blockIdx.y;
   for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < ldp; c += gridDim.x * blockDim.x) {
     float v = 0.f;
-    if (c < V3) v = (k < kPoseFeat) ? posedirs[static_cast<int64_t>(k) * V3 + c] : sdirs[static_cast<int64_t>(c) * L + (k - kPoseFeat)];
+    if (c < V3) v = (k < PF) ? posedirs[static_cast<int64_t>(k) * V3 + c] : sdirs[static_cast<int64_t>(c) * L + (k - PF)];
     PDX[static_cast<int64_t>(k) * ldp + c] = v;
   }
 }
@@ -481,24 +496,52 @@ __global__ void fold_jreg_kernel(const float* __restrict__ Jr, const float* __re
   }
 }
 
-}  // namespace
-
-// TMA descriptor of PDX [KT, ldp] fp32: boxes of 16 rows x 220 columns, no swizzle.
-int smplx_make_tmap(SmplxDeviceModel* bm) {
-  return make_tmap_2d(&bm->tmPDX, bm->PDX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, kPoseFeat + bm->L, bm->ldp,
-                      static_cast<uint64_t>(bm->ldp) * 4, kChunkRows, kPitch, false);
-}
-int smplx_tile_verts() { return kTV; }
-
-int smplx_build_pdx(const float* posedirs, const float* sdirs_full, int L, int V, int ldp, float* PDX,
-                    cudaStream_t st) {
-  build_pdx_kernel<<<dim3(32, kPoseFeat + L), 256, 0, st>>>(posedirs, sdirs_full, L, V * 3, ldp, PDX);
+// prep -> vertices -> joints for one body-model shape (NJ kinematic joints, PF pose features, NL landmarks)
+template <int NJ, int PF, int NL, int PB, bool kRaw>
+int body_forward_impl(const SmplxDeviceModel& bm, const float* rotvec, const float* shape, const float* expr,
+                      const float* transl, const float* K_det, const int* count, int max_persons, SmplxScratch& ws,
+                      float* v3d, float* v2d, float* j3d, float* j2d, float* transl_pelvis, cudaStream_t st) {
+  const int KT = PF + bm.L;
+  MHMR_REQUIRE(KT <= kKTMax, "smplx: too many blend-shape coefficients");
+  MHMR_REQUIRE(bm.num_joints == NJ && bm.pose_feat == PF && bm.n_lmk == NL, "body model / kernel shape mismatch");
+  body_prep_kernel<NJ, PF, kRaw><<<max_persons, 64, 0, st>>>(rotvec, shape, expr, bm.L - bm.num_betas, bm.Jt,
+                                                             bm.Jdirs, bm.parents, count, bm.num_betas, bm.center_idx,
+                                                             KT, ws.cf, ws.Amat, ws.xf, ws.jposed);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  static PerDeviceOnce once;
+  const int vsmem = static_cast<int>(sizeof(VertSmem<NJ, PB>)) + 128;
+  if (once.first()) {
+    MHMR_CUDA_CHECK(cudaFuncSetAttribute(smplx_vertex_kernel<NJ, PB>, cudaFuncAttributeMaxDynamicSharedMemorySize, vsmem));
+  }
+  const int tiles = (bm.V + kTV - 1) / kTV;
+  smplx_vertex_kernel<NJ, PB><<<tiles, kVertThreads, vsmem, st>>>(bm.tmPDX, KT, bm.vt, bm.lbs_weights_padded, ws.cf,
+                                                             ws.Amat, ws.xf, transl, K_det, count, bm.V, v3d, v2d);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  smplx_joints_kernel<NJ, NL><<<max_persons, 128, 0, st>>>(ws.jposed, ws.xf, transl, K_det, v3d, bm.extra_idx,
+                                                           bm.lmk_tri, bm.lmk_bary, count, bm.V, j3d, j2d,
+                                                           transl_pelvis);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }
 
-int smplx_fold_jreg(const float* Jr, const float* M, int V, int Q, float* out, cudaStream_t st) {
-  fold_jreg_kernel<<<dim3(kNJ, Q), 256, 0, st>>>(Jr, M, V, Q, out);
+}  // namespace
+
+// TMA descriptor of PDX [KT, ldp] fp32: boxes of 16 rows x 220 columns, no swizzle.
+int smplx_make_tmap(SmplxDeviceModel* bm) {
+  return make_tmap_2d(&bm->tmPDX, bm->PDX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, bm->pose_feat + bm->L, bm->ldp,
+                      static_cast<uint64_t>(bm->ldp) * 4, kChunkRows, kPitch, false);
+}
+int smplx_tile_verts() { return kTV; }
+
+int smplx_build_pdx(const float* posedirs, const float* sdirs_full, int PF, int L, int V, int ldp, float* PDX,
+                    cudaStream_t st) {
+  build_pdx_kernel<<<dim3(32, PF + L), 256, 0, st>>>(posedirs, sdirs_full, PF, L, V * 3, ldp, PDX);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
+}
+
+int smplx_fold_jreg(const float* Jr, const float* M, int NJ, int V, int Q, float* out, cudaStream_t st) {
+  fold_jreg_kernel<<<dim3(NJ, Q), 256, 0, st>>>(Jr, M, V, Q, out);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }
@@ -507,26 +550,21 @@ int smplx_forward(const SmplxDeviceModel& bm, const float* rotvec, const float* 
                   const float* transl, const float* K_det, const int* count, int max_persons,
                   SmplxScratch& ws, float* v3d, float* v2d, float* j3d, float* j2d, float* transl_pelvis,
                   cudaStream_t st) {
-  const int KT = kPoseFeat + bm.L;
-  MHMR_REQUIRE(KT <= kKTMax, "smplx: too many blend-shape coefficients");
-  smplx_prep_kernel<<<max_persons, 64, 0, st>>>(rotvec, shape, expr, transl, bm.Jt, bm.Jdirs, bm.parents,
-                                                count, bm.num_betas, bm.center_idx, KT, ws.cf, ws.Amat,
-                                                ws.xf, ws.jposed);
-  MHMR_CUDA_CHECK(cudaGetLastError());
-  static PerDeviceOnce once;
-  const int vsmem = static_cast<int>(sizeof(VertSmem)) + 128;
-  if (once.first()) {
-    MHMR_CUDA_CHECK(cudaFuncSetAttribute(smplx_vertex_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, vsmem));
-  }
-  const int tiles = (bm.V + kTV - 1) / kTV;
-  smplx_vertex_kernel<<<tiles, kVertThreads, vsmem, st>>>(bm.tmPDX, KT, bm.vt, bm.lbs_weights_padded, ws.cf, ws.Amat,
-                                                         ws.xf, transl, K_det, count, bm.V, v3d, v2d);
-  MHMR_CUDA_CHECK(cudaGetLastError());
-  smplx_joints_kernel<<<max_persons, 128, 0, st>>>(ws.jposed, ws.xf, transl, K_det, v3d, bm.extra_idx,
-                                                   bm.lmk_tri, bm.lmk_bary, count, bm.V, j3d, j2d,
-                                                   transl_pelvis);
-  MHMR_CUDA_CHECK(cudaGetLastError());
-  return MHMR_OK;
+  return body_forward_impl<kNJ, kPoseFeat, 51, 16, false>(bm, rotvec, shape, expr, transl, K_det, count, max_persons, ws,
+                                                      v3d, v2d, j3d, j2d, transl_pelvis, st);
+}
+
+int body_forward_raw(const SmplxDeviceModel& bm, const float* full_pose, const float* betas, const float* expr,
+                     const float* transl, const float* K, const int* count, int max_persons, SmplxScratch& ws,
+                     float* v3d, float* v2d, float* j3d, float* j2d, float* transl_pelvis, cudaStream_t st) {
+  if (bm.num_joints == 24)
+    return body_forward_impl<24, 207, 0, 8, true>(bm, full_pose, betas, expr, transl, K, count, max_persons, ws, v3d,
+                                               v2d, j3d, j2d, transl_pelvis, st);
+  if (bm.num_joints == kNJ)
+    return body_forward_impl<kNJ, kPoseFeat, 51, 16, true>(bm, full_pose, betas, expr, transl, K, count, max_persons, ws,
+                                                       v3d, v2d, j3d, j2d, transl_pelvis, st);
+  set_last_error("body model: only SMPL (24 joints) and SMPL-X (55 joints) are instantiated");
+  return MHMR_ERR_UNSUPPORTED;
 }
 
 }  // namespace mhmr

@@ -7,6 +7,8 @@ published checkpoints, `SMPLX_NEUTRAL.npz` or `smpl_mean_params.npz`):
   make_body_model  : SMPL-X-shaped body model (V=10475, 55 joints, 486 pose-corrective features,
                      51 static landmarks, 21 vertex-picked joints) as consumed by smplx.create at
                      blocks/smpl_layer.py:38
+  make_smpl_body_model, make_smplx2smpl, make_j_regressor_h36m : the evaluation assets of train.py:41-45, :400
+                     (SMPL-shaped body model, SMPL-X -> SMPL transfer matrix, H36M joint regressor)
 
 Everything is generated on the CPU from torch.Generator seeds so the GPU box, the build container and
 the golden-fixture script see bit-identical inputs.
@@ -213,6 +215,67 @@ def make_body_model(seed: int = 0, num_verts: int = NUM_VERTS, num_faces: int = 
     bm["lmk_bary_coords"] = bary / bary.sum(dim=1, keepdim=True)
     bm["extra_joints_idxs"] = torch.randint(0, V, (21,), generator=g)
     return bm
+
+
+SMPL_NUM_VERTS = 6890
+SMPL_NUM_FACES = 13776
+SMPL_NUM_JOINTS = 24
+SMPL_PARENTS = [-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21]
+
+
+def make_smpl_body_model(seed: int = 0, gender: str = "male") -> dict:
+    """SMPL-shaped body model (V = 6890, the standard 24-joint parent table, 207 pose-corrective features, 10 betas,
+    21 vertex-picked joints at the smplx.vertex_ids['smplh'] ids) in the dict layout of `api.body_model_from_smpl_pkl`.
+    Male and female differ through the seed."""
+    from .api import SMPL_EXTRA_JOINTS_IDXS
+
+    g = _gen(seed + 606 + (0 if gender == "male" else 17))
+    V, NJ = SMPL_NUM_VERTS, SMPL_NUM_JOINTS
+    bm = {"v_template": _randn(g, V, 3) * torch.tensor([0.25, 0.45, 0.12]),
+          "shapedirs": _randn(g, V, 3, 10, std=0.01),
+          "posedirs": _randn(g, (NJ - 1) * 9, V * 3, std=1e-3)}
+    Jr = torch.zeros(NJ, V)
+    for j in range(NJ):
+        ids = torch.randint(0, V, (32,), generator=g)
+        w = torch.rand(32, generator=g)
+        Jr[j].index_add_(0, ids, w / w.sum())
+    bm["J_regressor"] = Jr
+    W = torch.zeros(V, NJ)
+    ids = torch.randint(0, NJ, (V, 4), generator=g)
+    w = torch.rand(V, 4, generator=g) + 0.05
+    W.scatter_add_(1, ids, w / w.sum(dim=1, keepdim=True))
+    bm["lbs_weights"] = W
+    bm["parents"] = torch.tensor(SMPL_PARENTS, dtype=torch.int64)
+    bm["faces"] = torch.randint(0, V, (SMPL_NUM_FACES, 3), generator=g)
+    bm["extra_joints_idxs"] = torch.tensor(SMPL_EXTRA_JOINTS_IDXS, dtype=torch.int64)
+    bm["num_verts"] = V
+    return bm
+
+
+def make_smplx2smpl(seed: int = 0) -> torch.Tensor:
+    """SMPL-X -> SMPL transfer matrix [6890, 10475] with barycentric rows (3 distinct SMPL-X vertices, positive weights
+    summing to 1), as a torch sparse COO tensor (the dense fp32 matrix is 290 MB)."""
+    g = _gen(seed + 707)
+    R = SMPL_NUM_VERTS
+    pick = torch.randint(0, NUM_VERTS, (R, 3), generator=g)
+    pick[:, 1] = (pick[:, 0] + 1 + torch.randint(0, 50, (R,), generator=g)) % NUM_VERTS
+    pick[:, 2] = (pick[:, 1] + 1 + torch.randint(0, 50, (R,), generator=g)) % NUM_VERTS
+    w = torch.rand(R, 3, generator=g) + 0.05
+    w = w / w.sum(dim=1, keepdim=True)
+    rows = torch.arange(R).repeat_interleave(3)
+    return torch.sparse_coo_tensor(torch.stack([rows, pick.reshape(-1)]), w.reshape(-1),
+                                   (R, NUM_VERTS), check_invariants=True).coalesce()
+
+
+def make_j_regressor_h36m(seed: int = 0) -> torch.Tensor:
+    """H36M joint regressor [17, 6890]: non-negative rows summing to 1 over 48 random SMPL vertices each."""
+    g = _gen(seed + 808)
+    Jr = torch.zeros(17, SMPL_NUM_VERTS)
+    for j in range(17):
+        ids = torch.randint(0, SMPL_NUM_VERTS, (48,), generator=g)
+        w = torch.rand(48, generator=g)
+        Jr[j].index_add_(0, ids, w / w.sum())
+    return Jr
 
 
 def make_images(batch: int, img_size: int, seed: int = 0) -> torch.Tensor:
