@@ -25,8 +25,8 @@ struct DevBuf {
   size_t bytes = 0;
 };
 
-struct ArchSpec { int D, depth, heads; };
-const ArchSpec kArch[3] = {{384, 12, 6}, {768, 12, 12}, {1024, 24, 16}};
+struct ArchSpec { int D, depth; };
+const ArchSpec kArch[3] = {{384, 12}, {768, 12}, {1024, 24}};
 constexpr int kHphDim = 1024;
 constexpr int kCamDim = 99;
 
@@ -44,13 +44,26 @@ struct HphLayer {
   const float *ln1_g, *ln1_b, *Wq, *Wca_out, *bca_out;
   const float *ln2_g, *ln2_b, *Wff0, *bff0, *Wff3, *bff3;
 };
+// fp32 weights the SMPL-X head reads as they are: camera.freq_bands, x_attention_head.cross_{queries,values}_{x,y},
+// mlp_offset
+struct SmplxHeadWeights {
+  const float *freq_bands, *cq_x, *cq_y, *cv_x, *cv_y;
+  const float *off0_w, *off0_b, *off2_w, *off2_b;
+};
+// the Anny head's: mlp_fov_unique and fov_max, dec_pos_emb, dec_to_token, the output Linears of the four regressors,
+// useful_rotmat
+struct AnnyHeadWeights {
+  const float *fov0_w, *fov0_b, *fov2_w, *fov2_b, *fov_max, *dec_pos_emb, *dt_w, *dt_b;
+  const float *off2_w, *off2_b, *dist2_w, *dist2_b, *shape2_w, *shape2_b, *pose2_w, *useful_rotmat;
+};
 
 }  // namespace
 
 struct mhmr_engine {
   mhmr_config cfg{};
   std::string enc = "backbone.encoder.";   // state-dict prefix of the DINOv2 backbone
-  int D = 0, depth = 0, heads = 0, res = 0, N = 0, T = 0, C = 0, Cp = 0, Cq = 0, nkv = 0, ndec = 0;
+  int D = 0, depth = 0, res = 0, N = 0, T = 0, C = 0, Cp = 0, Cq = 0, nkv = 0, ndec = 0;
+  int dec_dim = 0, dec_mlp = 0;            // HPH decoder width and feed-forward width
   bool finalized = false;
   std::map<std::string, DevBuf> weights;   // raw fp32 device copies, keyed like the state_dict
   std::map<std::string, DevBuf> tables;    // int32 tables
@@ -75,7 +88,11 @@ struct mhmr_engine {
   float* rowadd = nullptr;    // [N, D]  pos_embed[1:] + patch bias
   float* cls_pos = nullptr;   // [D]
   std::vector<VitLayer> vit;
+  const float *norm_g = nullptr, *norm_b = nullptr;   // final LayerNorm of the backbone
   __half* Wcls0 = nullptr;    // [D, D]
+  const float *cls2_w = nullptr, *cls2_b = nullptr;   // detection output row [D] and bias [1]
+  SmplxHeadWeights smplx_w{};
+  AnnyHeadWeights anny_w{};
   __half* Wkv16 = nullptr;    // [nkv, Cp]
   float* Wkv32 = nullptr;     // [nkv, Cq]
   float* Wte_q = nullptr;     // [1024, Cq]
@@ -92,7 +109,7 @@ struct mhmr_engine {
   __half* Xlo = nullptr;       // lo plane of the two-term fp16 residual stream (hi plane = Xn16), gemm_tc.cuh
   int ln_slots = 0;
   float *X = nullptr, *z32 = nullptr, *scores_raw = nullptr, *KV32 = nullptr, *Kinv = nullptr;
-  int *det = nullptr, *count = nullptr, *img_off = nullptr;
+  int *count = nullptr, *img_off = nullptr;
   // central-stream refinement: token rows, input patches, residual streams and MLP hidden of the detected persons
   int* r_rowidx = nullptr;
   float *r_patch = nullptr, *r_x = nullptr, *r_h = nullptr, *r_term = nullptr;
@@ -100,8 +117,7 @@ struct mhmr_engine {
   unsigned int* r_barrier = nullptr;
   const float* Wpatch32 = nullptr;
   float *zc = nullptr, *query = nullptr, *vals = nullptr, *dKV = nullptr, *offh = nullptr, *xa = nullptr,
-        *qkvp = nullptr, *att = nullptr, *qca = nullptr, *ffh = nullptr, *dec = nullptr, *K_det = nullptr,
-        *one_count_x = nullptr;
+        *qkvp = nullptr, *att = nullptr, *qca = nullptr, *ffh = nullptr, *dec = nullptr, *K_det = nullptr;
   int* one = nullptr;  // device int == 1 (count for load-time skinny launches)
   SmplxScratch sx;
   GemmPlan patch_plan, cls0_plan, kv_plan;
@@ -161,9 +177,11 @@ struct mhmr_engine {
 
 namespace {
 
+#define GETW(dst, key, numel)                           \
+  if (((dst) = e->w(key, numel)) == nullptr) return MHMR_ERR_STATE;
 #define NEEDW(var, key, numel)                          \
-  const float* var = e->w(key, numel);                  \
-  if (var == nullptr) return MHMR_ERR_STATE;
+  const float* var;                                     \
+  GETW(var, key, numel)
 
 // CTA-pair 256x256 tiles (cta_group::2) whenever N is a multiple of 256, else single-CTA 128x128 tiles
 int pick_bn(int N) { return (N % 256 == 0) ? 512 : 128; }
@@ -265,7 +283,8 @@ int finalize_vit(mhmr_engine* e, cudaStream_t st) {
     TRY(gemm_plan_init(&L.fc1, e->Xn16, D, L.Wfc1, D, static_cast<int>(M), 4 * D, D, epi_fc1, f1, pick_bn(4 * D)));
     TRY(gemm_plan_init(&L.fc2, e->H16, 4 * D, L.Wfc2, 4 * D, static_cast<int>(M), D, 4 * D, epi_fc2, f2, pick_bn(D)));
   }
-  if (e->w(enc + "norm.weight", D) == nullptr || e->w(enc + "norm.bias", D) == nullptr) return MHMR_ERR_STATE;
+  GETW(e->norm_g, enc + "norm.weight", D)
+  GETW(e->norm_b, enc + "norm.bias", D)
   return MHMR_OK;
 }
 
@@ -290,40 +309,76 @@ int alloc_refine(mhmr_engine* e, int rows, cudaStream_t st) {
   return MHMR_OK;
 }
 
-int finalize_head(mhmr_engine* e, cudaStream_t st) {
-  const int D = e->D, N = e->N, Bm = e->cfg.max_batch, Pm = e->cfg.max_persons, C = e->C, Cp = e->Cp,
-            Cq = e->Cq, nb = e->cfg.num_betas, depth = e->cfg.xat_depth, inner = e->cfg.xat_num_heads * 32;
-  const int res = e->res;
-  const size_t BN = static_cast<size_t>(Bm) * N;
+// detection and decoder workspaces of both heads; the per-person ones are sized by the decoder and MLP widths
+int alloc_head_workspaces(mhmr_engine* e, cudaStream_t st) {
+  const int D = e->D, Bm = e->cfg.max_batch, Pm = e->cfg.max_persons, inner = e->cfg.xat_num_heads * 32;
+  const size_t BN = static_cast<size_t>(Bm) * e->N;
   TRY(e->alloc(&e->z32, BN * D));
-  TRY(e->alloc(&e->ctx16, BN * Cp));
+  TRY(e->alloc(&e->ctx16, BN * e->Cp));
   TRY(e->alloc(&e->scores_raw, BN));
   TRY(e->alloc(&e->KV32, BN * e->nkv));
   TRY(e->alloc(&e->Kinv, static_cast<size_t>(Bm) * 9));
-  TRY(e->alloc(&e->det, static_cast<size_t>(3) * Pm));
   TRY(e->alloc(&e->count, 4));
   TRY(e->alloc(&e->img_off, static_cast<size_t>(Bm) + 1));
   TRY(e->alloc(&e->one, 4));
   const int one_h = 1;
   MHMR_CUDA_CHECK(cudaMemcpyAsync(e->one, &one_h, sizeof(int), cudaMemcpyHostToDevice, st));
   MHMR_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&e->h_count), sizeof(int)));
+  TRY(e->alloc(&e->zc, static_cast<size_t>(Pm) * D));
+  TRY(e->alloc(&e->xa, static_cast<size_t>(Pm) * e->dec_dim));
+  TRY(e->alloc(&e->qkvp, static_cast<size_t>(Pm) * 3 * inner));
+  TRY(e->alloc(&e->att, static_cast<size_t>(Pm) * inner));
+  TRY(e->alloc(&e->qca, static_cast<size_t>(Pm) * inner));
+  TRY(e->alloc(&e->ffh, static_cast<size_t>(Pm) * e->dec_mlp));
+  return MHMR_OK;
+}
 
-  // detection
-  NEEDW(c0w, "mlp_classif.0.weight", static_cast<int64_t>(D) * D) NEEDW(c0b, "mlp_classif.0.bias", D)
-  NEEDW(c2w, "mlp_classif.2.weight", D) NEEDW(c2b, "mlp_classif.2.bias", 1)
-  (void)c2w; (void)c2b;
+// detection MLP under `p`: its hidden Linear runs as a GEMM on the fp16 context, its output row in rowdot_sigmoid
+int load_detector(mhmr_engine* e, const std::string& p, cudaStream_t st) {
+  const int D = e->D, BN = e->cfg.max_batch * e->N;
+  NEEDW(c0w, p + "0.weight", static_cast<int64_t>(D) * D) NEEDW(c0b, p + "0.bias", D)
+  GETW(e->cls2_w, p + "2.weight", D) GETW(e->cls2_b, p + "2.bias", 1)
   TRY(to_f16(e, c0w, D, D, D, D, &e->Wcls0, st));
   GemmEpi ce; ce.bias = c0b; ce.out = e->H16; ce.ldo = D;
-  TRY(gemm_plan_init(&e->cls0_plan, e->ctx16, Cp, e->Wcls0, D, static_cast<int>(BN), D, D, EPI_BIAS_RELU_F16, ce, pick_bn(D)));
-  NEEDW(o0w, "mlp_offset.0.weight", static_cast<int64_t>(D) * D) NEEDW(o0b, "mlp_offset.0.bias", D)
-  NEEDW(o2w, "mlp_offset.2.weight", 2ll * D) NEEDW(o2b, "mlp_offset.2.bias", 2)
-  (void)o0w; (void)o0b; (void)o2w; (void)o2b;
+  return gemm_plan_init(&e->cls0_plan, e->ctx16, e->Cp, e->Wcls0, D, BN, D, D, EPI_BIAS_RELU_F16, ce, pick_bn(D));
+}
+
+// HPH layer under `p` (PreNorm self-attention, cross-attention, feed-forward).  The cross-attention's to_kv weight
+// [2 inner, kv_cols] goes to *to_kv: each head packs the keys / values of all layers into one GEMM its own way.
+int load_hph_layer(mhmr_engine* e, const std::string& p, int kv_cols, HphLayer& L, const float** to_kv) {
+  const int dim = e->dec_dim, mlp = e->dec_mlp, inner = e->cfg.xat_num_heads * 32;
+  GETW(L.ln0_g, p + "0.norm.weight", dim) GETW(L.ln0_b, p + "0.norm.bias", dim)
+  GETW(L.Wqkv, p + "0.fn.to_qkv.weight", 3ll * inner * dim)
+  GETW(L.Wsa_out, p + "0.fn.to_out.0.weight", static_cast<int64_t>(dim) * inner)
+  GETW(L.bsa_out, p + "0.fn.to_out.0.bias", dim)
+  GETW(L.ln1_g, p + "1.norm.weight", dim) GETW(L.ln1_b, p + "1.norm.bias", dim)
+  GETW(*to_kv, p + "1.fn.to_kv.weight", 2ll * inner * kv_cols)
+  GETW(L.Wq, p + "1.fn.to_q.weight", static_cast<int64_t>(inner) * dim)
+  GETW(L.Wca_out, p + "1.fn.to_out.0.weight", static_cast<int64_t>(dim) * inner)
+  GETW(L.bca_out, p + "1.fn.to_out.0.bias", dim)
+  GETW(L.ln2_g, p + "2.norm.weight", dim) GETW(L.ln2_b, p + "2.norm.bias", dim)
+  GETW(L.Wff0, p + "2.fn.net.0.weight", static_cast<int64_t>(mlp) * dim) GETW(L.bff0, p + "2.fn.net.0.bias", mlp)
+  GETW(L.Wff3, p + "2.fn.net.3.weight", static_cast<int64_t>(dim) * mlp) GETW(L.bff3, p + "2.fn.net.3.bias", dim)
+  return MHMR_OK;
+}
+
+int finalize_head(mhmr_engine* e, cudaStream_t st) {
+  const int D = e->D, N = e->N, Bm = e->cfg.max_batch, Pm = e->cfg.max_persons, C = e->C, Cp = e->Cp,
+            Cq = e->Cq, nb = e->cfg.num_betas, depth = e->cfg.xat_depth, inner = e->cfg.xat_num_heads * 32;
+  const int res = e->res;
+  const size_t BN = static_cast<size_t>(Bm) * N;
+  TRY(alloc_head_workspaces(e, st));
+  TRY(load_detector(e, "mlp_classif.", st));
+  SmplxHeadWeights& hw = e->smplx_w;
+  GETW(hw.off0_w, "mlp_offset.0.weight", static_cast<int64_t>(D) * D) GETW(hw.off0_b, "mlp_offset.0.bias", D)
+  GETW(hw.off2_w, "mlp_offset.2.weight", 2ll * D) GETW(hw.off2_b, "mlp_offset.2.bias", 2)
 
   // HPH
   const std::string h = "x_attention_head.";
-  for (const char* nm : {"cross_queries_x", "cross_queries_y", "cross_values_x", "cross_values_y"})
-    if (e->w(h + nm, static_cast<int64_t>(res) * C) == nullptr) return MHMR_ERR_STATE;
-  if (e->w("camera.freq_bands", 16) == nullptr) return MHMR_ERR_STATE;
+  const int64_t rC = static_cast<int64_t>(res) * C;
+  GETW(hw.cq_x, h + "cross_queries_x", rC) GETW(hw.cq_y, h + "cross_queries_y", rC)
+  GETW(hw.cv_x, h + "cross_values_x", rC) GETW(hw.cv_y, h + "cross_values_y", rC)
+  GETW(hw.freq_bands, "camera.freq_bands", 16)
   const int token_dim = 318 + nb + 3 + C;
   const std::string t = h + "transformer.";
   NEEDW(tew, t + "to_token_embedding.weight", static_cast<int64_t>(kHphDim) * token_dim)
@@ -350,21 +405,8 @@ int finalize_head(mhmr_engine* e, cudaStream_t st) {
   e->hph.resize(depth);
   TRY(e->alloc(&e->Wkv32, static_cast<size_t>(e->nkv) * Cq));
   for (int l = 0; l < depth; ++l) {
-    HphLayer& L = e->hph[l];
-    const std::string p = t + "transformer.layers." + std::to_string(l) + ".";
-    NEEDW(a, p + "0.norm.weight", kHphDim) NEEDW(b, p + "0.norm.bias", kHphDim)
-    NEEDW(c, p + "0.fn.to_qkv.weight", 3ll * inner * kHphDim)
-    NEEDW(d, p + "0.fn.to_out.0.weight", static_cast<int64_t>(kHphDim) * inner) NEEDW(f, p + "0.fn.to_out.0.bias", kHphDim)
-    NEEDW(g, p + "1.norm.weight", kHphDim) NEEDW(hh, p + "1.norm.bias", kHphDim)
-    NEEDW(kvw, p + "1.fn.to_kv.weight", 2ll * inner * C)
-    NEEDW(qw, p + "1.fn.to_q.weight", static_cast<int64_t>(inner) * kHphDim)
-    NEEDW(co, p + "1.fn.to_out.0.weight", static_cast<int64_t>(kHphDim) * inner) NEEDW(cb, p + "1.fn.to_out.0.bias", kHphDim)
-    NEEDW(n2g, p + "2.norm.weight", kHphDim) NEEDW(n2b, p + "2.norm.bias", kHphDim)
-    NEEDW(f0, p + "2.fn.net.0.weight", static_cast<int64_t>(kHphDim) * kHphDim) NEEDW(f0b, p + "2.fn.net.0.bias", kHphDim)
-    NEEDW(f3, p + "2.fn.net.3.weight", static_cast<int64_t>(kHphDim) * kHphDim) NEEDW(f3b, p + "2.fn.net.3.bias", kHphDim)
-    L.ln0_g = a; L.ln0_b = b; L.Wqkv = c; L.Wsa_out = d; L.bsa_out = f;
-    L.ln1_g = g; L.ln1_b = hh; L.Wq = qw; L.Wca_out = co; L.bca_out = cb;
-    L.ln2_g = n2g; L.ln2_b = n2b; L.Wff0 = f0; L.bff0 = f0b; L.Wff3 = f3; L.bff3 = f3b;
+    const float* kvw = nullptr;
+    TRY(load_hph_layer(e, t + "transformer.layers." + std::to_string(l) + ".", C, e->hph[l], &kvw));
     TRY(repack_f32(kvw, C, 0, e->Wkv32 + static_cast<size_t>(l) * 2 * inner * Cq, Cq, 0, 2 * inner, C, true, st));
   }
   TRY(e->alloc(&e->Wkv16, static_cast<size_t>(e->nkv) * Cp));
@@ -391,16 +433,10 @@ int finalize_head(mhmr_engine* e, cudaStream_t st) {
   MHMR_CUDA_CHECK(cudaMemcpyAsync(e->bdec + 321 + nb, deb, 10 * 4, cudaMemcpyDeviceToDevice, st));  // init_expression = 0
 
   // per-person buffers
-  TRY(e->alloc(&e->zc, static_cast<size_t>(Pm) * D));
   TRY(e->alloc(&e->query, static_cast<size_t>(Pm) * Cq));
   TRY(e->alloc(&e->vals, static_cast<size_t>(Pm) * Cq));
   TRY(e->alloc(&e->dKV, static_cast<size_t>(Pm) * e->nkv));
   TRY(e->alloc(&e->offh, static_cast<size_t>(Pm) * D));
-  TRY(e->alloc(&e->xa, static_cast<size_t>(Pm) * kHphDim));
-  TRY(e->alloc(&e->qkvp, static_cast<size_t>(Pm) * 3 * inner));
-  TRY(e->alloc(&e->att, static_cast<size_t>(Pm) * inner));
-  TRY(e->alloc(&e->qca, static_cast<size_t>(Pm) * inner));
-  TRY(e->alloc(&e->ffh, static_cast<size_t>(Pm) * kHphDim));
   TRY(e->alloc(&e->dec, static_cast<size_t>(Pm) * e->ndec));
   TRY(e->alloc(&e->K_det, static_cast<size_t>(Pm) * 9));
   if (e->cfg.refine_central) TRY(alloc_refine(e, Pm, st));
@@ -454,45 +490,31 @@ int finalize_body(mhmr_engine* e, cudaStream_t st) {
 // Anny head (multi_hmr_anny/multi_hmr.py:41-95, encoder.py:16-31, hph.py): weights under the checkpoint's own keys.
 int finalize_anny(mhmr_engine* e, cudaStream_t st) {
   const int D = e->D, N = e->N, Bm = e->cfg.max_batch, Pm = e->cfg.max_persons, nb = e->cfg.num_betas;
-  const int dim = e->cfg.xat_dim, mlp = e->cfg.xat_mlp_dim, J = e->cfg.num_joints, depth = e->cfg.xat_depth;
+  const int dim = e->dec_dim, J = e->cfg.num_joints, depth = e->cfg.xat_depth;
   const int inner = e->cfg.xat_num_heads * 32, J6 = 6 * J, J6p = (J6 + 3) & ~3;
   const size_t BN = static_cast<size_t>(Bm) * N;
-  TRY(e->alloc(&e->z32, BN * D));
-  TRY(e->alloc(&e->ctx16, BN * e->Cp));
-  TRY(e->alloc(&e->scores_raw, BN));
-  TRY(e->alloc(&e->KV32, BN * e->nkv));
-  TRY(e->alloc(&e->Kinv, static_cast<size_t>(Bm) * 9));
+  TRY(alloc_head_workspaces(e, st));
   TRY(e->alloc(&e->K_use, static_cast<size_t>(Bm) * 9));
-  TRY(e->alloc(&e->count, 4));
-  TRY(e->alloc(&e->img_off, static_cast<size_t>(Bm) + 1));
   TRY(e->alloc(&e->det_score, Pm));
   TRY(e->alloc(&e->anny_ints, 2));
-  TRY(e->alloc(&e->one, 4));
-  const int one_h = 1;
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->one, &one_h, sizeof(int), cudaMemcpyHostToDevice, st));
-  MHMR_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&e->h_count), sizeof(int)));
 
   // detection: mlp_det hidden layer as a GEMM on the normed fp16 features (encoder.py:26,59)
-  NEEDW(c0w, "encoder.mlp_det.0.weight", static_cast<int64_t>(D) * D) NEEDW(c0b, "encoder.mlp_det.0.bias", D)
-  NEEDW(c2w, "encoder.mlp_det.2.weight", D) NEEDW(c2b, "encoder.mlp_det.2.bias", 1)
-  (void)c2w; (void)c2b;
-  TRY(to_f16(e, c0w, D, D, D, D, &e->Wcls0, st));
-  GemmEpi ce; ce.bias = c0b; ce.out = e->H16; ce.ldo = D;
-  TRY(gemm_plan_init(&e->cls0_plan, e->ctx16, e->Cp, e->Wcls0, D, static_cast<int>(BN), D, D, EPI_BIAS_RELU_F16, ce, pick_bn(D)));
+  TRY(load_detector(e, "encoder.mlp_det.", st));
   // field of view from the cls token (encoder.py:29-31,50)
-  NEEDW(f0w, "encoder.mlp_fov_unique.0.weight", static_cast<int64_t>(D) * D) NEEDW(f0b, "encoder.mlp_fov_unique.0.bias", D)
-  NEEDW(f2w, "encoder.mlp_fov_unique.2.weight", D) NEEDW(f2b, "encoder.mlp_fov_unique.2.bias", 1)
-  NEEDW(fmax, "encoder.fov_max", 1)
-  (void)f0w; (void)f0b; (void)f2w; (void)f2b; (void)fmax;
+  AnnyHeadWeights& hw = e->anny_w;
+  GETW(hw.fov0_w, "encoder.mlp_fov_unique.0.weight", static_cast<int64_t>(D) * D)
+  GETW(hw.fov0_b, "encoder.mlp_fov_unique.0.bias", D)
+  GETW(hw.fov2_w, "encoder.mlp_fov_unique.2.weight", D) GETW(hw.fov2_b, "encoder.mlp_fov_unique.2.bias", 1)
+  GETW(hw.fov_max, "encoder.fov_max", 1)
   TRY(e->alloc(&e->cls_x, static_cast<size_t>(Bm) * D));
   TRY(e->alloc(&e->cls_h, static_cast<size_t>(Bm) * D));
 
   // decoder tokens of every cell: dec_to_token(feat) + dec_pos_emb (multi_hmr.py:127-128), fp16 GEMM output
-  NEEDW(dtw, "dec_to_token.weight", static_cast<int64_t>(dim) * D) NEEDW(dtb, "dec_to_token.bias", dim)
-  NEEDW(pos, "dec_pos_emb", static_cast<int64_t>(N) * dim)
-  TRY(to_f16(e, dtw, D, dim, D, D, &e->Wdt16, st));
+  GETW(hw.dt_w, "dec_to_token.weight", static_cast<int64_t>(dim) * D) GETW(hw.dt_b, "dec_to_token.bias", dim)
+  GETW(hw.dec_pos_emb, "dec_pos_emb", static_cast<int64_t>(N) * dim)
+  TRY(to_f16(e, hw.dt_w, D, dim, D, D, &e->Wdt16, st));
   TRY(e->alloc(&e->dt_rowadd, static_cast<size_t>(N) * dim));
-  TRY(add_vec(pos, dtb, e->dt_rowadd, static_cast<int64_t>(N) * dim, dim, st));
+  TRY(add_vec(hw.dec_pos_emb, hw.dt_b, e->dt_rowadd, static_cast<int64_t>(N) * dim, dim, st));
   TRY(e->alloc(&e->dec16, BN * dim));
   GemmEpi te; te.rowadd = e->dt_rowadd; te.rows_in = N; te.out = e->dec16; te.ldo = dim;
   TRY(gemm_plan_init(&e->dt_plan, e->ctx16, e->Cp, e->Wdt16, D, static_cast<int>(BN), dim, D, EPI_ROWADD_F16, te, pick_bn(dim)));
@@ -501,21 +523,8 @@ int finalize_anny(mhmr_engine* e, cudaStream_t st) {
   e->hph.resize(depth);
   TRY(e->alloc(&e->Wkv16, static_cast<size_t>(e->nkv) * dim));
   for (int l = 0; l < depth; ++l) {
-    HphLayer& L = e->hph[l];
-    const std::string p = "decoder.transformer.layers." + std::to_string(l) + ".";
-    NEEDW(a, p + "0.norm.weight", dim) NEEDW(b, p + "0.norm.bias", dim)
-    NEEDW(c, p + "0.fn.to_qkv.weight", 3ll * inner * dim)
-    NEEDW(d, p + "0.fn.to_out.0.weight", static_cast<int64_t>(dim) * inner) NEEDW(f, p + "0.fn.to_out.0.bias", dim)
-    NEEDW(g, p + "1.norm.weight", dim) NEEDW(hh, p + "1.norm.bias", dim)
-    NEEDW(kvw, p + "1.fn.to_kv.weight", 2ll * inner * dim)
-    NEEDW(qw, p + "1.fn.to_q.weight", static_cast<int64_t>(inner) * dim)
-    NEEDW(co, p + "1.fn.to_out.0.weight", static_cast<int64_t>(dim) * inner) NEEDW(cb, p + "1.fn.to_out.0.bias", dim)
-    NEEDW(n2g, p + "2.norm.weight", dim) NEEDW(n2b, p + "2.norm.bias", dim)
-    NEEDW(f0, p + "2.fn.net.0.weight", static_cast<int64_t>(mlp) * dim) NEEDW(f0bb, p + "2.fn.net.0.bias", mlp)
-    NEEDW(f3, p + "2.fn.net.3.weight", static_cast<int64_t>(dim) * mlp) NEEDW(f3b, p + "2.fn.net.3.bias", dim)
-    L.ln0_g = a; L.ln0_b = b; L.Wqkv = c; L.Wsa_out = d; L.bsa_out = f;
-    L.ln1_g = g; L.ln1_b = hh; L.Wq = qw; L.Wca_out = co; L.bca_out = cb;
-    L.ln2_g = n2g; L.ln2_b = n2b; L.Wff0 = f0; L.bff0 = f0bb; L.Wff3 = f3; L.bff3 = f3b;
+    const float* kvw = nullptr;
+    TRY(load_hph_layer(e, "decoder.transformer.layers." + std::to_string(l) + ".", dim, e->hph[l], &kvw));
     TRY(f32_to_f16_2d(kvw, dim, e->Wkv16 + static_cast<size_t>(l) * 2 * inner * dim, dim, 2 * inner, dim, st));
   }
   GemmEpi ke; ke.out = e->KV32; ke.ldo = e->nkv;
@@ -524,15 +533,14 @@ int finalize_anny(mhmr_engine* e, cudaStream_t st) {
   // regressors (multi_hmr.py:59-66): the four first Linears stacked; mlp_pose's init_body_pose columns folded into
   // its bias, and init_body_pose added to the bias of its second Linear (:157)
   NEEDW(o0w, "mlp_offset.0.weight", static_cast<int64_t>(dim) * dim) NEEDW(o0b, "mlp_offset.0.bias", dim)
-  NEEDW(o2w, "mlp_offset.2.weight", 2ll * dim) NEEDW(o2b, "mlp_offset.2.bias", 2)
+  GETW(hw.off2_w, "mlp_offset.2.weight", 2ll * dim) GETW(hw.off2_b, "mlp_offset.2.bias", 2)
   NEEDW(d0w, "mlp_dist.0.weight", static_cast<int64_t>(dim) * dim) NEEDW(d0b, "mlp_dist.0.bias", dim)
-  NEEDW(d2w, "mlp_dist.2.weight", dim) NEEDW(d2b, "mlp_dist.2.bias", 1)
+  GETW(hw.dist2_w, "mlp_dist.2.weight", dim) GETW(hw.dist2_b, "mlp_dist.2.bias", 1)
   NEEDW(s0w, "mlp_shape.0.weight", static_cast<int64_t>(dim) * dim) NEEDW(s0b, "mlp_shape.0.bias", dim)
-  NEEDW(s2w, "mlp_shape.2.weight", static_cast<int64_t>(nb) * dim) NEEDW(s2b, "mlp_shape.2.bias", nb)
+  GETW(hw.shape2_w, "mlp_shape.2.weight", static_cast<int64_t>(nb) * dim) GETW(hw.shape2_b, "mlp_shape.2.bias", nb)
   NEEDW(p0w, "mlp_pose.0.weight", static_cast<int64_t>(dim) * (dim + J6)) NEEDW(p0b, "mlp_pose.0.bias", dim)
-  NEEDW(p2w, "mlp_pose.2.weight", static_cast<int64_t>(J6) * dim) NEEDW(p2b, "mlp_pose.2.bias", J6)
-  NEEDW(useful, "useful_rotmat", J) NEEDW(init, "init_body_pose", J6)
-  (void)o2w; (void)o2b; (void)d2w; (void)d2b; (void)s2w; (void)s2b; (void)useful;
+  GETW(hw.pose2_w, "mlp_pose.2.weight", static_cast<int64_t>(J6) * dim) NEEDW(p2b, "mlp_pose.2.bias", J6)
+  GETW(hw.useful_rotmat, "useful_rotmat", J) NEEDW(init, "init_body_pose", J6)
   TRY(e->alloc(&e->W1, static_cast<size_t>(4) * dim * dim));
   TRY(e->alloc(&e->b1, static_cast<size_t>(4) * dim));
   const size_t blk = static_cast<size_t>(dim) * dim;
@@ -554,12 +562,6 @@ int finalize_anny(mhmr_engine* e, cudaStream_t st) {
   TRY(add_vec(p2b, init, e->b_pose2, J6, J6, st));
 
   // per-person buffers
-  TRY(e->alloc(&e->zc, static_cast<size_t>(Pm) * D));
-  TRY(e->alloc(&e->xa, static_cast<size_t>(Pm) * dim));
-  TRY(e->alloc(&e->qkvp, static_cast<size_t>(Pm) * 3 * inner));
-  TRY(e->alloc(&e->att, static_cast<size_t>(Pm) * inner));
-  TRY(e->alloc(&e->qca, static_cast<size_t>(Pm) * inner));
-  TRY(e->alloc(&e->ffh, static_cast<size_t>(Pm) * mlp));
   TRY(e->alloc(&e->offh, static_cast<size_t>(Pm) * 4 * dim));
   TRY(e->alloc(&e->dec, static_cast<size_t>(Pm) * J6p));
   if (e->cfg.refine_central) TRY(alloc_refine(e, Pm + Bm, st));
@@ -627,13 +629,11 @@ int vit_forward(mhmr_engine* e, const ImgSrc& x, int B, float* z_out, cudaStream
     TRY(run_plan(e, MHMR_CAT_GEMM_FC2, L.fc2, M, st));
   }
   // final norm, cls dropped: fp32 features (head query side, optional user copy) + fp16 context columns
-  const float* ng = e->w(e->enc + "norm.weight");
-  const float* nb = e->w(e->enc + "norm.bias");
   if (e->ln_fold) {
     LAUNCH(MHMR_CAT_LAYERNORM,
-           layernorm_split(e->Xn16, e->Xlo, ng, nb, e->ctx16, e->Cp, e->z32, D, M, D, 1e-6f, T, 1, st));
+           layernorm_split(e->Xn16, e->Xlo, e->norm_g, e->norm_b, e->ctx16, e->Cp, e->z32, D, M, D, 1e-6f, T, 1, st));
   } else {
-    LAUNCH(MHMR_CAT_LAYERNORM, layernorm(e->X, ng, nb, e->ctx16, e->Cp, e->z32, D, M, D, 1e-6f, T, 1, st));
+    LAUNCH(MHMR_CAT_LAYERNORM, layernorm(e->X, e->norm_g, e->norm_b, e->ctx16, e->Cp, e->z32, D, M, D, 1e-6f, T, 1, st));
   }
   if (z_out != nullptr)
     MHMR_CUDA_CHECK(cudaMemcpyAsync(z_out, e->z32, static_cast<size_t>(B) * N * D * 4, cudaMemcpyDeviceToDevice, st));
@@ -664,44 +664,79 @@ int refine_streams(mhmr_engine* e, const ImgSrc& x, const int* det_b, const int*
   return MHMR_OK;
 }
 
+// Detection: the hidden layer as a GEMM over every cell, the score row + sigmoid (`clamp`: clamped sigmoid, SMPL-X;
+// `logits`: optional copy of the pre-sigmoid scores), then the forced persons or NMS.  The true count (may exceed max_persons: reported as an error
+// by mhmr_sync_count, which reads the pinned host copy) goes to count_true, the count clamped to max_persons, which the
+// per-person kernels iterate over, to e->count + 2.
+int detect(mhmr_engine* e, int B, float det_thresh, int nms, const int64_t* forced_idx, int forced_P, bool clamp,
+           float* logits, float* scores_map, int* det_idx, float* det_score, int* count_true, cudaStream_t st) {
+  const int D = e->D, res = e->res, Pm = e->cfg.max_persons, BN = B * e->N;
+  int* det_b = det_idx; int* det_y = det_idx + Pm; int* det_x = det_idx + 2 * Pm;
+  int* count = e->count + 2;
+  TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->cls0_plan, BN, st));
+  LAUNCH(MHMR_CAT_HEAD, rowdot_sigmoid(e->H16, D, e->cls2_w, e->cls2_b, e->scores_raw, logits, clamp, BN, D, st));
+  if (forced_idx != nullptr) {
+    LAUNCH(MHMR_CAT_HEAD, forced_detections(e->scores_raw, scores_map, B, res, forced_idx, forced_P, det_b, det_y, det_x,
+                                            det_score, count_true, count, e->img_off, st));
+  } else {
+    LAUNCH(MHMR_CAT_HEAD, nms_compact(e->scores_raw, scores_map, B, res, nms, det_thresh, Pm, det_b, det_y, det_x,
+                                      det_score, count_true, count, e->img_off, st));
+  }
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->h_count, count_true, sizeof(int), cudaMemcpyDeviceToHost, st));
+  return MHMR_OK;
+}
+
+// HPH layers on the person tokens e->xa (cross_attn_transformer.py / hph.py): PreNorm self-attention among the persons
+// of one image, cross-attention to the keys / values of every cell (e->KV32), feed-forward
+int hph_decoder(mhmr_engine* e, const int* det_b, const int* count, cudaStream_t st) {
+  const int dim = e->dec_dim, mlp = e->dec_mlp, Pm = e->cfg.max_persons, N = e->N;
+  const int heads = e->cfg.xat_num_heads, inner = heads * 32;
+  for (int l = 0; l < e->cfg.xat_depth; ++l) {
+    HphLayer& L = e->hph[l];
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wqkv, dim, nullptr, 3 * inner, L.ln0_g, L.ln0_b, 1e-5f, 0,
+                                        nullptr, 0, e->qkvp, 3 * inner, st));
+    LAUNCH(MHMR_CAT_HEAD, hph_self_attn(e->qkvp, 3 * inner, det_b, e->img_off, count, Pm, heads, e->att, inner, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->att, inner, count, Pm, inner, L.Wsa_out, inner, L.bsa_out, dim, nullptr, nullptr,
+                                        0.f, 0, e->xa, dim, e->xa, dim, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wq, dim, nullptr, inner, L.ln1_g, L.ln1_b, 1e-5f, 0,
+                                        nullptr, 0, e->qca, inner, st));
+    LAUNCH(MHMR_CAT_HEAD, hph_cross_attn(e->qca, inner, e->KV32, e->nkv, l * 2 * inner, l * 2 * inner + inner, det_b, count,
+                                         Pm, heads, N, e->att, inner, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->att, inner, count, Pm, inner, L.Wca_out, inner, L.bca_out, dim, nullptr, nullptr,
+                                        0.f, 0, e->xa, dim, e->xa, dim, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wff0, dim, L.bff0, mlp, L.ln2_g, L.ln2_b, 1e-5f, 2,
+                                        nullptr, 0, e->ffh, mlp, st));
+    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->ffh, mlp, count, Pm, mlp, L.Wff3, mlp, L.bff3, dim, nullptr, nullptr, 0.f, 0,
+                                        e->xa, dim, e->xa, dim, st));
+  }
+  return MHMR_OK;
+}
+
 int head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float det_thresh, int nms, const int64_t* forced_idx,
                  int forced_P, const mhmr_outputs* o, cudaStream_t st) {
   const int D = e->D, N = e->N, res = e->res, Pm = e->cfg.max_persons, Cq = e->Cq, nb = e->cfg.num_betas;
-  const int heads = e->cfg.xat_num_heads, inner = heads * 32, BN = B * N;
+  const SmplxHeadWeights& hw = e->smplx_w;
   int* det_b = o->det_idx; int* det_y = o->det_idx + Pm; int* det_x = o->det_idx + 2 * Pm;
-  int* count_true = o->count;   // true number of detections (may exceed max_persons: reported as an error)
-  int* count = e->count + 2;    // clamped to max_persons: what the per-person kernels iterate over
+  int* count = e->count + 2;
   LAUNCH(MHMR_CAT_HEAD, invert_K(K, e->Kinv, B, st));
-  LAUNCH(MHMR_CAT_HEAD, ctx_fourier(e->Kinv, e->w("camera.freq_bands"), e->ctx16, e->Cp, B, res, D, e->Cp - D, st));
+  LAUNCH(MHMR_CAT_HEAD, ctx_fourier(e->Kinv, hw.freq_bands, e->ctx16, e->Cp, B, res, D, e->Cp - D, st));
   // detection (model.py:133-158)
-  TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->cls0_plan, BN, st));
-  LAUNCH(MHMR_CAT_HEAD, rowdot_sigmoid(e->H16, D, e->w("mlp_classif.2.weight"), e->w("mlp_classif.2.bias"), e->scores_raw,
-                                       nullptr, true, BN, D, st));
-  if (forced_idx != nullptr) {
-    LAUNCH(MHMR_CAT_HEAD, forced_detections(e->scores_raw, o->scores_map, B, res, forced_idx, forced_P, det_b, det_y, det_x,
-                         o->det_score, count_true, count, e->img_off, st));
-  } else {
-    LAUNCH(MHMR_CAT_HEAD, nms_compact(e->scores_raw, o->scores_map, B, res, nms, det_thresh, Pm, det_b, det_y, det_x,
-                       o->det_score, count_true, count, e->img_off, st));
-  }
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->h_count, count_true, sizeof(int), cudaMemcpyDeviceToHost, st));
+  TRY(detect(e, B, det_thresh, nms, forced_idx, forced_P, true, nullptr, o->scores_map, o->det_idx, o->det_score, o->count,
+             st));
   // keys / values of both decoder layers for every token (to_kv, cross_attn_transformer.py:187)
-  TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->kv_plan, BN, st));
-  const std::string h = "x_attention_head.";
+  TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->kv_plan, B * N, st));
   const float* xr = nullptr;
   if (e->cfg.refine_central) {
     TRY(refine_streams(e, x, det_b, det_y, det_x, count, 0, nullptr, st));
     xr = e->r_x;
   }
-  LAUNCH(MHMR_CAT_HEAD, person_gather(e->z32, xr, e->w(e->enc + "norm.weight"), e->w(e->enc + "norm.bias"),
-                       e->Kinv, e->w("camera.freq_bands"), e->w(h + "cross_queries_x"),
-                       e->w(h + "cross_queries_y"), e->w(h + "cross_values_x"), e->w(h + "cross_values_y"),
-                       det_b, det_y, det_x, count, Pm, res, D, e->zc, e->query, e->vals, Cq, st));
+  LAUNCH(MHMR_CAT_HEAD, person_gather(e->z32, xr, e->norm_g, e->norm_b, e->Kinv, hw.freq_bands, hw.cq_x, hw.cq_y, hw.cv_x,
+                                      hw.cv_y, det_b, det_y, det_x, count, Pm, res, D, e->zc, e->query, e->vals, Cq, st));
   // offset head (model.py:258)
-  LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->zc, D, count, Pm, D, e->w("mlp_offset.0.weight"), D, e->w("mlp_offset.0.bias"), D,
-                       nullptr, nullptr, 0.f, 1, nullptr, 0, e->offh, D, st));
-  LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->offh, D, count, Pm, D, e->w("mlp_offset.2.weight"), D, e->w("mlp_offset.2.bias"), 2,
-                       nullptr, nullptr, 0.f, 0, nullptr, 0, o->offset, 2, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->zc, D, count, Pm, D, hw.off0_w, D, hw.off0_b, D, nullptr, nullptr, 0.f, 1, nullptr, 0,
+                                      e->offh, D, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->offh, D, count, Pm, D, hw.off2_w, D, hw.off2_b, 2, nullptr, nullptr, 0.f, 0, nullptr,
+                                      0, o->offset, 2, st));
   // learned value embeddings injected at the detected cells (model.py:514-517)
   LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->vals, Cq, count, Pm, e->C, e->Wkv32, Cq, nullptr, e->nkv, nullptr, nullptr, 0.f, 0,
                        nullptr, 0, e->dKV, e->nkv, st));
@@ -709,24 +744,7 @@ int head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float d
   // token embedding (cross_attn_transformer.py:352-357)
   LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->query, Cq, count, Pm, e->C, e->Wte_q, Cq, e->te_const, kHphDim, nullptr, nullptr, 0.f,
                        0, nullptr, 0, e->xa, kHphDim, st));
-  for (int l = 0; l < e->cfg.xat_depth; ++l) {
-    HphLayer& L = e->hph[l];
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, kHphDim, count, Pm, kHphDim, L.Wqkv, kHphDim, nullptr, 3 * inner, L.ln0_g, L.ln0_b,
-                         1e-5f, 0, nullptr, 0, e->qkvp, 3 * inner, st));
-    LAUNCH(MHMR_CAT_HEAD, hph_self_attn(e->qkvp, 3 * inner, det_b, e->img_off, count, Pm, heads, e->att, inner, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->att, inner, count, Pm, inner, L.Wsa_out, inner, L.bsa_out, kHphDim, nullptr, nullptr,
-                         0.f, 0, e->xa, kHphDim, e->xa, kHphDim, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, kHphDim, count, Pm, kHphDim, L.Wq, kHphDim, nullptr, inner, L.ln1_g, L.ln1_b, 1e-5f,
-                         0, nullptr, 0, e->qca, inner, st));
-    LAUNCH(MHMR_CAT_HEAD, hph_cross_attn(e->qca, inner, e->KV32, e->nkv, l * 2 * inner, l * 2 * inner + inner, det_b, count, Pm,
-                          heads, N, e->att, inner, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->att, inner, count, Pm, inner, L.Wca_out, inner, L.bca_out, kHphDim, nullptr, nullptr,
-                         0.f, 0, e->xa, kHphDim, e->xa, kHphDim, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, kHphDim, count, Pm, kHphDim, L.Wff0, kHphDim, L.bff0, kHphDim, L.ln2_g, L.ln2_b,
-                         1e-5f, 2, nullptr, 0, e->ffh, kHphDim, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->ffh, kHphDim, count, Pm, kHphDim, L.Wff3, kHphDim, L.bff3, kHphDim, nullptr, nullptr,
-                         0.f, 0, e->xa, kHphDim, e->xa, kHphDim, st));
-  }
+  TRY(hph_decoder(e, det_b, count, st));
   LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, kHphDim, count, Pm, kHphDim, e->Wdec, kHphDim, e->bdec, e->ndec, nullptr, nullptr, 0.f,
                        0, nullptr, 0, e->dec, e->ndec, st));
   const float focal_norm = static_cast<float>(e->cfg.img_size / (2.0 * tan(30.0 * 3.14159265358979323846 / 180.0)));
@@ -747,24 +765,13 @@ int head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float d
 int anny_head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float det_thresh, int nms,
                       const int64_t* forced_idx, int forced_P, const mhmr_anny_outputs* o, cudaStream_t st) {
   const int D = e->D, N = e->N, T = e->T, res = e->res, Pm = e->cfg.max_persons, Bm = e->cfg.max_batch;
-  const int nb = e->cfg.num_betas, dim = e->cfg.xat_dim, mlp = e->cfg.xat_mlp_dim, J = e->cfg.num_joints;
-  const int heads = e->cfg.xat_num_heads, inner = heads * 32, BN = B * N, J6p = (6 * J + 3) & ~3;
+  const int nb = e->cfg.num_betas, dim = e->dec_dim, J = e->cfg.num_joints, BN = B * N, J6p = (6 * J + 3) & ~3;
+  const AnnyHeadWeights& hw = e->anny_w;
   int* det_b = o->det_idx; int* det_y = o->det_idx + Pm; int* det_x = o->det_idx + 2 * Pm;
   int* count = e->count + 2;
-  const float* ng = e->w(e->enc + "norm.weight");
-  const float* nbias = e->w(e->enc + "norm.bias");
   // detection (encoder.py:59-60, multi_hmr.py:116-124)
-  TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->cls0_plan, BN, st));
-  LAUNCH(MHMR_CAT_HEAD, rowdot_sigmoid(e->H16, D, e->w("encoder.mlp_det.2.weight"), e->w("encoder.mlp_det.2.bias"),
-                                       e->scores_raw, o->logits, false, BN, D, st));
-  if (forced_idx != nullptr) {
-    LAUNCH(MHMR_CAT_HEAD, forced_detections(e->scores_raw, o->scores_map, B, res, forced_idx, forced_P, det_b, det_y, det_x,
-                                            e->det_score, o->count, count, e->img_off, st));
-  } else {
-    LAUNCH(MHMR_CAT_HEAD, nms_compact(e->scores_raw, o->scores_map, B, res, nms, det_thresh, Pm, det_b, det_y, det_x,
-                                      e->det_score, o->count, count, e->img_off, st));
-  }
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(e->h_count, o->count, sizeof(int), cudaMemcpyDeviceToHost, st));
+  TRY(detect(e, B, det_thresh, nms, forced_idx, forced_P, false, o->logits, o->scores_map, o->det_idx, e->det_score,
+             o->count, st));
   // decoder tokens of every cell and the keys / values of every HPH layer
   TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->dt_plan, BN, st));
   TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->kv_plan, BN, st));
@@ -781,50 +788,31 @@ int anny_head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, fl
     LAUNCH(MHMR_CAT_HEAD, cls_gather(e->X, nullptr, D, T, B, D, e->cls_x, st));
   }
   // field of view and intrinsics (encoder.py:50-56)
-  LAUNCH(MHMR_CAT_HEAD, skinny_linear(cls_src, D, e->anny_ints, Bm, D, e->w("encoder.mlp_fov_unique.0.weight"), D,
-                                      e->w("encoder.mlp_fov_unique.0.bias"), D, ng, nbias, 1e-6f, 1, nullptr, 0, e->cls_h,
-                                      D, st));
-  LAUNCH(MHMR_CAT_HEAD, anny_camera(e->cls_h, D, e->w("encoder.mlp_fov_unique.2.weight"), e->w("encoder.mlp_fov_unique.2.bias"),
-                                    e->w("encoder.fov_max"), K, B, e->cfg.img_size, o->fov, o->K_regressed, e->K_use,
-                                    e->Kinv, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(cls_src, D, e->anny_ints, Bm, D, hw.fov0_w, D, hw.fov0_b, D, e->norm_g, e->norm_b,
+                                      1e-6f, 1, nullptr, 0, e->cls_h, D, st));
+  LAUNCH(MHMR_CAT_HEAD, anny_camera(e->cls_h, D, hw.fov2_w, hw.fov2_b, hw.fov_max, K, B, e->cfg.img_size, o->fov,
+                                    o->K_regressed, e->K_use, e->Kinv, st));
   ++e->launches;  // anny_camera = 2 kernels
   // queries: dec_to_token(final-normed feature) + dec_pos_emb at the detected cells (multi_hmr.py:131)
-  LAUNCH(MHMR_CAT_HEAD, anny_gather(e->z32, xr, ng, nbias, e->w("dec_pos_emb"), det_b, det_y, det_x, count, Pm, res, D,
-                                    dim, e->zc, e->xa, st));
-  LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->zc, D, count, Pm, D, e->w("dec_to_token.weight"), D, e->w("dec_to_token.bias"), dim,
-                                      nullptr, nullptr, 0.f, 0, e->xa, dim, e->xa, dim, st));
-  // HPH (hph.py:133-140): PreNorm self-attention, cross-attention, feed-forward
-  for (int l = 0; l < e->cfg.xat_depth; ++l) {
-    HphLayer& L = e->hph[l];
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wqkv, dim, nullptr, 3 * inner, L.ln0_g, L.ln0_b, 1e-5f, 0,
-                                        nullptr, 0, e->qkvp, 3 * inner, st));
-    LAUNCH(MHMR_CAT_HEAD, hph_self_attn(e->qkvp, 3 * inner, det_b, e->img_off, count, Pm, heads, e->att, inner, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->att, inner, count, Pm, inner, L.Wsa_out, inner, L.bsa_out, dim, nullptr, nullptr,
-                                        0.f, 0, e->xa, dim, e->xa, dim, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wq, dim, nullptr, inner, L.ln1_g, L.ln1_b, 1e-5f, 0,
-                                        nullptr, 0, e->qca, inner, st));
-    LAUNCH(MHMR_CAT_HEAD, hph_cross_attn(e->qca, inner, e->KV32, e->nkv, l * 2 * inner, l * 2 * inner + inner, det_b, count,
-                                         Pm, heads, N, e->att, inner, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->att, inner, count, Pm, inner, L.Wca_out, inner, L.bca_out, dim, nullptr, nullptr,
-                                        0.f, 0, e->xa, dim, e->xa, dim, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, L.Wff0, dim, L.bff0, mlp, L.ln2_g, L.ln2_b, 1e-5f, 2,
-                                        nullptr, 0, e->ffh, mlp, st));
-    LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->ffh, mlp, count, Pm, mlp, L.Wff3, mlp, L.bff3, dim, nullptr, nullptr, 0.f, 0,
-                                        e->xa, dim, e->xa, dim, st));
-  }
+  LAUNCH(MHMR_CAT_HEAD, anny_gather(e->z32, xr, e->norm_g, e->norm_b, hw.dec_pos_emb, det_b, det_y, det_x, count, Pm, res,
+                                    D, dim, e->zc, e->xa, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->zc, D, count, Pm, D, hw.dt_w, D, hw.dt_b, dim, nullptr, nullptr, 0.f, 0, e->xa, dim,
+                                      e->xa, dim, st));
+  // HPH (hph.py:133-140)
+  TRY(hph_decoder(e, det_b, count, st));
   // regressors: hidden layers of offset | dist | shape | pose at once, then the four output Linears
   float* hid = e->offh;
   LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, dim, count, Pm, dim, e->W1, dim, e->b1, 4 * dim, nullptr, nullptr, 0.f, 1,
                                       nullptr, 0, hid, 4 * dim, st));
-  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid, 4 * dim, count, Pm, dim, e->w("mlp_offset.2.weight"), dim, e->w("mlp_offset.2.bias"),
-                                      2, nullptr, nullptr, 0.f, 0, nullptr, 0, o->offset, 2, st));
-  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + dim, 4 * dim, count, Pm, dim, e->w("mlp_dist.2.weight"), dim,
-                                      e->w("mlp_dist.2.bias"), 1, nullptr, nullptr, 0.f, 0, nullptr, 0, o->dist_pp, 1, st));
-  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + 2 * dim, 4 * dim, count, Pm, dim, e->w("mlp_shape.2.weight"), dim,
-                                      e->w("mlp_shape.2.bias"), nb, nullptr, nullptr, 0.f, 0, nullptr, 0, o->shape, nb, st));
-  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + 3 * dim, 4 * dim, count, Pm, dim, e->w("mlp_pose.2.weight"), dim, e->b_pose2,
-                                      6 * J, nullptr, nullptr, 0.f, 0, nullptr, 0, e->dec, J6p, st));
-  LAUNCH(MHMR_CAT_HEAD, anny_person_post(e->dec, J6p, J, e->w("useful_rotmat"), o->shape, nb, o->offset, o->dist_pp, e->K_use,
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid, 4 * dim, count, Pm, dim, hw.off2_w, dim, hw.off2_b, 2, nullptr, nullptr, 0.f, 0,
+                                      nullptr, 0, o->offset, 2, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + dim, 4 * dim, count, Pm, dim, hw.dist2_w, dim, hw.dist2_b, 1, nullptr, nullptr,
+                                      0.f, 0, nullptr, 0, o->dist_pp, 1, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + 2 * dim, 4 * dim, count, Pm, dim, hw.shape2_w, dim, hw.shape2_b, nb, nullptr,
+                                      nullptr, 0.f, 0, nullptr, 0, o->shape, nb, st));
+  LAUNCH(MHMR_CAT_HEAD, skinny_linear(hid + 3 * dim, 4 * dim, count, Pm, dim, hw.pose2_w, dim, e->b_pose2, 6 * J, nullptr,
+                                      nullptr, 0.f, 0, nullptr, 0, e->dec, J6p, st));
+  LAUNCH(MHMR_CAT_HEAD, anny_person_post(e->dec, J6p, J, hw.useful_rotmat, o->shape, nb, o->offset, o->dist_pp, e->K_use,
                                          e->Kinv, det_b, det_y, det_x, count, Pm, o->rotmat, o->rotmat_homo, o->rotvec,
                                          o->dist, o->loc, o->transl, o->K_det, st));
   return MHMR_OK;
@@ -858,8 +846,13 @@ int mhmr_create(const mhmr_config* cfg, mhmr_engine** out) {
   auto e = std::make_unique<mhmr_engine>();
   e->cfg = *cfg;
   const ArchSpec& a = kArch[cfg->arch];
-  e->D = a.D; e->depth = a.depth; e->heads = a.heads;
-  if (cfg->head == MHMR_HEAD_ANNY) e->enc = "encoder.backbone.";
+  e->D = a.D; e->depth = a.depth;
+  e->dec_dim = e->dec_mlp = kHphDim;
+  if (cfg->head == MHMR_HEAD_ANNY) {
+    e->enc = "encoder.backbone.";
+    e->dec_dim = cfg->xat_dim;
+    e->dec_mlp = cfg->xat_mlp_dim;
+  }
   e->res = cfg->img_size / 14;
   e->N = e->res * e->res;
   e->T = e->N + 1;
@@ -920,15 +913,24 @@ int mhmr_finalize(mhmr_engine* h) {
   return MHMR_OK;
 }
 
-static int forward_impl(mhmr_engine* h, const ImgSrc& x, const float* K, int B, float det_thresh,
-                        int nms_kernel_size, const int64_t* forced_idx, int forced_P, const mhmr_outputs* out,
-                        void* stream) {
-  MHMR_REQUIRE(h != nullptr && K != nullptr && out != nullptr, "null argument");
-  if (!h->finalized) { set_last_error("mhmr_forward before mhmr_finalize"); return MHMR_ERR_STATE; }
-  MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_SMPLX, "mhmr_forward needs an SMPL-X engine (use mhmr_forward_anny)");
+// checks of the engine, batch and forced persons that every forward entry makes; `entry` names it in the messages
+static int check_forward(mhmr_engine* h, const void* out, int head, const char* entry, int B, const int64_t* forced_idx,
+                         int forced_P) {
+  MHMR_REQUIRE(h != nullptr && out != nullptr, "null argument");
+  if (!h->finalized) { set_last_error(std::string(entry) + " before mhmr_finalize"); return MHMR_ERR_STATE; }
+  MHMR_REQUIRE(h->cfg.head == head, std::string(entry) + " needs an engine created with head = " +
+                                        (head == MHMR_HEAD_ANNY ? "MHMR_HEAD_ANNY" : "MHMR_HEAD_SMPLX"));
   MHMR_REQUIRE(B >= 1 && B <= h->cfg.max_batch, "batch exceeds max_batch");
   MHMR_REQUIRE(forced_idx == nullptr || (forced_P >= 0 && forced_P <= h->cfg.max_persons),
                "forced_P exceeds max_persons");
+  return MHMR_OK;
+}
+
+static int forward_impl(mhmr_engine* h, const ImgSrc& x, const float* K, int B, float det_thresh,
+                        int nms_kernel_size, const int64_t* forced_idx, int forced_P, const mhmr_outputs* out,
+                        void* stream) {
+  MHMR_REQUIRE(K != nullptr, "null argument");
+  TRY(check_forward(h, out, MHMR_HEAD_SMPLX, "mhmr_forward", B, forced_idx, forced_P));
   MHMR_REQUIRE(out->scores_map && out->count && out->det_idx && out->det_score && out->offset && out->loc &&
                    out->dist_pp && out->dist && out->rotmat && out->rotvec && out->shape && out->expression &&
                    out->transl && out->transl_pelvis && out->v3d && out->j3d && out->j2d,
@@ -961,12 +963,7 @@ int mhmr_forward_u8(mhmr_engine* h, const uint8_t* img_u8, const float* lut, con
 static int forward_anny_impl(mhmr_engine* h, const ImgSrc& x, const float* K, int B, float det_thresh,
                              int nms_kernel_size, const int64_t* forced_idx, int forced_P, const mhmr_anny_outputs* out,
                              void* stream) {
-  MHMR_REQUIRE(h != nullptr && out != nullptr, "null argument");
-  if (!h->finalized) { set_last_error("mhmr_forward_anny before mhmr_finalize"); return MHMR_ERR_STATE; }
-  MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_ANNY, "mhmr_forward_anny needs an engine created with head = MHMR_HEAD_ANNY");
-  MHMR_REQUIRE(B >= 1 && B <= h->cfg.max_batch, "batch exceeds max_batch");
-  MHMR_REQUIRE(forced_idx == nullptr || (forced_P >= 0 && forced_P <= h->cfg.max_persons),
-               "forced_P exceeds max_persons");
+  TRY(check_forward(h, out, MHMR_HEAD_ANNY, "mhmr_forward_anny", B, forced_idx, forced_P));
   // multi_hmr.py:118: an even kernel changes the pooled map's shape and the reference fails on the comparison
   MHMR_REQUIRE(forced_idx != nullptr || nms_kernel_size <= 1 || nms_kernel_size % 2 == 1,
                "nms_kernel_size must be odd");

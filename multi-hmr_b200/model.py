@@ -73,8 +73,181 @@ def interpolate_pos_embed(pos_embed: torch.Tensor, grid: int) -> torch.Tensor:
     return torch.cat((pos[:, :1], patch.permute(0, 2, 3, 1).reshape(1, -1, d)), dim=1)
 
 
-class Model:
+class _EngineModel:
+    """What the SMPL-X and Anny models share: one engine behind the C-ABI, the weight upload, the forward call."""
+
+    _IGNORED_PREFIX = ""   # state-dict keys load_state_dict drops
+    _POS_EMBED_KEY = ""    # the backbone's pos_embed, interpolated to the working grid at upload
+    _SKIPPED_KEYS = ()     # state-dict keys the engine does not read
+    _ENTRY = ""            # forward entry of the C-ABI; "_u8" appended for uint8 images
+    _OUT_STRUCT = None     # ctypes struct of that entry's output pointers, one field per output tensor
+    PROFILE_CATEGORIES = ("misc", "layernorm", "gemm_qkv", "attention", "gemm_proj", "gemm_fc1", "gemm_fc2",
+                          "gemm_other", "head", "smplx", "refine")
+
+    def __init__(self, backbone, img_size, max_batch, max_persons, refine_central, device):
+        if not torch.cuda.is_available():
+            raise RuntimeError(f"multihmr_b200.{type(self).__name__} needs a CUDA device (sm_90a); there is no CPU "
+                               "fallback")
+        self.device = torch.device(device if device is not None else "cuda:0")
+        self.backbone_name, self.img_size, self.patch_size = backbone, int(img_size), PATCH_SIZE
+        self.embed_dim = EMBED_DIM[backbone]
+        # capacity of the per-person buffers for the WHOLE batch; the reference has no limit, so the default
+        # scales with the batch (crowded scenes: 16 persons per image on average)
+        self.max_batch = int(max_batch)
+        self.max_persons = int(max_persons) if max_persons is not None else DEFAULT_PERSONS_PER_IMAGE * self.max_batch
+        self.refine_central = bool(refine_central)
+        self.res = self.img_size // PATCH_SIZE
+        self._lib = _lib.load()
+        self._handle = None
+        self._state = {}
+        self._finalized = False
+        self.training = False
+
+    # ------------------------------------------------------------------ nn.Module-like surface
+    def to(self, *a, **k):
+        return self
+
+    def cuda(self, *a, **k):
+        return self
+
+    def eval(self):
+        return self
+
+    def state_dict(self):
+        return dict(self._state)
+
+    def load_state_dict(self, state_dict, strict=False):
+        """Accepts the reference's state-dict keys; keys under `_IGNORED_PREFIX` are ignored."""
+        if self._finalized:
+            raise RuntimeError("weights are frozen after the first forward")
+        unexpected = []
+        for k, v in state_dict.items():
+            if k.startswith(self._IGNORED_PREFIX):
+                continue
+            if not torch.is_tensor(v):
+                unexpected.append(k)
+                continue
+            self._state[k] = v.detach()
+        if strict and unexpected:
+            raise RuntimeError(f"unexpected keys: {unexpected}")
+        return SimpleNamespace(missing_keys=[], unexpected_keys=unexpected)
+
+    # ------------------------------------------------------------------ load-time packing
+    def _head_config(self) -> dict:
+        """The `_Config` fields of the head (all but arch, sizes, capacities and refine_central)."""
+        raise NotImplementedError
+
+    def _upload_extras(self):
+        """Uploads what the engine needs beyond the state dict."""
+
+    def _set_weight(self, key, t):
+        t = t.detach().to(torch.float32).contiguous()
+        check(self._lib.mhmr_set_weight(self._handle, key.encode(), ptr(t), c_int64(t.numel())), f"set_weight({key})")
+
+    def finalize(self):
+        if self._finalized:
+            return self
+        with torch.cuda.device(self.device):
+            cfg = _Config(arch=ARCH_ID[self.backbone_name], img_size=self.img_size, max_batch=self.max_batch,
+                          max_persons=self.max_persons, refine_central=1 if self.refine_central else 0,
+                          **self._head_config())
+            h = c_void_p()
+            check(self._lib.mhmr_create(ctypes.byref(cfg), ctypes.byref(h)), "mhmr_create")
+            self._handle = h
+            for k, v in self._state.items():
+                if k == self._POS_EMBED_KEY:
+                    v = interpolate_pos_embed(v.cpu(), self.res)
+                if k in self._SKIPPED_KEYS:
+                    continue
+                self._set_weight(k, v)
+            self._upload_extras()
+            check(self._lib.mhmr_finalize(self._handle), "mhmr_finalize")
+        self._finalized = True
+        return self
+
+    def __del__(self):
+        try:
+            if self._handle is not None:
+                self._lib.mhmr_destroy(self._handle)
+                self._handle = None
+        except Exception:
+            pass
+
+    # ------------------------------------------------------------------ forward
+    def _prepare_image(self, x):
+        """-> (image on the device, fused): uint8 [B,S,S,3] RGB goes to the fused loader (normalize_rgb + patch rows in
+        one kernel), anything else is the normalised [B,3,S,S] image as fp32."""
+        fused = x.dtype == torch.uint8
+        if fused:
+            x = x.to(self.device, non_blocking=True).contiguous()
+            assert x.dim() == 4 and x.shape[3] == 3 and x.shape[1] == x.shape[2] == self.img_size, "bad image shape"
+        else:
+            x = x.to(self.device, dtype=torch.float32, non_blocking=True).contiguous()
+            assert x.dim() == 4 and x.shape[1] == 3 and x.shape[2] == x.shape[3] == self.img_size, "bad image shape"
+        return x, fused
+
+    def _forced_idx(self, rows, B):
+        """Index rows (batch, y, x[, 4th]) of the forced persons -> [4, P] int64 host tensor, zeros as the missing 4th
+        row.  The reference indexes tensors with idx and raises IndexError when it is out of range (model.py:246-255);
+        the kernels trust the indices, so they are validated here."""
+        rows = [i.to(torch.int64).cpu() for i in rows]
+        h_idx = torch.stack(rows if len(rows) == 4 else rows + [torch.zeros_like(rows[0])])
+        P = int(h_idx.shape[1])
+        if P > 0:
+            if h_idx[0].min() < 0 or h_idx[0].max() >= B or h_idx[1:3].min() < 0 or h_idx[1:3].max() >= self.res:
+                raise IndexError(f"idx out of range for batch {B} and a {self.res}x{self.res} token grid")
+            if P > self.max_persons:
+                raise _lib.MhmrError(f"{P} forced persons > max_persons {self.max_persons}")
+        return h_idx
+
+    def _run(self, x, fused, K, det_thresh, nms_kernel_size, fidx, t):
+        """Enqueues the forward into the output tensors `t` (None: not wanted) on the current stream and returns the
+        number of persons."""
+        if isinstance(det_thresh, list):
+            det_thresh = det_thresh[0]                                               # model.py:614-615
+        o = self._OUT_STRUCT(*[ptr(t[n]).value if t[n] is not None else None for n, _ in self._OUT_STRUCT._fields_])
+        fP = 0
+        if fidx is not None:
+            fP = int(fidx.shape[1])
+            fidx = fidx.to(self.device).contiguous()
+        stream = c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        args = (ptr(K), c_int(x.shape[0]), ctypes.c_float(float(det_thresh)), c_int(int(nms_kernel_size)), ptr(fidx),
+                c_int(fP), ctypes.byref(o), stream)
+        if fused:
+            from .preprocess import device_table
+            entry = self._ENTRY + "_u8"
+            check(getattr(self._lib, entry)(self._handle, ptr(x), ptr(device_table(self.device)), *args), entry)
+        else:
+            check(getattr(self._lib, self._ENTRY)(self._handle, ptr(x), *args), self._ENTRY)
+        n = c_int(0)
+        check(self._lib.mhmr_sync_count(self._handle, stream, ctypes.byref(n)), "mhmr_sync_count")
+        self.last_outputs = t
+        return int(n.value)
+
+    def last_launch_count(self) -> int:
+        return int(self._lib.mhmr_last_launch_count(self._handle))
+
+    def set_profiling(self, enable: bool):
+        self.finalize()
+        check(self._lib.mhmr_set_profiling(self._handle, c_int(1 if enable else 0)), "mhmr_set_profiling")
+
+    def get_profile(self) -> dict:
+        """{category: (device ms summed over launches, launches)} since profiling was enabled / last read."""
+        n = len(self.PROFILE_CATEGORIES)
+        ms, cnt = (ctypes.c_float * n)(), (ctypes.c_int * n)()
+        check(self._lib.mhmr_get_profile(self._handle, ms, cnt), "mhmr_get_profile")
+        return {c: (float(ms[i]), int(cnt[i])) for i, c in enumerate(self.PROFILE_CATEGORIES)}
+
+
+class Model(_EngineModel):
     """H100-native drop-in for reference `model.Model` (inference path)."""
+
+    # the reference's checkpoints exclude the body model's buffers (train.py:195-201)
+    _IGNORED_PREFIX = "smpl_layer."
+    _POS_EMBED_KEY = "backbone.encoder.pos_embed"
+    _SKIPPED_KEYS = ("backbone.encoder.mask_token", "x_attention_head.init_betas_kid", "x_attention_head.init_expression")
+    _ENTRY = "mhmr_forward"
+    _OUT_STRUCT = _Outputs
 
     def __init__(self, backbone="dinov2_vitb14", pretrained_backbone=False, img_size=896,
                  camera_embedding="geometric", camera_embedding_num_bands=16,
@@ -94,63 +267,16 @@ class Model:
         if person_center not in KINEMATIC_JOINTS:
             raise NotImplementedError(f"person_center {person_center!r}: only the 55 kinematic SMPL-X joints are "
                                       "supported as person centre (vertex-picked joints / landmarks are not)")
-        if not torch.cuda.is_available():
-            raise RuntimeError("multihmr_b200.Model needs a CUDA device (sm_90a); there is no CPU fallback")
-        self.device = torch.device(device if device is not None else "cuda:0")
-        self.backbone_name = backbone
-        self.img_size = img_size
-        self.patch_size = PATCH_SIZE
-        self.embed_dim = EMBED_DIM[backbone]
+        super().__init__(backbone, img_size, max_batch, max_persons, refine_central, device)
         self.nearness = nearness
         self.clip_dist = (clip_dist,)
         self.xat_depth, self.xat_num_heads, self.num_betas = xat_depth, xat_num_heads, num_betas
         self.person_center = person_center
         self.fovn = 60
-        # capacity of the per-person buffers for the WHOLE batch; the reference has no limit, so the default
-        # scales with the batch (crowded scenes: 16 persons per image on average)
-        self.max_batch = int(max_batch)
-        self.max_persons = int(max_persons) if max_persons is not None else DEFAULT_PERSONS_PER_IMAGE * self.max_batch
-        self.refine_central = bool(refine_central)
-        self.res = img_size // PATCH_SIZE
         self.num_verts = NUM_VERTS
-        self._lib = _lib.load()
-        self._handle = None
-        self._state = {}
-        self._finalized = False
         self.smpl_layer = {}
-        self.training = False
         if body_model is not None:
             self.set_body_model(body_model)
-
-    # ------------------------------------------------------------------ nn.Module-like surface
-    def to(self, *a, **k):
-        return self
-
-    def cuda(self, *a, **k):
-        return self
-
-    def eval(self):
-        return self
-
-    def state_dict(self):
-        return dict(self._state)
-
-    def load_state_dict(self, state_dict, strict=False):
-        """Accepts the reference's `model_state_dict` (demo.py:103).  `smpl_layer.*` keys are ignored, as the
-        reference's checkpoints exclude them (train.py:195-201)."""
-        if self._finalized:
-            raise RuntimeError("weights are frozen after the first forward")
-        unexpected = []
-        for k, v in state_dict.items():
-            if k.startswith("smpl_layer."):
-                continue
-            if not torch.is_tensor(v):
-                unexpected.append(k)
-                continue
-            self._state[k] = v.detach()
-        if strict and unexpected:
-            raise RuntimeError(f"unexpected keys: {unexpected}")
-        return SimpleNamespace(missing_keys=[], unexpected_keys=unexpected)
 
     def set_body_model(self, bm: dict):
         """Body-model buffers as `smplx.create(..., 'smplx', gender='neutral', use_pca=False,
@@ -162,36 +288,20 @@ class Model:
         self.smpl_layer = {"neutral_10": layer, "neutral_11": layer}  # demo.py:310 reads .bm_x.faces
 
     # ------------------------------------------------------------------ load-time packing
-    def _set_weight(self, key, t):
-        t = t.detach().to(torch.float32).contiguous()
-        check(self._lib.mhmr_set_weight(self._handle, key.encode(), ptr(t), c_int64(t.numel())), f"set_weight({key})")
-
     def _set_table(self, key, t):
         t = t.detach().to(torch.int32).contiguous().cpu()
         check(self._lib.mhmr_set_table_i32(self._handle, key.encode(), ptr(t), c_int64(t.numel())), f"set_table({key})")
 
     def finalize(self):
-        if self._finalized:
-            return self
-        if not hasattr(self, "_bm"):
+        if not self._finalized and not hasattr(self, "_bm"):
             raise RuntimeError("no body model: call set_body_model() (SMPL-X buffers) before the first forward")
-        with torch.cuda.device(self.device):
-            return self._finalize_on_device()
+        return super().finalize()
 
-    def _finalize_on_device(self):
-        cfg = _Config(ARCH_ID[self.backbone_name], self.img_size, self.max_batch, self.max_persons, self.xat_depth,
-                      self.xat_num_heads, self.num_betas, KINEMATIC_JOINTS.index(self.person_center),
-                      self.num_verts, 1 if self.refine_central else 0)
-        h = c_void_p()
-        check(self._lib.mhmr_create(ctypes.byref(cfg), ctypes.byref(h)), "mhmr_create")
-        self._handle = h
-        sd = self._state
-        for k, v in sd.items():
-            if k == "backbone.encoder.pos_embed":
-                v = interpolate_pos_embed(v.cpu(), self.res)
-            if k in ("backbone.encoder.mask_token", "x_attention_head.init_betas_kid", "x_attention_head.init_expression"):
-                continue
-            self._set_weight(k, v)
+    def _head_config(self):
+        return dict(xat_depth=self.xat_depth, xat_num_heads=self.xat_num_heads, num_betas=self.num_betas,
+                    person_center_idx=KINEMATIC_JOINTS.index(self.person_center), num_verts=self.num_verts)
+
+    def _upload_extras(self):
         self._set_weight("camera.freq_bands", torch.linspace(1.0, 32.0, 16))       # blocks/camera_embed.py:46
         bm = self._bm
         nb = self.num_betas
@@ -208,17 +318,6 @@ class Model:
         self._set_table("smplx.parents", bm["parents"])
         self._set_table("smplx.extra_joints_idxs", bm["extra_joints_idxs"])
         self._set_table("smplx.lmk_tri", bm["faces"][bm["lmk_faces_idx"]])
-        check(self._lib.mhmr_finalize(self._handle), "mhmr_finalize")
-        self._finalized = True
-        return self
-
-    def __del__(self):
-        try:
-            if self._handle is not None:
-                self._lib.mhmr_destroy(self._handle)
-                self._handle = None
-        except Exception:
-            pass
 
     # ------------------------------------------------------------------ forward
     def _alloc_outputs(self, B, want_v2d, want_z):
@@ -241,54 +340,20 @@ class Model:
             return self._forward_raw(x, K, idx, det_thresh, nms_kernel_size, want_v2d, want_z)
 
     def _forward_raw(self, x, K, idx, det_thresh, nms_kernel_size, want_v2d, want_z):
-        if isinstance(det_thresh, list):
-            det_thresh = det_thresh[0]                                               # model.py:614-615
-        fused = x.dtype == torch.uint8   # uint8 [B,S,S,3] RGB: fused loader (normalize_rgb + patch rows in one kernel)
-        if fused:
-            x = x.to(self.device, non_blocking=True).contiguous()
-            assert x.dim() == 4 and x.shape[3] == 3 and x.shape[1] == x.shape[2] == self.img_size, "bad image shape"
-        else:
-            x = x.to(self.device, dtype=torch.float32, non_blocking=True).contiguous()
-            assert x.dim() == 4 and x.shape[1] == 3 and x.shape[2] == x.shape[3] == self.img_size, "bad image shape"
+        x, fused = self._prepare_image(x)
         K = K.to(self.device, dtype=torch.float32, non_blocking=True).contiguous()
         B = x.shape[0]
         assert K.shape == (B, 3, 3), "K must be [B,3,3]"
         t = self._alloc_outputs(B, want_v2d, want_z)
-        o = _Outputs(*[ptr(t[n]).value if t[n] is not None else None for n in _OUT_FIELDS])
-        fidx, fP, unsort = None, 0, None
+        fidx, unsort = None, None
         if idx is not None:
-            fidx = torch.stack([i.to(torch.int64) for i in idx[:4]] if len(idx) >= 4 else
-                               [i.to(torch.int64) for i in idx[:3]] + [torch.zeros_like(idx[0], dtype=torch.int64)])
-            fP = int(fidx.shape[1])
-            # the reference indexes tensors with idx and raises IndexError when it is out of range
-            # (model.py:246-255); the kernels trust the indices, so they are validated here
-            h_idx = fidx.cpu()
-            if fP > 0:
-                if (h_idx[0].min() < 0 or h_idx[0].max() >= B or h_idx[1:3].min() < 0
-                        or h_idx[1:3].max() >= self.res):
-                    raise IndexError(f"idx out of range for batch {B} and a {self.res}x{self.res} token grid")
-                if fP > self.max_persons:
-                    raise _lib.MhmrError(f"{fP} forced persons > max_persons {self.max_persons}")
-                if (h_idx[0][1:] < h_idx[0][:-1]).any():
-                    # persons of one image must be contiguous for the engine: run in image order, restore after
-                    order = torch.argsort(h_idx[0], stable=True)
-                    h_idx = h_idx[:, order]
-                    unsort = torch.argsort(order).to(self.device)
-            fidx = h_idx.to(self.device).contiguous()
-        stream = c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-        if fused:
-            from .preprocess import device_table
-            lut = device_table(self.device)
-            check(self._lib.mhmr_forward_u8(self._handle, ptr(x), ptr(lut), ptr(K), c_int(B),
-                                            ctypes.c_float(float(det_thresh)), c_int(int(nms_kernel_size)), ptr(fidx),
-                                            c_int(fP), ctypes.byref(o), stream), "mhmr_forward_u8")
-        else:
-            check(self._lib.mhmr_forward(self._handle, ptr(x), ptr(K), c_int(B), ctypes.c_float(float(det_thresh)),
-                                         c_int(int(nms_kernel_size)), ptr(fidx), c_int(fP), ctypes.byref(o), stream),
-                  "mhmr_forward")
-        n = c_int(0)
-        check(self._lib.mhmr_sync_count(self._handle, stream, ctypes.byref(n)), "mhmr_sync_count")
-        P = int(n.value)
+            fidx = self._forced_idx(idx[:4] if len(idx) >= 4 else idx[:3], B)
+            if (fidx[0][1:] < fidx[0][:-1]).any():
+                # persons of one image must be contiguous for the engine: run in image order, restore after
+                order = torch.argsort(fidx[0], stable=True)
+                fidx = fidx[:, order]
+                unsort = torch.argsort(order).to(self.device)
+        P = self._run(x, fused, K, det_thresh, nms_kernel_size, fidx, t)
         if unsort is not None and P > 0:
             per_person = ("det_score", "offset", "loc", "dist_pp", "dist", "rotmat", "rotvec", "shape", "expression",
                           "transl", "transl_pelvis", "v3d", "v2d", "j3d", "j2d")
@@ -296,7 +361,6 @@ class Model:
                 if t[k] is not None:
                     t[k][:P] = t[k][:P].index_select(0, unsort)
             t["det_idx"][:, :P] = t["det_idx"][:, :P].index_select(1, unsort)
-        self.last_outputs = t
         return t, P
 
     def forward(self, x, idx=None, det_thresh=0.3, nms_kernel_size=3, K=None, is_training=False, *args, **kwargs):
@@ -358,20 +422,3 @@ class Model:
                                                ptr(out["transl_pelvis"]), stream), "mhmr_smplx_forward")
         out["transl_pelvis"] = out["transl_pelvis"][:, None]
         return out
-
-    def last_launch_count(self) -> int:
-        return int(self._lib.mhmr_last_launch_count(self._handle))
-
-    PROFILE_CATEGORIES = ("misc", "layernorm", "gemm_qkv", "attention", "gemm_proj", "gemm_fc1", "gemm_fc2",
-                          "gemm_other", "head", "smplx", "refine")
-
-    def set_profiling(self, enable: bool):
-        self.finalize()
-        check(self._lib.mhmr_set_profiling(self._handle, c_int(1 if enable else 0)), "mhmr_set_profiling")
-
-    def get_profile(self) -> dict:
-        """{category: (device ms summed over launches, launches)} since profiling was enabled / last read."""
-        n = len(self.PROFILE_CATEGORIES)
-        ms, cnt = (ctypes.c_float * n)(), (ctypes.c_int * n)()
-        check(self._lib.mhmr_get_profile(self._handle, ms, cnt), "mhmr_get_profile")
-        return {c: (float(ms[i]), int(cnt[i])) for i, c in enumerate(self.PROFILE_CATEGORIES)}

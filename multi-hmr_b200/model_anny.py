@@ -10,13 +10,11 @@ after it (centre bone, translation, projection) runs in the sm_90a kernels behin
 from __future__ import annotations
 
 import ctypes
-from types import SimpleNamespace
 
 import torch
 
-from . import _lib
 from ._lib import c_int, c_void_p, check, ptr
-from .model import ARCH_ID, EMBED_DIM, PATCH_SIZE, _Config, interpolate_pos_embed
+from .model import ARCH_ID, PATCH_SIZE, _EngineModel
 
 ANNY_SHAPE_KEYS = ("age", "gender", "weight", "height", "muscle", "proportions")   # multi_hmr.py:171
 _OUT_FIELDS = ("scores_map", "logits", "count", "det_idx", "K_regressed", "fov", "K_det", "offset", "loc", "dist",
@@ -39,8 +37,14 @@ def create_anny_body_model():
     return bm
 
 
-class ModelAnny:
+class ModelAnny(_EngineModel):
     """H100-native drop-in for reference `multi_hmr_anny.multi_hmr.Multi_HMR` (inference path)."""
+
+    _IGNORED_PREFIX = "body_model."   # the body model's own buffers
+    _POS_EMBED_KEY = "encoder.backbone.pos_embed"
+    _SKIPPED_KEYS = ("encoder.backbone.mask_token", "eye")
+    _ENTRY = "mhmr_forward_anny"
+    _OUT_STRUCT = _AnnyOutputs
 
     def __init__(self, img_size=896, backbone="dinov2_vits14", pretrained_backbone=False, xat_dim=512, xat_depth=8,
                  xat_heads=16, xat_dim_head=32, xat_mlp_dim=4 * 512, xat_dropout=0.0, person_center="head",
@@ -54,22 +58,9 @@ class ModelAnny:
         assert img_size % PATCH_SIZE == 0, "Invalid img size"                           # multi_hmr.py:47
         if xat_dim_head != 32:
             raise NotImplementedError("the HPH kernels are built for xat_dim_head = 32")
-        if not torch.cuda.is_available():
-            raise RuntimeError("multihmr_b200.ModelAnny needs a CUDA device (sm_90a); there is no CPU fallback")
-        self.device = torch.device(device if device is not None else "cuda:0")
-        self.backbone_name, self.img_size, self.patch_size = backbone, int(img_size), PATCH_SIZE
-        self.embed_dim = EMBED_DIM[backbone]
+        super().__init__(backbone, img_size, max_batch, max_persons, refine_central, device)
         self.xat_dim, self.xat_depth, self.xat_heads, self.xat_mlp_dim = xat_dim, xat_depth, xat_heads, xat_mlp_dim
         self.num_betas, self.person_center = num_betas, person_center
-        self.max_batch = int(max_batch)
-        self.max_persons = int(max_persons) if max_persons is not None else 16 * self.max_batch
-        self.refine_central = bool(refine_central)
-        self.res = self.img_size // PATCH_SIZE
-        self._lib = _lib.load()
-        self._handle = None
-        self._state = {}
-        self._finalized = False
-        self.training = False
         self.body_model = (body_model if body_model is not None else create_anny_body_model()).to(self.device)
         self.person_center_idx = list(self.body_model.bone_labels).index(person_center)
         self.n_joints = len(self.body_model.bone_labels)
@@ -77,64 +68,10 @@ class ModelAnny:
         if any(l >= num_betas for _, l in self._shape_cols):
             raise ValueError("the body model's phenotype labels do not fit in num_betas shape outputs")
 
-    # ------------------------------------------------------------------ nn.Module-like surface
-    def to(self, *a, **k):
-        return self
-
-    def cuda(self, *a, **k):
-        return self
-
-    def eval(self):
-        return self
-
-    def state_dict(self):
-        return dict(self._state)
-
-    def load_state_dict(self, state_dict, strict=False):
-        """Accepts `Multi_HMR.state_dict()` keys; the body model's own buffers (`body_model.*`) are ignored."""
-        if self._finalized:
-            raise RuntimeError("weights are frozen after the first forward")
-        unexpected = []
-        for k, v in state_dict.items():
-            if k.startswith("body_model."):
-                continue
-            if not torch.is_tensor(v):
-                unexpected.append(k)
-                continue
-            self._state[k] = v.detach()
-        if strict and unexpected:
-            raise RuntimeError(f"unexpected keys: {unexpected}")
-        return SimpleNamespace(missing_keys=[], unexpected_keys=unexpected)
-
-    def finalize(self):
-        if self._finalized:
-            return self
-        with torch.cuda.device(self.device):
-            cfg = _Config(ARCH_ID[self.backbone_name], self.img_size, self.max_batch, self.max_persons, self.xat_depth,
-                          self.xat_heads, self.num_betas, self.person_center_idx, 0, 1 if self.refine_central else 0,
-                          HEAD_ANNY, self.xat_dim, self.xat_mlp_dim, self.n_joints)
-            h = c_void_p()
-            check(self._lib.mhmr_create(ctypes.byref(cfg), ctypes.byref(h)), "mhmr_create")
-            self._handle = h
-            for k, v in self._state.items():
-                if k == "encoder.backbone.pos_embed":
-                    v = interpolate_pos_embed(v.cpu(), self.res)
-                if k in ("encoder.backbone.mask_token", "eye"):
-                    continue
-                t = v.detach().to(torch.float32).contiguous()
-                check(self._lib.mhmr_set_weight(self._handle, k.encode(), ptr(t), ctypes.c_int64(t.numel())),
-                      f"set_weight({k})")
-            check(self._lib.mhmr_finalize(self._handle), "mhmr_finalize")
-        self._finalized = True
-        return self
-
-    def __del__(self):
-        try:
-            if self._handle is not None:
-                self._lib.mhmr_destroy(self._handle)
-                self._handle = None
-        except Exception:
-            pass
+    def _head_config(self):
+        return dict(xat_depth=self.xat_depth, xat_num_heads=self.xat_heads, num_betas=self.num_betas,
+                    person_center_idx=self.person_center_idx, head=HEAD_ANNY, xat_dim=self.xat_dim,
+                    xat_mlp_dim=self.xat_mlp_dim, num_joints=self.n_joints)
 
     # ------------------------------------------------------------------ forward
     def forward_raw(self, x, K=None, idx=None, det_thresh=0.3, nms_kernel_size=3, want_z=False):
@@ -144,16 +81,8 @@ class ModelAnny:
             return self._forward_raw(x, K, idx, det_thresh, nms_kernel_size, want_z)
 
     def _forward_raw(self, x, K, idx, det_thresh, nms_kernel_size, want_z):
-        if isinstance(det_thresh, list):
-            det_thresh = det_thresh[0]
         dev = self.device
-        fused = x.dtype == torch.uint8
-        if fused:
-            x = x.to(dev, non_blocking=True).contiguous()
-            assert x.dim() == 4 and x.shape[3] == 3 and x.shape[1] == x.shape[2] == self.img_size, "bad image shape"
-        else:
-            x = x.to(dev, dtype=torch.float32, non_blocking=True).contiguous()
-            assert x.dim() == 4 and x.shape[1] == 3 and x.shape[2] == x.shape[3] == self.img_size, "bad image shape"
+        x, fused = self._prepare_image(x)
         B = x.shape[0]
         if K is not None:
             K = K.to(dev, dtype=torch.float32, non_blocking=True).contiguous()
@@ -165,35 +94,12 @@ class ModelAnny:
              "K_det": f(Pm, 3, 3), "offset": f(Pm, 2), "loc": f(Pm, 2), "dist": f(Pm), "dist_pp": f(Pm),
              "shape": f(Pm, nb), "rotmat": f(Pm, J, 3, 3), "rotmat_homo": f(Pm, J, 4, 4), "rotvec": f(Pm, J, 3),
              "transl": f(Pm, 3), "z": f(B, r * r, self.embed_dim) if want_z else None}
-        o = _AnnyOutputs(*[ptr(t[n]).value if t[n] is not None else None for n in _OUT_FIELDS])
-        fidx, fP = None, 0
+        fidx = None
         if idx is not None:
-            fidx = torch.stack([i.to(torch.int64).cpu() for i in idx[:3]] + [torch.zeros_like(idx[0], dtype=torch.int64).cpu()])
-            fP = int(fidx.shape[1])
-            if fP > 0:
-                if fidx[0].min() < 0 or fidx[0].max() >= B or fidx[1:3].min() < 0 or fidx[1:3].max() >= r:
-                    raise IndexError(f"idx out of range for batch {B} and a {r}x{r} token grid")
-                if fP > Pm:
-                    raise _lib.MhmrError(f"{fP} forced persons > max_persons {Pm}")
-                if (fidx[0][1:] < fidx[0][:-1]).any():
-                    raise ValueError("idx must list the persons of each image contiguously, in image order")
-            fidx = fidx.to(dev).contiguous()
-        stream = c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        Kp = ptr(K) if K is not None else None
-        if fused:
-            from .preprocess import device_table
-            lut = device_table(dev)
-            check(self._lib.mhmr_forward_anny_u8(self._handle, ptr(x), ptr(lut), Kp, c_int(B),
-                                                 ctypes.c_float(float(det_thresh)), c_int(int(nms_kernel_size)),
-                                                 ptr(fidx), c_int(fP), ctypes.byref(o), stream), "mhmr_forward_anny_u8")
-        else:
-            check(self._lib.mhmr_forward_anny(self._handle, ptr(x), Kp, c_int(B), ctypes.c_float(float(det_thresh)),
-                                              c_int(int(nms_kernel_size)), ptr(fidx), c_int(fP), ctypes.byref(o),
-                                              stream), "mhmr_forward_anny")
-        n = c_int(0)
-        check(self._lib.mhmr_sync_count(self._handle, stream, ctypes.byref(n)), "mhmr_sync_count")
-        self.last_outputs = t
-        return t, int(n.value)
+            fidx = self._forced_idx(idx[:3], B)
+            if (fidx[0][1:] < fidx[0][:-1]).any():
+                raise ValueError("idx must list the persons of each image contiguously, in image order")
+        return t, self._run(x, fused, K, det_thresh, nms_kernel_size, fidx, t)
 
     def place(self, out_bm, t, P, want_v2d):
         """Body-model output -> camera space (mhmr_anny_place): v3d, j3d, j2d, v2d, transl_pelvis."""
@@ -253,6 +159,3 @@ class ModelAnny:
         return [persons[i] for i in order]
 
     __call__ = forward
-
-    def last_launch_count(self) -> int:
-        return int(self._lib.mhmr_last_launch_count(self._handle))

@@ -131,6 +131,28 @@ def test_no_detection_even_nms_and_bulk_path(cuda_device):
     assert err["v3d"] < 1e-2
 
 
+def test_forced_idx_validation(cuda_device):
+    """Forced persons are checked before anything is enqueued: an index outside the batch or the token grid raises
+    IndexError, persons not grouped by image raise ValueError, more persons than max_persons raise MhmrError."""
+    from multihmr_b200 import _lib
+
+    case, sd, bm, x, K, idx = au.build_inputs("anny_224_S_forced")
+    m = au.build_engine(case, sd, bm, max_persons=8)
+    for row, value in ((0, case["batch"]), (1, case["img_size"] // 14), (2, -1)):
+        bad = tuple(t.clone() for t in idx)
+        bad[row][0] = value
+        with pytest.raises(IndexError):
+            m(x, K=K, idx=bad, is_training=True)
+    P = idx[0].shape[0]
+    perm = torch.tensor([P - 1 - i for i in range(P)])
+    with pytest.raises(ValueError, match="contiguously"):
+        m(x, K=K, idx=tuple(t[perm] for t in idx), is_training=True)
+    crowd = tuple(torch.cat([t] * 2) for t in idx)   # 10 persons, still grouped by image
+    crowd = tuple(t[torch.argsort(crowd[0], stable=True)] for t in crowd)
+    with pytest.raises(_lib.MhmrError, match="max_persons"):
+        m(x, K=K, idx=crowd, is_training=True)
+
+
 def _anny_head_reference(z, sd, idx, K, depth, heads, fp16_context=True):
     """The Anny head of oracle/anny_ref.py (hph, _mlp and the post-processing of anny_forward) in fp64 on the engine's
     final-normed features z [B, N, D], rounded to fp16 where the engine rounds (engine.cu, Anny setup):
