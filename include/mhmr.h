@@ -440,6 +440,43 @@ int mhmr_body_forward(mhmr_body* h, int P, const float* full_pose, const float* 
                       const float* transl, const float* K, float* v3d, float* v2d, float* j3d, float* j2d,
                       float* transl_pelvis, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Mesh renderer: the overlay of reference utils/render.py:175 `render_meshes` (pyrender / OpenGL there), reached from
+ * demo.py:340-346 `overlay_human_meshes`, the rotating video (demo.py:159-195), app.py and train.py:440-469.  A
+ * z-buffer rasterizer over meshes already on the device, for any body model (SMPL-X, Anny): one sample per pixel
+ * centre, top-left fill rule, back faces culled, near plane 0.05 / far plane 100, pyrender's metallic-roughness
+ * shading under a white directional light at the camera plus ambient 0.3, then the reference's 3x3 foreground
+ * smoothing and alpha blend.  Four launches per call, no host synchronisation.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct mhmr_render mhmr_render;
+typedef struct mhmr_render_args {
+  int views, H, W;              /* B views of H x W pixels                                                        */
+  const uint8_t* images;        /* backgrounds [*, H, W, 3] RGB                                                   */
+  const int32_t* view_image;    /* [views]: background image of each view; person p is drawn into view b when
+                                   person_image[p] == view_image[b]                                               */
+  const float* K;               /* [views, 3, 3] intrinsics, fx > 0 and fy > 0 (a view without is left empty)     */
+  const float* pose;            /* [views, 3, 4] world -> camera [R | t] (OpenCV convention, R a rotation), NULL = I */
+  const float* verts;           /* [max_persons, num_verts, 3] in world (camera) coordinates, metres              */
+  int max_persons;
+  const int32_t* person_image;  /* [max_persons] image of each person (the engine's det_idx[0])                   */
+  const int32_t* count;         /* [1] persons, read on the device (clamped to [0, max_persons])                  */
+  const float* colors;          /* [max_persons, 3] base colours in [0, 1]                                        */
+  float alpha, intensity, metallic, roughness;
+  int smooth;                   /* 1: trimesh's angle-weighted vertex normals; 0: face normals                    */
+  uint8_t* overlay;             /* out [views, H, W, 3]                                                           */
+  float* depth;                 /* out [views, H, W] camera z, 0 = background (nullable)                          */
+  int32_t* person;              /* out [views, H, W] person index, -1 = background (nullable)                     */
+} mhmr_render_args;
+/* faces int32 [F, 3] (host or device); every index must lie in [0, num_verts).  Builds the vertex -> face CSR of the
+ * normal pass; synchronises `stream`. */
+int mhmr_render_create(const int32_t* faces, int num_faces, int num_verts, void* stream, mhmr_render** out);
+int mhmr_render_destroy(mhmr_render* h);
+/* face_bits: bits of the depth key's low word that hold the face index; max_persons may be up to 2^(32 - face_bits). */
+int mhmr_render_info(const mhmr_render* h, int* num_faces, int* num_verts, int* face_bits);
+/* Every pointer of `a` is a device pointer.  The handle owns a key buffer of 8 B per pixel per view, grown on demand
+ * (growing frees the old buffer, which waits for the device).  One call at a time per handle. */
+int mhmr_render_forward(mhmr_render* h, const mhmr_render_args* a, void* stream);
+
 /* Kernel launches enqueued by the last mhmr_forward (bench.py's `gpu_launches`). */
 int mhmr_last_launch_count(mhmr_engine* h);
 

@@ -43,8 +43,29 @@ def load() -> ctypes.CDLL:
     lib = ctypes.CDLL(LIB_PATH)
     lib.mhmr_last_error.restype = ctypes.c_char_p
     lib.mhmr_last_error.argtypes = []
+    _declare_render(lib)
     _lib = lib
     return lib
+
+
+class RenderArgs(ctypes.Structure):
+    """`mhmr_render_args` of include/mhmr.h."""
+
+    _fields_ = [("views", c_int), ("H", c_int), ("W", c_int), ("images", c_void_p), ("view_image", c_void_p),
+                ("K", c_void_p), ("pose", c_void_p), ("verts", c_void_p), ("max_persons", c_int),
+                ("person_image", c_void_p), ("count", c_void_p), ("colors", c_void_p), ("alpha", c_float),
+                ("intensity", c_float), ("metallic", c_float), ("roughness", c_float), ("smooth", c_int),
+                ("overlay", c_void_p), ("depth", c_void_p), ("person", c_void_p)]
+
+
+def _declare_render(lib) -> None:
+    P = ctypes.POINTER
+    lib.mhmr_render_create.argtypes = [c_void_p, c_int, c_int, c_void_p, P(c_void_p)]
+    lib.mhmr_render_destroy.argtypes = [c_void_p]
+    lib.mhmr_render_info.argtypes = [c_void_p, P(c_int), P(c_int), P(c_int)]
+    lib.mhmr_render_forward.argtypes = [c_void_p, P(RenderArgs), c_void_p]
+    for f in (lib.mhmr_render_create, lib.mhmr_render_destroy, lib.mhmr_render_info, lib.mhmr_render_forward):
+        f.restype = c_int
 
 
 def check(rc: int, what: str = "") -> None:

@@ -248,6 +248,24 @@ class HostBatchLoader:
         return x, k
 
 
+def overlay_human_meshes(humans, faces, K, model, img_pil, unique_color=False, alpha=0.8, _color=None):
+    """demo.py:128-158: the persons of `forward_model` drawn over the photo with `render.render_meshes`, on the
+    device (the vertices stay there).  Colours default to this package's `render.PALETTE` (the first one for
+    every person with `unique_color`).  Returns (uint8 array [H,W,3], colours)."""
+    from .render import PALETTE, render_meshes
+
+    if _color is None:
+        _color = [PALETTE[0] for _ in range(len(humans))] if unique_color else list(PALETTE)
+    K0 = torch.as_tensor(K)[0].detach().cpu().double().numpy()
+    focal, princpt = np.asarray([K0[0, 0], K0[1, 1]]), np.asarray([K0[0, -1], K0[1, -1]])
+    arr = np.asarray(img_pil)
+    if len(humans) > 0:
+        name = "verts_smplx" if "verts_smplx" in humans[0] else "v3d"
+        arr = render_meshes(arr, [h[name] for h in humans], [faces] * len(humans),
+                            {"focal": focal, "princpt": princpt}, alpha=alpha, color=_color)
+    return arr, _color
+
+
 def forward_model(model, input_image, camera_parameters, det_thresh=0.3, nms_kernel_size=1):
     """One forward on an image batch and its intrinsics (demo.py:108-126).  The reference wraps the call in
     no_grad + fp16 autocast; here precision is fixed by the kernels (fp16 tensor-core operands, fp32

@@ -17,6 +17,8 @@ from __future__ import annotations
 
 import math
 
+import numpy as np
+
 import torch
 
 BACKBONES = {
@@ -415,6 +417,58 @@ def _rotation(rv: torch.Tensor) -> torch.Tensor:
     ax = rv / ang
     Kx = torch.tensor([[0.0, -ax[2], ax[1]], [ax[2], 0.0, -ax[0]], [-ax[1], ax[0], 0.0]])
     return torch.eye(3) + torch.sin(ang) * Kx + (1 - torch.cos(ang)) * (Kx @ Kx)
+
+
+def _ellipsoid(n_lat: int, n_lon: int):
+    """Unit UV sphere: vertices [2 + (n_lat-1) n_lon, 3] and faces wound so that cross(v1-v0, v2-v0) points out."""
+    verts = [[0.0, -1.0, 0.0]]
+    for i in range(1, n_lat):
+        th = np.pi * i / n_lat
+        for j in range(n_lon):
+            ph = 2 * np.pi * j / n_lon
+            verts.append([np.sin(th) * np.cos(ph), -np.cos(th), np.sin(th) * np.sin(ph)])
+    verts.append([0.0, 1.0, 0.0])
+    ring = lambda i, j: 1 + (i - 1) * n_lon + (j % n_lon)
+    faces = []
+    for j in range(n_lon):
+        faces.append([0, ring(1, j), ring(1, j + 1)])
+        faces.append([len(verts) - 1, ring(n_lat - 1, j + 1), ring(n_lat - 1, j)])
+        for i in range(1, n_lat - 1):
+            faces.append([ring(i, j), ring(i + 1, j), ring(i + 1, j + 1)])
+            faces.append([ring(i, j), ring(i + 1, j + 1), ring(i, j + 1)])
+    v, f = np.asarray(verts), np.asarray(faces)
+    p = v[f]
+    n = np.cross(p[:, 1] - p[:, 0], p[:, 2] - p[:, 0])
+    flip = (n * p.mean(1)).sum(-1) < 0
+    f[flip] = f[flip][:, [0, 2, 1]]
+    return v, f
+
+
+# (centre, radii) of the parts of a blob person 1.7 m tall, y down (OpenCV camera convention)
+_BLOB_PARTS = [((0.0, -0.75, 0.0), (0.11, 0.13, 0.11)), ((0.0, -0.35, 0.0), (0.19, 0.28, 0.12)),
+               ((-0.27, -0.35, 0.0), (0.06, 0.3, 0.06)), ((0.27, -0.35, 0.0), (0.06, 0.3, 0.06)),
+               ((-0.1, 0.35, 0.0), (0.08, 0.42, 0.08)), ((0.1, 0.35, 0.0), (0.08, 0.42, 0.08))]
+
+
+def make_blob_people(positions, seed: int = 0, n_lat: int = 8, n_lon: int = 12):
+    """Structured test meshes for the renderer: one person = six tessellated ellipsoids (head, torso, arms, legs)
+    with one shared topology.  positions: [P,3] pelvis positions in camera coordinates (metres).  Each person gets a
+    seeded scale, yaw and part jitter.  Returns (verts fp32 [P,V,3], faces int64 [F,3])."""
+    g = np.random.default_rng(seed)
+    uv, uf = _ellipsoid(n_lat, n_lon)
+    faces = np.concatenate([uf + k * len(uv) for k in range(len(_BLOB_PARTS))])
+    out = []
+    for pos in np.asarray(positions, np.float64).reshape(-1, 3):
+        s = g.uniform(0.85, 1.1)
+        yaw = g.uniform(-0.6, 0.6)
+        Ry = np.array([[np.cos(yaw), 0, np.sin(yaw)], [0, 1, 0], [-np.sin(yaw), 0, np.cos(yaw)]])
+        parts = []
+        for c, r in _BLOB_PARTS:
+            rr = np.asarray(r) * g.uniform(0.9, 1.15, 3)
+            cc = np.asarray(c) + g.normal(0, 0.01, 3)
+            parts.append((uv * rr + cc) * s)
+        out.append(np.concatenate(parts) @ Ry.T + pos)
+    return np.asarray(out, np.float32), faces.astype(np.int64)
 
 
 class AnnyLikeBodyModel(torch.nn.Module):
