@@ -30,21 +30,22 @@ def split16(t):
     return hi + r16(t - hi)
 
 
-def ln_linear(x, g, b, w, bias, mode, shift=None):
-    """Linear(LayerNorm(x)) with the engine's rounding points.  mode: 'exact' | 'sep' | 'fold' | 'fold_shift'"""
+def ln_linear(x, g, b, w, bias, mode, shift=None, qa=r16, qw=r16):
+    """Linear(LayerNorm(x)) with the engine's rounding points.  mode: 'exact' | 'sep' | 'fold' | 'fold_shift'.
+    qa / qw round the folded GEMM's operands (fp16 by default)."""
     D = x.shape[-1]
     if mode == "exact":
         return F.linear(F.layer_norm(x, (D,), g, b, EPS), w, bias)
     if mode == "sep":
         return F.linear(r16(F.layer_norm(x, (D,), g, b, EPS)), r16(w), bias)
     wf = w * g
-    wf = r16(wf - wf.mean(1, keepdim=True))   # W' = W diag(gamma) with centred rows, fp16
+    wf = qw(wf - wf.mean(1, keepdim=True))   # W' = W diag(gamma) with centred rows, rounded
     b2 = bias + w @ b
     mean = x.mean(-1, keepdim=True)
     var = (x * x).mean(-1, keepdim=True) - mean * mean
     rstd = torch.rsqrt(var.clamp_min(0) + EPS)
     if mode == "fold":
-        return rstd * F.linear(r16(x), wf) + b2
+        return rstd * F.linear(qa(x), wf) + b2
     # fold_shift: the fp16 copy holds x - shift (shift = the row mean one residual update earlier)
     return rstd * F.linear(r16(x - shift), wf) + b2
 
@@ -56,9 +57,12 @@ def attention(q, k, v):
     return torch.matmul(r16(p), v) / p.sum(dim=-1, keepdim=True)
 
 
-def forward(x_img, sd, name, pre, mode, o_in=None):
+def forward(x_img, sd, name, pre, mode, o_in=None, mlp8=None, keep_cls=False):
     """mode 'sep' / 'fold' / 'fold_shift': bulk pass, returns (z, [O16 per layer], stats).  mode 'refine': fp32
-    stream fed with the given attention outputs."""
+    stream fed with the given attention outputs.  mlp8 = (fc1 A, fc1 W, fc2 A, fc2 W): the 'fold' bulk pass rounds
+    the operands of fc1 (raw stream, folded W') and fc2 (GELU output, W2) with these functions instead of fp16
+    (tools/precision_study.py --fp8).
+    keep_cls: z keeps the final-normed cls row in front."""
     cfg = dinov2_ref.ARCHS[name]
     H = cfg["num_heads"]
     if mode == "refine" or mode == "exact":
@@ -97,15 +101,17 @@ def forward(x_img, sd, name, pre, mode, o_in=None):
         x = x + sd[p + "ls1.gamma"] * F.linear(o, wp if full else r16(wp), sd[p + "attn.proj.bias"])
         if mode.startswith("fold"):
             x = split16(x)
+        qa1, qw1, qa2, qw2 = (r16,) * 4 if mlp8 is None else mlp8
         h = ln_linear(x, sd[p + "norm2.weight"], sd[p + "norm2.bias"], sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"],
-                      "exact" if full else mode, shift)
+                      "exact" if full else mode, shift, qa1, qw1)
         h = F.gelu(h)
         w2 = sd[p + "mlp.fc2.weight"]
         shift = x.mean(-1, keepdim=True)
-        x = x + sd[p + "ls2.gamma"] * F.linear(h if full else r16(h), w2 if full else r16(w2), sd[p + "mlp.fc2.bias"])
+        x = x + sd[p + "ls2.gamma"] * F.linear(h if full else qa2(h), w2 if full else qw2(w2), sd[p + "mlp.fc2.bias"])
         if mode.startswith("fold"):
             x = split16(x)
-    z = F.layer_norm(x, (D,), sd[pre + "norm.weight"], sd[pre + "norm.bias"], EPS)[:, 1:]
+    z = F.layer_norm(x, (D,), sd[pre + "norm.weight"], sd[pre + "norm.bias"], EPS)
+    z = z if keep_cls else z[:, 1:]
     return z, outs, ratios
 
 

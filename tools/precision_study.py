@@ -5,6 +5,8 @@ reports the output error vs the golden fixture (= the unmodified reference) with
 off / split in two fp16 terms.  TEST/DIAGNOSTIC TOOL, never on the product path.
 
     python tools/precision_study.py [case] [--classes ...]
+    python tools/precision_study.py --refine [case] [--reuse-o]
+    python tools/precision_study.py --fp8 [case ...]        FP8 (e4m3, block-scaled) MLP operands, see fp8_study
 """
 import argparse
 import math
@@ -17,7 +19,9 @@ import torch.nn.functional as F
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+import ln_fold_study  # noqa: E402
 import parity_util as pu  # noqa: E402
 from oracle import multihmr_ref, smplx_ref  # noqa: E402
 
@@ -233,8 +237,150 @@ def refine_study(name, reuse_o=False):
                           ("v3d", "rotmat", "shape", "dist", "scores", "expression", "transl", "loc", "j3d")})
 
 
+# ---------------------------------------------------------------------------------------------------
+# "fp8" study: the engine's folded bulk pass (tools/ln_fold_study.py) with the operands of fc1 and fc2 in e4m3 with
+# power-of-two block scales, with and without the fp32 refinement of the detected rows (which reuses O16).
+E4M3_MAX = 448.0
+BLOCK = 128
+
+
+def pow2_scale(amax):
+    """s = 2^ceil(log2(amax / 448)) (exact: frexp), 1 for an all-zero block; amax / s <= 448 always."""
+    m, e = torch.frexp(amax / E4M3_MAX)
+    e = torch.where(m == 0.5, e - 1, e)
+    return torch.where(amax > 0, torch.ldexp(torch.ones_like(amax), e), torch.ones_like(amax))
+
+
+def e4m3(t):
+    return t.to(torch.float8_e4m3fn).to(torch.float32)
+
+
+def q8_act(t):
+    """activations: one scale per (row, 128-column block); returns the dequantised operand"""
+    sh = t.shape
+    b = t.reshape(*sh[:-1], sh[-1] // BLOCK, BLOCK)
+    s = pow2_scale(b.abs().amax(-1, keepdim=True))
+    return (e4m3(b / s) * s).reshape(sh)
+
+
+def q8_w(w):
+    """weights [N, K]: one scale per (128 output rows x 128 K) block (N padded to a multiple of 128)"""
+    N, K = w.shape
+    Np = -(-N // BLOCK) * BLOCK
+    wp = F.pad(w, (0, 0, 0, Np - N)).reshape(Np // BLOCK, BLOCK, K // BLOCK, BLOCK)
+    s = pow2_scale(wp.abs().amax(dim=(1, 3), keepdim=True))
+    return (e4m3(wp / s) * s).reshape(Np, K)[:N]
+
+
+FP8_KEYS = ("scores", "rotvec", "shape", "dist", "loc", "v3d")
+
+
+# which MLP GEMMs take e4m3 operands: (fc1 A, fc1 W, fc2 A, fc2 W), None = the fp16 engine
+FP8_VARIANTS = {"fp16": None, "fp8 fc1+fc2": (q8_act, q8_w) * 2, "fp8 fc1 only": (q8_act, q8_w, r16, r16),
+                "fp8 fc2 only": (r16, r16, q8_act, q8_w)}
+
+
+def _bulk_and_refined(x, sd, backbone, pre, mlp8):
+    """(bulk features with cls row, refined features with cls row): the refined pass is the fp32 stream of every
+    token fed with the bulk pass's O16, so any row of it is what the engine's refinement computes for that row."""
+    zb, outs, _ = ln_fold_study.forward(x, sd, backbone, pre, "fold", mlp8=mlp8, keep_cls=True)
+    zr, _, _ = ln_fold_study.forward(x, sd, backbone, pre, "refine", o_in=outs, keep_cls=True)
+    return zb, zr
+
+
+def _err(out, gold, keys=FP8_KEYS):
+    # the detection goldens hold the reference's person dicts (no dist)
+    return {k: (out[k].reshape(gold[k].shape) - gold[k].float()).abs().max().item() for k in keys if k in gold}
+
+
+def _smplx_tail(case, sd, bm, x, K, idx, zb, zr):
+    """multihmr_ref.model_forward after the backbone, the engine's way: detection, context and to_kv on the bulk
+    features (fp16 head operands, Emu), the persons' queries from zr (bulk or refined rows)."""
+    cfg = multihmr_ref.RefConfig(backbone=case["backbone"], img_size=case["img_size"])
+    body = smplx_ref.SMPLXShim(bm, 10)
+    emu = Emu(sd)
+    zA, zR = zb[:, 1:], zr[:, 1:]
+    B, N, D = zA.shape
+    h = w = int(math.sqrt(N))
+    forced = idx is not None
+    scores, scores_det, idx = multihmr_ref.detection(zA, sd, 3, 0.3, idx, forced, emu)
+    b_idx, y_idx, x_idx = idx[0], idx[1], idx[2]
+    z_central = zR[b_idx, y_idx * w + x_idx]
+    offset = multihmr_ref.regression_mlp(z_central, sd, "mlp_offset")
+    K_det = K[b_idx]
+    z_K = multihmr_ref.embed_camera(K, h, w, cfg)
+    z_central = torch.cat([z_central, z_K[b_idx, y_idx, x_idx]], 1)
+    z_all = torch.cat([zA, z_K.reshape(B, N, -1)], 2)
+    loc = (torch.stack([x_idx, y_idx]).permute(1, 0) + 0.5 + offset) * 14
+    rotmat, shape, expression, cam = multihmr_ref.hph_forward(z_central, z_all, idx, sd, cfg, F.linear, emu)
+    rotvec = multihmr_ref.roma_ref.rotmat_to_rotvec(rotmat)
+    dist = cam[:, 0][:, None] * (K_det[:, [0], [0]] / multihmr_ref.focal_from_fov(cfg.fovn, x.shape[-1]))
+    dist = torch.clamp(torch.exp(dist) - 1e-10, 0, 50)
+    out = {"rotvec": rotvec, "shape": shape, "dist": dist, "loc": loc, "scores": scores if forced else scores_det}
+    out.update(multihmr_ref.smpl_layer_forward(body, rotvec, shape, loc, dist, K_det, expression, 15))
+    return out, torch.stack([b_idx, y_idx, x_idx], 1)
+
+
+def _anny_tail(case, sd, bm, x, K, idx, zb, zr):
+    """oracle.anny_ref.anny_forward with the engine's sources: detection logits and decoder context from the bulk
+    features, the camera (cls row) and the persons' queries from zr.  Head in fp32."""
+    from unittest import mock
+
+    import anny_util
+    from oracle import anny_ref
+    pre_hph = anny_ref.hph
+    w = int(math.sqrt(zb.shape[1] - 1))
+    dim = sd["dec_to_token.weight"].shape[0]
+    dec_r = F.linear(zr[:, 1:], sd["dec_to_token.weight"], sd["dec_to_token.bias"]) + sd["dec_pos_emb"].reshape(1, w * w, dim)
+    queries = iter([dec_r[b, idx[1][idx[0] == b] * w + idx[2][idx[0] == b]]
+                    for b in torch.unique(idx[0], sorted=True).tolist()])
+
+    def hph(q, ctx, sd_, depth, heads):
+        return pre_hph(next(queries), ctx, sd_, depth, heads)
+
+    with mock.patch.object(anny_ref, "intermediate_layers_with_cls", lambda *a, **k: (zb[:, 1:], zr[:, 0])), \
+            mock.patch.object(anny_ref, "hph", hph):
+        out = anny_util.oracle(case, sd, bm, x, K, idx)
+    return out, torch.stack([idx[0], idx[1], idx[2]], 1)
+
+
+def fp8_study(name):
+    """max |d| per output vs the golden for the fp16 and the FP8-MLP bulk pass, each without and with refinement;
+    returns {(variant, refined): (persons, same detections, {output: max |d|})}"""
+    anny = name.startswith("anny")
+    if anny:
+        import anny_util
+        case, sd, bm, x, K, idx = anny_util.build_inputs(name)
+        gold, pre, tail = anny_util.load_golden(name), "encoder.backbone.", _anny_tail
+    else:
+        case, sd, bm, x, K, idx = pu.build_inputs(name)
+        gold, pre, tail = pu.load_golden(name), "backbone.encoder.", _smplx_tail
+    res = {}
+    with torch.no_grad():
+        for variant, mlp8 in FP8_VARIANTS.items():
+            zb, zr = _bulk_and_refined(x, sd, case["backbone"], pre, mlp8)
+            for refined in (False, True):
+                out, det = tail(case, sd, bm, x, K, idx, zb, zr if refined else zb)
+                label = f"{variant:12s} {'refined' if refined else 'bulk   '}"
+                n_gold = gold["v3d"].shape[0]
+                # natural detections: the same count, each within half a patch of the golden's location
+                same = det.shape[0] == n_gold and ("idx" in gold or
+                                                   (out["loc"] - gold["loc"]).abs().max().item() < 7.0)
+                e = _err(out, gold) if det.shape[0] == n_gold else {}
+                res[(variant, refined)] = (det.shape[0], same, e)
+                print(f"{name:18s} {label}  persons {det.shape[0]}/{n_gold} {'same' if same else 'DIFFERENT'}  " +
+                      " ".join(f"{k} {v:.2e}" for k, v in e.items()), flush=True)
+    return res
+
+
 if __name__ == "__main__":
-    if "--refine" in sys.argv:
+    if "--fp8" in sys.argv:
+        torch.set_num_threads(min(32, os.cpu_count()))
+        for n in [a for a in sys.argv[1:] if not a.startswith("--")] or ["s_224_S_forced", "s_224_S_detect",
+                                                                         "s_224_S_outliers", "s_280_L_forced",
+                                                                         "anny_280_L_forced"]:
+            fp8_study(n)
+    elif "--refine" in sys.argv:
         torch.set_num_threads(min(32, os.cpu_count()))
         names = [a for a in sys.argv[1:] if not a.startswith("--")] or ["s_280_L_forced"]
         refine_study(names[0], reuse_o="--reuse-o" in sys.argv)
