@@ -168,7 +168,10 @@ int mhmr_op_split_rowstats(const float* X, void* xhi, void* xlo, int64_t ld16, f
  * bias2[n] = bias[n] + sum_k ln_b[k] W[n,k]; W fp32 [N, K], W16 fp16 [N, K]. */
 int mhmr_op_fold_ln_linear(const float* W, const float* bias, const float* ln_g, const float* ln_b, void* W16,
                            float* bias2, int N, int K, void* stream);
-/* The GEMM of mhmr_op_gemm_f16 with the engine's internal epilogues (kinds 6-9):
+/* The GEMM of mhmr_op_gemm_f16 as the engine runs it: every epilogue kind (0-5 as above, with rows_out / row_off
+ * for kind 4, and the internal kinds 6-9), and a plan built for M rows but run on the first M_run <= M of them
+ * (M_run 0 runs all M), which is how the engine runs its maximum-batch plans at a smaller batch: rows
+ * M_run .. M-1 of A are loaded and nothing is written for them.
  *   6  LS_RESID_SPLIT  x = (x16 + xlo) + gamma * (acc + bias) written back as two fp16 planes (pitch ldx16), and per
  *                      row the (sum, sum of squares) of the new x over the N/stat_slots columns of each slot into
  *                      stats [M, stat_slots]; stat_slots = 2 * ceil(N / tile), tile 128 (block_n 128) or 256
@@ -179,8 +182,8 @@ int mhmr_op_fold_ln_linear(const float* W, const float* bias, const float* ln_g,
  *   9  ROWADD_F16      out16 = acc + rowadd[m % rows_in] */
 int mhmr_op_gemm_internal(const void* A, int64_t lda, const void* W, int64_t ldw, int M, int N, int K, int epilogue,
                           const float* bias, const float* gamma, void* x16, void* xlo, int64_t ldx16, float* stats,
-                          int stat_slots, const float* rowadd, int rows_in, void* out, int64_t ldo, int block_n,
-                          void* stream);
+                          int stat_slots, const float* rowadd, int rows_in, int rows_out, int row_off, void* out,
+                          int64_t ldo, int block_n, int M_run, void* stream);
 /* Camera rays of every token (model.py:160-187): Kinv [B, 3, 3] = K^-1, then ctx[b*res*res + n, col0 + j] = fp16 of
  * feature j < 99 of cell n (the (row, col) grid passed as (x, y)), zero for 99 <= j < pad_cols (<= 128). */
 int mhmr_op_camera_ctx(const float* K, int B, const float* freqs, float* Kinv, void* ctx, int64_t ld, int res, int col0,

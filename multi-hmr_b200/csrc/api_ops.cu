@@ -284,21 +284,23 @@ int mhmr_op_fold_ln_linear(const float* W, const float* bias, const float* ln_g,
 
 int mhmr_op_gemm_internal(const void* A, int64_t lda, const void* W, int64_t ldw, int M, int N, int K, int epilogue,
                           const float* bias, const float* gamma, void* x16, void* xlo, int64_t ldx16, float* stats,
-                          int stat_slots, const float* rowadd, int rows_in, void* out, int64_t ldo, int block_n,
-                          void* stream) {
-  MHMR_REQUIRE(epilogue >= EPI_NUM_PUBLIC_KINDS && epilogue < EPI_NUM_KINDS,
-               "gemm_internal: epilogue must be an internal kind (6..9)");
+                          int stat_slots, const float* rowadd, int rows_in, int rows_out, int row_off, void* out,
+                          int64_t ldo, int block_n, int M_run, void* stream) {
+  MHMR_REQUIRE(epilogue >= 0 && epilogue < EPI_NUM_KINDS, "gemm_internal: epilogue must be a kind in 0..9");
   MHMR_REQUIRE(epilogue != EPI_LS_RESID_SPLIT || (ldx16 >= N && aligned16(x16) && aligned16(xlo)),
                "gemm_internal: the split planes must cover N columns and be 16-byte aligned");
   MHMR_REQUIRE(epilogue == EPI_LS_RESID_SPLIT || (ldo >= N && aligned16(out)),
                "gemm_internal: the output must cover N columns and be 16-byte aligned");
   MHMR_REQUIRE(stats == nullptr || aligned16(stats), "gemm_internal: stats must be 16-byte aligned");
   MHMR_REQUIRE(rowadd == nullptr || aligned16(rowadd), "gemm_internal: rowadd must be 16-byte aligned");
+  MHMR_REQUIRE(M_run >= 0 && M_run <= M, "gemm_internal: M_run must be in [0, M] (0 runs all M rows)");
   GemmEpi ep;
   ep.bias = bias;
   ep.gamma = gamma;
   ep.rowadd = rowadd;
   ep.rows_in = rows_in;
+  ep.rows_out = rows_out;
+  ep.row_off = row_off;
   ep.out = out;
   ep.ldo = ldo;
   ep.x16 = static_cast<__half*>(x16);
@@ -310,7 +312,7 @@ int mhmr_op_gemm_internal(const void* A, int64_t lda, const void* W, int64_t ldw
   int rc = gemm_plan_init(&plan, static_cast<const __half*>(A), lda, static_cast<const __half*>(W), ldw, M, N, K,
                           epilogue, ep, block_n);
   if (rc != MHMR_OK) return rc;
-  return gemm_plan_run(&plan, static_cast<cudaStream_t>(stream));
+  return gemm_plan_run_rows(&plan, M_run > 0 ? M_run : M, static_cast<cudaStream_t>(stream));
 }
 
 int mhmr_op_camera_ctx(const float* K, int B, const float* freqs, float* Kinv, void* ctx, int64_t ld, int res, int col0,

@@ -18,10 +18,11 @@
 // together with O += P_{j-1} V_{j-1} and runs the softmax of S_j while that PV is in flight, and the two take
 // turns issuing their wgmmas (named barriers), so one's softmax runs under the other's MMAs.
 //
-// Ragged sequence (T = N + 1 is 1 mod 128 at 224, 448, 672 and 896 px, 17 mod 128 at 280 and 1288 px): keys
-// beyond T in the last tile are masked to -inf (the rows there belong to the next image or are zero-filled by
-// TMA); a last tile of at most 32 keys runs 32 keys wide (S by m64n32, PV by 2 k-steps). Query rows beyond T are
-// computed and not stored.
+// Ragged sequence (T = N + 1 is 1 mod 128 at 224, 448, 672 and 896 px, 17 mod 128 at 280 and 1288 px): the QKV
+// tensor map is 3-D (column, token, image), so TMA zero-fills the rows of a tile beyond the image's T rather than
+// reading the next image's (P = 0 times a non-finite value there would be NaN); the keys beyond T in the last
+// tile are masked to -inf. A last tile of at most 32 keys runs 32 keys wide (S by m64n32, PV by 2 k-steps). Query
+// rows beyond T are computed and not stored.
 //
 // Grid at ViT-L (16 heads) on 132 SMs: 896 px batch 8 (T = 4097) 4224 CTAs = 32.0 waves; 672 px batch 4
 // (T = 2305) 1216 CTAs = 9.2 waves; 1288 px batch 2 (T = 8465) 2144 CTAs = 16.2 waves.
@@ -161,7 +162,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ 
       if (elect_one_sync()) {
         mbar_arrive_expect_tx(q_full, kTileBytes);
         // Q is read by one CTA, K / V by every query tile of the (image, head): keep K / V in L2
-        tma_load_2d_hint(sQ, &tmQKV, q_full, head * kHeadDim, row0 + q0, kCacheEvictFirst);
+        tma_load_3d_hint(sQ, &tmQKV, q_full, head * kHeadDim, q0, img, kCacheEvictFirst);
       }
       __syncwarp();
       for (int j = 0; j < n_kv; ++j) {
@@ -170,8 +171,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ 
         if (elect_one_sync()) {
           uint8_t* dk = sKV + 2 * s * kTileBytes;
           mbar_arrive_expect_tx(&kv_full[s], 2 * kTileBytes);
-          tma_load_2d_hint(dk, &tmQKV, &kv_full[s], D + head * kHeadDim, row0 + j * kBlockKV, kCacheEvictLast);
-          tma_load_2d_hint(dk + kTileBytes, &tmQKV, &kv_full[s], 2 * D + head * kHeadDim, row0 + j * kBlockKV,
+          tma_load_3d_hint(dk, &tmQKV, &kv_full[s], D + head * kHeadDim, j * kBlockKV, img, kCacheEvictLast);
+          tma_load_3d_hint(dk + kTileBytes, &tmQKV, &kv_full[s], 2 * D + head * kHeadDim, j * kBlockKV, img,
                            kCacheEvictLast);
         }
         __syncwarp();
@@ -286,9 +287,9 @@ int attention_forward(const __half* qkv, int64_t ld_qkv, __half* out, int64_t ld
   MHMR_REQUIRE(D % kHeadDim == 0, "attention: embed dim must be a multiple of 64");
   MHMR_REQUIRE(ld_qkv % 8 == 0 && ldo % 8 == 0, "attention: row pitches must be multiples of 8");
   MHMR_REQUIRE(B > 0 && T > 0, "attention: empty problem");
-  CUtensorMap tm;
-  int rc = make_tmap_2d(&tm, qkv, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, static_cast<uint64_t>(B) * T, 3ull * D,
-                        ld_qkv * 2, 128, 64, true);
+  CUtensorMap tm;  // (column, token, image): boxes of 64 columns x 128 tokens of one image
+  int rc = make_tmap_3d(&tm, qkv, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, B, T, 3ull * D,
+                        static_cast<uint64_t>(T) * ld_qkv * 2, ld_qkv * 2, 128, 64, true);
   if (rc != MHMR_OK) return rc;
   const int heads = D / kHeadDim;
   const int n_qt = (T + kBlockQ - 1) / kBlockQ;

@@ -55,6 +55,11 @@ const char* get_last_error();
 int make_tmap_2d(CUtensorMap* out, const void* gptr, CUtensorMapDataType dtype, int elem_bytes,
                  uint64_t rows, uint64_t cols, uint64_t pitch_bytes, uint32_t box_rows,
                  uint32_t box_cols, bool swizzle128);
+// The same over a stack of `depth` such matrices, `depth_pitch_bytes` apart; the box is box_rows x box_cols of one
+// matrix, so a box that crosses the last row is zero-filled instead of reading the next matrix.
+int make_tmap_3d(CUtensorMap* out, const void* gptr, CUtensorMapDataType dtype, int elem_bytes,
+                 uint64_t depth, uint64_t rows, uint64_t cols, uint64_t depth_pitch_bytes, uint64_t pitch_bytes,
+                 uint32_t box_rows, uint32_t box_cols, bool swizzle128);
 
 int device_sm_count();
 // Function attributes (cudaFuncSetAttribute) and the SM count are per DEVICE: `first()` is true the first time
@@ -152,6 +157,18 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorM
       :
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)),
         "r"(c_inner), "r"(c_outer), "l"(cache_hint)
+      : "memory");
+}
+// 3-D tile load (make_tmap_3d): column, row within matrix `c_depth`.
+__device__ __forceinline__ void tma_load_3d_hint(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar,
+                                                 int32_t c_inner, int32_t c_row, int32_t c_depth,
+                                                 uint64_t cache_hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)),
+        "r"(c_inner), "r"(c_row), "r"(c_depth), "l"(cache_hint)
       : "memory");
 }
 // 2-D tile store shared -> global (bulk async group).

@@ -595,10 +595,7 @@ struct ProfScope {
 
 int run_plan(mhmr_engine* e, int cat, GemmPlan& plan, int M, cudaStream_t st) {
   ProfScope ps_(e, cat, st);
-  GemmPlan p = plan;  // tensor maps were built for the maximum M; the kernel bounds rows by p.M
-  p.M = M;
-  p.grid = gemm_plan_grid(&p, M);
-  TRY(gemm_plan_run(&p, st));
+  TRY(gemm_plan_run_rows(&plan, M, st));  // plans are built for the maximum batch
   ++e->launches;
   return MHMR_OK;
 }

@@ -319,4 +319,12 @@ int gemm_plan_run(const GemmPlan* plan, cudaStream_t stream) {
   return plan->bn == 256 ? launch_bn<256, 1>(plan, stream) : launch_bn<128, 1>(plan, stream);
 }
 
+int gemm_plan_run_rows(const GemmPlan* plan, int M, cudaStream_t stream) {
+  MHMR_REQUIRE(M > 0 && M <= plan->M, "gemm: a plan runs at most the rows it was built for");
+  GemmPlan p = *plan;  // the tensor map of A still spans plan->M rows; the kernel stores only rows below p.M
+  p.M = M;
+  p.grid = gemm_plan_grid(&p, M);
+  return gemm_plan_run(&p, stream);
+}
+
 }  // namespace mhmr

@@ -74,6 +74,9 @@ struct GemmPlan {
 int gemm_plan_init(GemmPlan* plan, const __half* A, int64_t lda, const __half* W, int64_t ldw, int M,
                    int N, int K, int epi_kind, const GemmEpi& ep, int bn);
 int gemm_plan_run(const GemmPlan* plan, cudaStream_t stream);
+// Runs the plan on its first M (<= plan->M) rows: re-gridded for M, rows M .. plan->M - 1 are loaded (the tensor
+// map covers them) but neither stored nor counted in the statistics.  The engine runs its maximum-batch plans so.
+int gemm_plan_run_rows(const GemmPlan* plan, int M, cudaStream_t stream);
 // launch geometry for `M` rows with this plan's tile shape
 int gemm_plan_grid(const GemmPlan* plan, int M);
 // partial-statistics slots per row that an EPI_LS_RESID_SPLIT GEMM with N columns and tile selector `bn` writes

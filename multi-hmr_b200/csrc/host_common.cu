@@ -66,6 +66,35 @@ int make_tmap_2d(CUtensorMap* out, const void* gptr, CUtensorMapDataType dtype, 
   return MHMR_OK;
 }
 
+int make_tmap_3d(CUtensorMap* out, const void* gptr, CUtensorMapDataType dtype, int elem_bytes,
+                 uint64_t depth, uint64_t rows, uint64_t cols, uint64_t depth_pitch_bytes, uint64_t pitch_bytes,
+                 uint32_t box_rows, uint32_t box_cols, bool swizzle128) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (fn == nullptr) {
+    set_last_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+    return MHMR_ERR_CUDA;
+  }
+  if (swizzle128 && box_cols * static_cast<uint32_t>(elem_bytes) != 128u) {
+    set_last_error("make_tmap_3d: 128B swizzle needs a 128-byte inner box");
+    return MHMR_ERR_ARG;
+  }
+  cuuint64_t gdim[3] = {cols, rows, depth};
+  cuuint64_t gstride[2] = {pitch_bytes, depth_pitch_bytes};
+  cuuint32_t box[3] = {box_cols, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, dtype, 3, const_cast<void*>(gptr), gdim, gstride, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled (3-D) failed with CUresult " + std::to_string(static_cast<int>(r)) +
+                   " (depth=" + std::to_string(depth) + " rows=" + std::to_string(rows) +
+                   " cols=" + std::to_string(cols) + " pitch=" + std::to_string(pitch_bytes) + ")");
+    return MHMR_ERR_CUDA;
+  }
+  return MHMR_OK;
+}
+
 bool PerDeviceOnce::first() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return true;

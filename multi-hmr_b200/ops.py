@@ -287,21 +287,23 @@ def fold_ln_linear(w, bias, ln_g, ln_b):
 
 
 def gemm_internal(a, w, epilogue, block_n, out=None, bias=None, gamma=None, hi=None, lo=None, stats=None, rowadd=None,
-                  rows_in=0):
-    """The GEMM a [M, K] @ w [N, K]^T with an internal epilogue (6 split residual update of (hi, lo) + stats, 7 / 8
-    folded-LN consumer from stats, 9 fp16 row add); stats fp32 [M, slots, 2]."""
+                  rows_in=0, rows_out=0, row_off=0, m_run=None):
+    """The GEMM a [M, K] @ w [N, K]^T with any epilogue kind: 0-5 as gemm_f16, 6 split residual update of (hi, lo) +
+    stats, 7 / 8 folded-LN consumer from stats, 9 fp16 row add; stats fp32 [M, slots, 2].  m_run < M runs a plan
+    built for M rows on its first m_run rows, as the engine does at a smaller batch."""
     _cuda(a, w, out, bias, gamma, hi, lo, stats, rowadd)
     _contig(stats, rowadd, bias, gamma)
     assert a.dtype == w.dtype == torch.float16 and a.stride(1) == 1 and w.stride(1) == 1
-    assert out is None or (out.dtype == torch.float16 and out.stride(1) == 1)
+    assert out is None or (out.dtype in (torch.float16, torch.float32) and out.stride(1) == 1)
     assert hi is None or (hi.dtype == lo.dtype == torch.float16 and hi.stride() == lo.stride() and hi.stride(1) == 1)
     M, K = a.shape
     N = w.shape[0]
     rc = _lib.load().mhmr_op_gemm_internal(
         ptr(a), c_int64(a.stride(0)), ptr(w), c_int64(w.stride(0)), c_int(M), c_int(N), c_int(K), c_int(epilogue),
         ptr(bias), ptr(gamma), ptr(hi), ptr(lo), c_int64(hi.stride(0) if hi is not None else 0), ptr(stats),
-        c_int(stats.shape[1] if stats is not None else 0), ptr(rowadd), c_int(rows_in), ptr(out),
-        c_int64(out.stride(0) if out is not None else 0), c_int(block_n), stream_ptr())
+        c_int(stats.shape[1] if stats is not None else 0), ptr(rowadd), c_int(rows_in), c_int(rows_out),
+        c_int(row_off), ptr(out), c_int64(out.stride(0) if out is not None else 0), c_int(block_n),
+        c_int(0 if m_run is None else m_run), stream_ptr())
     check(rc, "mhmr_op_gemm_internal")
     return out
 

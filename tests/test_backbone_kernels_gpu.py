@@ -10,27 +10,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-pytestmark = pytest.mark.gpu
+from fp64_util import SENTINEL, SENTINEL16, U, _acc_tol, _gelu_tol, _report, _ulp16
 
-U = 2.0 ** -24  # unit roundoff of fp32
-SENTINEL = 12345.0
-SENTINEL16 = -1234.0  # exact in fp16
+pytestmark = pytest.mark.gpu
 
 
 def _gen(seed):
     return torch.Generator(device="cpu").manual_seed(seed)
-
-
-def _report(name, err, tol):
-    r = (err / tol).max().item() if err.numel() else 0.0
-    print(f"  {name}: worst err/tol {r:.3f} (max err {err.max().item() if err.numel() else 0.0:.2e})")
-    return r
-
-
-def _ulp16(v):
-    """fp16 ulp of |v| (subnormal spacing 2^-24 below 2^-14)."""
-    e = torch.floor(torch.log2(v.abs().clamp_min(2.0 ** -14)))
-    return torch.exp2(e - 10)
 
 
 def _outliers(x, g, n=4, mag=150.0):
@@ -227,13 +213,6 @@ def test_fold_ln_linear(cuda_device, N, K):
 
 
 # ---------------------------------------------------------------------------------------------------- GEMM kinds 6-9
-def _acc_tol(a, w):
-    """fp32 tensor-core accumulation of exact fp16 products: one fp32 accumulation per 16-deep k step, each within
-    2 u of the running sum, plus the alignment inside a step: (K/4 + 16) u sum|a w| covers both with margin."""
-    K = a.shape[1]
-    return (K / 4 + 16) * U * (a.abs() @ w.abs().t())
-
-
 @pytest.mark.parametrize("bn,N,M", [(128, 384, 300), (512, 768, 300), (512, 1024, 77)])
 def test_gemm_split_residual_and_stats(cuda_device, bn, N, M):
     from multihmr_b200 import ops
@@ -291,11 +270,6 @@ def test_gemm_split_residual_and_stats(cuda_device, bn, N, M):
     # sensitivity: stats written to the other half's slot
     swapped = s_ref.reshape(M, slots // 2, 2).flip(2).reshape(M, slots)
     assert torch.any((gs[..., 0] - swapped).abs() > s_tol)
-
-
-def _gelu_tol(y):
-    # Abramowitz-Stegun erf (|error| <= 1.5e-7) and ~8 fp32 operations on the way
-    return 0.5 * y.abs() * (1.5e-7 + 8 * U) + 4 * U * y.abs()
 
 
 @pytest.mark.parametrize("gelu", [False, True])

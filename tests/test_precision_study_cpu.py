@@ -21,4 +21,6 @@ def test_fp8_study_reports_fp16_and_fp8_with_and_without_refinement():
     assert all(persons == 5 and same for persons, same, _ in res.values())
     v3d = {key: e["v3d"] for key, (_, _, e) in res.items()}
     assert v3d[("fp16", True)] < 1e-4 < v3d[("fp8 fc1+fc2", True)] < v3d[("fp8 fc1+fc2", False)]
-    assert 4.3e-3 < v3d[("fp8 fc1+fc2", True)] < 4.9e-3       # DESIGN.md §3 table: 4.6e-3
+    # DESIGN.md §3 table: 4.6e-3 with MKL's AVX-512 kernels.  Its SSE4.2 and AVX2 kernels sum the fp32 products in
+    # other orders, which flips some e4m3 roundings: 4.77e-3 and 4.91e-3.  The band holds all three with ~6% margin.
+    assert 4.3e-3 < v3d[("fp8 fc1+fc2", True)] < 5.2e-3

@@ -29,10 +29,22 @@ def test_restatement_reproduces_golden(name):
         gold = {k: g[k] for k in g.files}
     assert np.array_equal(out["index"], gold["index"])
     assert np.array_equal(out["depth"].astype(np.float32), gold["depth"])
+    d = np.abs(out["rgb"].astype(np.int16) - gold["rgb"])
+    assert d.max() <= 1 and (d == 0).mean() > 0.999
+    # The overlay truncates fg * blend + (1 - fg) * img to uint8, with fg the reference's fp32 3x3 conv.  Its last bit
+    # depends on the CPU kernel the conv runs (AVX-512 and AVX2 kernels round 2/9 + ... + 2/9 - 1 differently), so
+    # where fg > 0 and the exact value lies within 1e-3 of an integer the truncation may go either way: +-1 there.
+    # Every other value must be exact.
     overlay = gold["overlay_minus_photo"] + img.astype(np.int16)
-    for got, ref in ((out["rgb"], gold["rgb"]), (out["overlay"], overlay)):
-        d = np.abs(got.astype(np.int16) - ref)
-        assert d.max() <= 1 and (d == 0).mean() > 0.999
+    fgm = (gold["depth"] > 0).astype(np.float64)
+    H, W = fgm.shape
+    pad = np.pad(fgm, 1)
+    box = sum(pad[dy:dy + H, dx:dx + W] for dy in range(3) for dx in range(3))
+    fg = (np.maximum(2.0 * box / 9.0 - 1.0, 0.0) * fgm)[..., None]
+    val = fg * (alpha * gold["rgb"].astype(np.float64) + (1.0 - alpha) * img) + (1.0 - fg) * img
+    either = (fg > 0) & (np.abs(val - np.round(val)) < 1e-3)
+    d = np.abs(out["overlay"].astype(np.int16) - overlay)
+    assert d.max() <= 1 and np.all(d[~either] == 0)
     assert (gold["depth"] > 0).mean() > 0.05
 
 
