@@ -358,6 +358,16 @@ int mhmr_smplx_forward(mhmr_engine* h, int P, const float* rotvec, const float* 
                        const float* expression, const float* loc, const float* dist, const float* K_det,
                        float* v3d, float* v2d, float* j3d, float* j2d, float* transl, float* transl_pelvis,
                        void* stream);
+/* Backward of mhmr_smplx_forward for the same inputs: upstream gradients g_v3d [P,V,3], g_v2d [P,V,2], g_j3d /
+ * g_j2d [P,127,3 / 2], g_transl [P,3], g_transl_pelvis [P,3], each nullable (NULL = zero); input gradients
+ * d_rotvec [P,53,3], d_shape [P,nb], d_expression [P,10] (nullable: not computed), d_loc [P,2], d_dist [P] are
+ * written, not accumulated.  Stateless (recomputes the forward quantities it needs), no float atomics: repeated
+ * calls are bitwise identical and each person's gradients do not depend on the other persons.  Asynchronous. */
+int mhmr_smplx_backward(mhmr_engine* h, int P, const float* rotvec, const float* shape, const float* expression,
+                        const float* loc, const float* dist, const float* K_det, const float* g_v3d, const float* g_v2d,
+                        const float* g_j3d, const float* g_j2d, const float* g_transl, const float* g_transl_pelvis,
+                        float* d_rotvec, float* d_shape, float* d_expression, float* d_loc, float* d_dist,
+                        void* stream);
 /* ------------------------------------------------------------------------------------------------
  * Sharded batches (one process per GPU, image shards per rank; SURVEY.md §8e).  The reference is single-GPU
  * (README.md:107); these entry points are what a multi-GPU caller of `forward_model` binds.
@@ -442,6 +452,14 @@ int mhmr_body_info(const mhmr_body* h, int* num_verts, int* num_joints_out, int*
 int mhmr_body_forward(mhmr_body* h, int P, const float* full_pose, const float* betas, const float* expression,
                       const float* transl, const float* K, float* v3d, float* v2d, float* j3d, float* j2d,
                       float* transl_pelvis, void* stream);
+/* Backward of mhmr_body_forward for the same inputs: upstream gradients g_v3d [P,V,3], g_v2d [P,V,2], g_j3d / g_j2d
+ * [P,num_joints_out,3 / 2], g_transl_pelvis [P,3], each nullable (NULL = zero); input gradients d_full_pose [P,NJ,3],
+ * d_betas [P,num_betas], d_expression [P,10] (SMPL-X; nullable: not computed), d_transl [P,3] are written, not
+ * accumulated.  Stateless, no float atomics, batch-independent bits; asynchronous. */
+int mhmr_body_backward(mhmr_body* h, int P, const float* full_pose, const float* betas, const float* expression,
+                       const float* transl, const float* K, const float* g_v3d, const float* g_v2d, const float* g_j3d,
+                       const float* g_j2d, const float* g_transl_pelvis, float* d_full_pose, float* d_betas,
+                       float* d_expression, float* d_transl, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Mesh renderer: the overlay of reference utils/render.py:175 `render_meshes` (pyrender / OpenGL there), reached from

@@ -13,6 +13,7 @@ struct mhmr_body {
   int kind = 0, V = 0, nb = 0, ne = 0, NJ = 0, max_persons = 0;
   SmplxDeviceModel bm;
   SmplxScratch ws;
+  SmplxGradScratch gs;
   int* count = nullptr;
   std::vector<void*> allocs;
   ~mhmr_body() {
@@ -125,9 +126,14 @@ int body_build(mhmr_body* h, const float* v_template, const float* shapedirs, co
   TRY(h->alloc(&h->ws.xf, static_cast<size_t>(Pm) * 16));
   TRY(h->alloc(&h->ws.jposed, static_cast<size_t>(Pm) * NJ * 3));
   TRY(h->alloc(&h->count, 1));
-  // loading finishes before the staging buffers are freed and before the caller may free its arrays
-  MHMR_CUDA_CHECK(cudaStreamSynchronize(st));
-  return MHMR_OK;
+  // backward scratch and the vertex -> joint table (synchronises: loading finishes before the staging buffers are
+  // freed and before the caller may free its arrays)
+  return smplx_grad_init(bm, Pm, [h](void** p, size_t bytes) {
+    uint8_t* q = nullptr;
+    const int rc = h->alloc(&q, bytes);
+    *p = q;
+    return rc;
+  }, &h->gs, st);
 }
 
 }  // namespace
@@ -191,6 +197,21 @@ int mhmr_body_forward(mhmr_body* h, int P, const float* full_pose, const float* 
   MHMR_CUDA_CHECK(cudaMemcpyAsync(h->count, &P, sizeof(int), cudaMemcpyHostToDevice, st));
   return body_forward_raw(h->bm, full_pose, betas, expression, transl, K, h->count, P, h->ws, v3d, v2d, j3d, j2d,
                           transl_pelvis, st);
+}
+
+int mhmr_body_backward(mhmr_body* h, int P, const float* full_pose, const float* betas, const float* expression,
+                       const float* transl, const float* K, const float* g_v3d, const float* g_v2d, const float* g_j3d,
+                       const float* g_j2d, const float* g_transl_pelvis, float* d_full_pose, float* d_betas,
+                       float* d_expression, float* d_transl, void* stream) {
+  MHMR_REQUIRE(h != nullptr, "null body model");
+  MHMR_REQUIRE(P >= 0 && P <= h->max_persons, "P exceeds the handle's max_persons");
+  MHMR_REQUIRE(full_pose && betas && transl && K && d_full_pose && d_betas && d_transl, "null argument");
+  MHMR_REQUIRE(h->ne == 0 || expression != nullptr, "SMPL-X needs an expression array");
+  if (P == 0) return MHMR_OK;
+  BodyGrads g;
+  g.v3d = g_v3d; g.v2d = g_v2d; g.j3d = g_j3d; g.j2d = g_j2d; g.tp = g_transl_pelvis;
+  return body_backward_raw(h->bm, h->gs, P, full_pose, betas, expression, transl, K, g, d_full_pose, d_betas,
+                           h->ne ? d_expression : nullptr, d_transl, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

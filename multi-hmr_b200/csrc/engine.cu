@@ -120,6 +120,7 @@ struct mhmr_engine {
         *qkvp = nullptr, *att = nullptr, *qca = nullptr, *ffh = nullptr, *dec = nullptr, *K_det = nullptr;
   int* one = nullptr;  // device int == 1 (count for load-time skinny launches)
   SmplxScratch sx;
+  SmplxGradScratch sxg;
   GemmPlan patch_plan, cls0_plan, kv_plan;
   int* h_count = nullptr;  // pinned host copy of the person count
   int r_rows = 0;          // capacity of the refined rows (persons, plus one cls row per image for the Anny head)
@@ -484,7 +485,13 @@ int finalize_body(mhmr_engine* e, cudaStream_t st) {
   TRY(e->alloc(&e->sx.Amat, static_cast<size_t>(Pm) * 55 * 12));
   TRY(e->alloc(&e->sx.xf, static_cast<size_t>(Pm) * 16));
   TRY(e->alloc(&e->sx.jposed, static_cast<size_t>(Pm) * 55 * 3));
-  return MHMR_OK;
+  // backward scratch of mhmr_smplx_backward and its vertex -> joint table
+  return smplx_grad_init(bm, Pm, [e](void** p, size_t bytes) {
+    uint8_t* q = nullptr;
+    const int rc = e->alloc(&q, bytes);
+    *p = q;
+    return rc;
+  }, &e->sxg, st);
 }
 
 // Anny head (multi_hmr_anny/multi_hmr.py:41-95, encoder.py:16-31, hph.py): weights under the checkpoint's own keys.
@@ -1037,6 +1044,23 @@ int mhmr_smplx_forward(mhmr_engine* h, int P, const float* rotvec, const float* 
   TRY(loc_to_transl(loc, dist, K_det, P, transl, st));
   return smplx_forward(h->bm, rotvec, shape, expression, transl, K_det, h->count + 1, P, h->sx, v3d, v2d, j3d, j2d,
                        transl_pelvis, st);
+}
+
+int mhmr_smplx_backward(mhmr_engine* h, int P, const float* rotvec, const float* shape, const float* expression,
+                        const float* loc, const float* dist, const float* K_det, const float* g_v3d, const float* g_v2d,
+                        const float* g_j3d, const float* g_j2d, const float* g_transl, const float* g_transl_pelvis,
+                        float* d_rotvec, float* d_shape, float* d_expression, float* d_loc, float* d_dist,
+                        void* stream) {
+  MHMR_REQUIRE(h != nullptr, "null engine");
+  if (!h->finalized) { set_last_error("mhmr_smplx_backward before mhmr_finalize"); return MHMR_ERR_STATE; }
+  MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_SMPLX, "mhmr_smplx_backward needs an SMPL-X engine");
+  MHMR_REQUIRE(P >= 1 && P <= h->cfg.max_persons, "P exceeds max_persons");
+  MHMR_REQUIRE(rotvec && shape && expression && loc && dist && K_det && d_rotvec && d_shape && d_loc && d_dist,
+               "null argument");
+  BodyGrads g;
+  g.v3d = g_v3d; g.v2d = g_v2d; g.j3d = g_j3d; g.j2d = g_j2d; g.tp = g_transl_pelvis;
+  return smplx_backward(h->bm, h->sxg, P, rotvec, shape, expression, loc, dist, K_det, g, g_transl, d_rotvec, d_shape,
+                        d_expression, d_loc, d_dist, static_cast<cudaStream_t>(stream));
 }
 
 int mhmr_last_launch_count(mhmr_engine* h) { return h != nullptr ? h->launches : 0; }

@@ -1,5 +1,7 @@
 // Host-callable launchers of the non-GEMM kernels (one translation unit each).
 #pragma once
+#include <functional>
+
 #include "common.cuh"
 
 namespace mhmr {
@@ -149,5 +151,38 @@ int smplx_forward(const SmplxDeviceModel& bm, const float* rotvec, const float* 
 int body_forward_raw(const SmplxDeviceModel& bm, const float* full_pose, const float* betas, const float* expr,
                      const float* transl, const float* K, const int* count, int max_persons, SmplxScratch& ws,
                      float* v3d, float* v2d, float* j3d, float* j2d, float* transl_pelvis, cudaStream_t st);
+
+// Backward of the two layers (DESIGN.md §9).  Scratch sized by max_persons at create / finalize; each call
+// recomputes what it needs from the inputs, so it does not depend on an earlier forward or its scratch.
+struct SmplxGradScratch {
+  int max_persons = 0;
+  SmplxScratch fw;                  // recomputed prep (cf, A, placement, posed joints)
+  float* v3d = nullptr;             // [Pm, V, 3] recomputed vertices (only when a 2-D upstream gradient is given)
+  float *j3d = nullptr, *j2d = nullptr, *tp = nullptr;  // [Pm, J, 3], [Pm, J, 2], [Pm, 3]
+  float* transl = nullptr;          // [Pm, 3] placed layer: K^-1 [loc, 1] dist
+  float* gJ = nullptr;              // [Pm, J, 3] per-output-joint upstream gradient
+  float* part = nullptr;            // [tiles, Pm, NJ*12 + KT + 12] per-tile partial sums
+  size_t part_bytes = 0;
+  int* count = nullptr;
+  int *v2j_ptr = nullptr, *v2j_jt = nullptr;  // vertex -> output-joint table (CSR over vertices)
+  float* v2j_w = nullptr;
+};
+// Upstream gradients; each nullable (= zero).  v3d [P,V,3], v2d [P,V,2], j3d [P,J,3], j2d [P,J,2], tp [P,3].
+struct BodyGrads {
+  const float *v3d = nullptr, *v2d = nullptr, *j3d = nullptr, *j2d = nullptr, *tp = nullptr;
+};
+// Allocates through `alloc(&ptr, bytes)` (owned by the caller's handle) and uploads the vertex -> joint table built
+// from bm's extra_idx / lmk tables; synchronises `st`.
+int smplx_grad_init(const SmplxDeviceModel& bm, int max_persons, const std::function<int(void**, size_t)>& alloc,
+                    SmplxGradScratch* gs, cudaStream_t st);
+// Placed layer: d_rotvec [P,53,3], d_shape [P,num_betas], d_expr [P,10] (nullable), d_loc [P,2], d_dist [P].
+int smplx_backward(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* rotvec, const float* shape,
+                   const float* expr, const float* loc, const float* dist, const float* K_det, const BodyGrads& g,
+                   const float* g_transl, float* d_rotvec, float* d_shape, float* d_expr, float* d_loc, float* d_dist,
+                   cudaStream_t st);
+// Raw body model: d_full_pose [P,NJ,3], d_betas [P,num_betas], d_expr [P,10] (nullable), d_transl [P,3].
+int body_backward_raw(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* full_pose,
+                      const float* betas, const float* expr, const float* transl, const float* K, const BodyGrads& g,
+                      float* d_full_pose, float* d_betas, float* d_expr, float* d_transl, cudaStream_t st);
 
 }  // namespace mhmr

@@ -11,6 +11,9 @@
 //   * one CTA per SM (80 vertices = 240 columns per CTA for V = 10475 on the 132 SMs of an H100); the CTA's column slab
 //     is streamed through a TMA-fed shared-memory ring and 16 persons are accumulated per streamed row
 //     (the matrix is read from HBM once; further blocks of 16 persons re-stream it from L2).
+#include <utility>
+#include <vector>
+
 #include "kernels.cuh"
 
 namespace mhmr {
@@ -563,6 +566,627 @@ int body_forward_raw(const SmplxDeviceModel& bm, const float* full_pose, const f
   if (bm.num_joints == kNJ)
     return body_forward_impl<kNJ, kPoseFeat, 51, 16, true>(bm, full_pose, betas, expr, transl, K, count, max_persons, ws,
                                                        v3d, v2d, j3d, j2d, transl_pelvis, st);
+  set_last_error("body model: only SMPL (24 joints) and SMPL-X (55 joints) are instantiated");
+  return MHMR_ERR_UNSUPPORTED;
+}
+
+// ================================================================================================
+// Backward: input gradients of the two layers above (DESIGN.md §9).  Stateless: each call recomputes the per-person
+// prep with body_prep_kernel into its own scratch, plus the vertex / joint forward when a 2-D upstream gradient needs
+// the projected points.  No float atomics: every cross-CTA sum goes through per-tile partials that the person kernel
+// adds in tile order, so the bits do not depend on scheduling or on the other persons of the call.
+//   1. body_grad_joints_kernel   per person: gJ = g_j3d + proj^T g_j2d (+ g_transl_pelvis on joint 0)
+//   2. body_grad_stream_kernel   per 80-vertex tile, 16 persons per pass over the tile's PDX slab:
+//        g_o (vertex outputs, incl. the landmark / vertex-picked joints through the vertex->joint table),
+//        g_q = R_root^T g_o, T_i = sum_j w_ij A_j, g_vposed = T_i[:3,:3]^T g_q;
+//        streamed rows k: v_posed += cf_k PDX_k (forward contraction) and g_cf_k = PDX_k . g_vposed (reduction);
+//        then g_A_j = sum_i w_ij g_q_i [v_posed_i; 1]^T, sum_i g_o_i and sum_i g_o_i q_i^T as tile partials
+//   3. body_grad_person_kernel   per person: tile sums, placement, A -> G, kinematic chain in reverse, pose
+//        features, Rodrigues, J(beta) = Jt + Jdirs beta, loc / dist
+// ================================================================================================
+namespace {
+
+#define TRY_RC(...)                 \
+  do {                              \
+    int rc_ = (__VA_ARGS__);        \
+    if (rc_ != MHMR_OK) return rc_; \
+  } while (0)
+
+constexpr int kGTV = 80;            // vertices per CTA: 131 tiles for V = 10475 on 132 SMs
+constexpr int kGTC = kGTV * 3;       // 240 columns
+constexpr int kGThreads = 256;
+constexpr int kGPB = 16;             // persons per pass over the slab
+constexpr int kGRows = 16;           // PDX rows per staged chunk: (row, person) = 256 dot products per chunk
+constexpr int kGStages = 3;          // cp.async ring depth
+constexpr int kGvpPitch = kGTC + 1;  // odd pitch: the 16 persons of one row group read 16 distinct banks
+constexpr int kGChunkF4 = kGRows * kGTC / 4;  // 960 float4 per chunk
+
+template <int NJ>
+struct GradSmem {
+  float stage[kGStages][kGRows][kGTC];
+  float pfs[kKTMax][kGPB];
+  float Ws[kGTV][NJ];
+  float gvp[kGPB][kGvpPitch];
+  float go[kGPB][kGTC];
+  float vps[kGPB][kGTC];
+  float Ts[kGPB][kGTV][12];  // skinning transforms, then the outer products g_q [v_posed; 1]^T
+};
+
+__device__ __forceinline__ void cp_async16_zfill(void* smem, const void* gmem, bool pred) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "r"(pred ? 16 : 0)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// perspective_projection backward at the camera-space point o: out2 = K[:2] . (o / o_z) (o_z / o_z has derivative 0)
+__device__ __forceinline__ void proj_grad(const float* o, const float* Kd, float g0, float g1, float* go) {
+  const float iz = 1.f / o[2];
+  const float gu = Kd[0] * g0 + Kd[3] * g1, gw = Kd[1] * g0 + Kd[4] * g1;
+  go[0] += gu * iz;
+  go[1] += gw * iz;
+  go[2] -= (gu * o[0] + gw * o[1]) * iz * iz;
+}
+
+// d<g, R(r)>/dr for R = I + A(a) K(r) + B(a) K(r)^2, A = sin a / a, B = (1 - cos a) / a^2, a = ||r + eps||:
+// eps = 1e-8 is smplx.batch_rodrigues, eps = 0 with `roma` is roma.rotvec_to_rotmat (first-order below 1e-6 rad).
+// Below a = 0.5 A, B and their derivatives come from their Taylor series (truncation < 1e-9), which keeps the
+// a^3 / a^4 cancellations of the closed forms out of fp32 and makes r = 0 exact.
+__device__ void rotvec_grad(float rx, float ry, float rz, float eps, bool roma, const float* g, float* out) {
+  const float ge[3] = {g[7] - g[5], g[2] - g[6], g[3] - g[1]};  // <g, K(e_k)>
+  const float ex = rx + eps, ey = ry + eps, ez = rz + eps;
+  const float a = sqrtf(ex * ex + ey * ey + ez * ez);
+  if (roma && a < 1e-6f) {
+    out[0] = ge[0]; out[1] = ge[1]; out[2] = ge[2];
+    return;
+  }
+  const float a2 = a * a;
+  float A, B, Ap, Bp;
+  if (a < 0.5f) {
+    A = 1.f - a2 / 6.f * (1.f - a2 / 20.f * (1.f - a2 / 42.f * (1.f - a2 / 72.f)));
+    B = 0.5f * (1.f - a2 / 12.f * (1.f - a2 / 30.f * (1.f - a2 / 56.f * (1.f - a2 / 90.f))));
+    Ap = -a / 3.f * (1.f - a2 / 10.f * (1.f - a2 / 28.f * (1.f - a2 / 54.f)));
+    Bp = -a / 12.f * (1.f - a2 / 15.f * (1.f - a2 * (3.f / 112.f) * (1.f - a2 / 67.5f)));
+  } else {
+    const float s = sinf(a), c = cosf(a), h = sinf(0.5f * a);
+    const float omc = 2.f * h * h;
+    A = s / a;
+    B = omc / a2;
+    Ap = (a * c - s) / a2;
+    Bp = (a * s - 2.f * omc) / (a2 * a);
+  }
+  const float Kr[9] = {0.f, -rz, ry, rz, 0.f, -rx, -ry, rx, 0.f};
+  float gK = 0.f, gKK = 0.f;
+#pragma unroll
+  for (int m = 0; m < 3; ++m)
+#pragma unroll
+    for (int n = 0; n < 3; ++n) {
+      const float kk = Kr[m * 3] * Kr[n] + Kr[m * 3 + 1] * Kr[3 + n] + Kr[m * 3 + 2] * Kr[6 + n];
+      gK += g[m * 3 + n] * Kr[m * 3 + n];
+      gKK += g[m * 3 + n] * kk;
+    }
+  const float e[3] = {ex, ey, ez};
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    float E[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // K(e_k)
+    if (k == 0) { E[5] = -1.f; E[7] = 1.f; }
+    if (k == 1) { E[2] = 1.f; E[6] = -1.f; }
+    if (k == 2) { E[1] = -1.f; E[3] = 1.f; }
+    float gM = 0.f;  // <g, E K + K E>
+#pragma unroll
+    for (int m = 0; m < 3; ++m)
+#pragma unroll
+      for (int n = 0; n < 3; ++n) {
+        float v = 0.f;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) v += E[m * 3 + q] * Kr[q * 3 + n] + Kr[m * 3 + q] * E[q * 3 + n];
+        gM += g[m * 3 + n] * v;
+      }
+    const float dadr = a > 0.f ? e[k] / a : 0.f;
+    out[k] = dadr * (Ap * gK + Bp * gKK) + A * ge[k] + B * gM;
+  }
+}
+
+// 1. per-output-joint upstream gradient (camera space)
+__global__ void __launch_bounds__(128)
+body_grad_joints_kernel(const float* __restrict__ j3d, const float* __restrict__ K, const float* __restrict__ g_j3d,
+                        const float* __restrict__ g_j2d, const float* __restrict__ g_tp, int J, float* __restrict__ gJ) {
+  const int p = blockIdx.x, j = threadIdx.x;
+  if (j >= J) return;
+  const int64_t pj = static_cast<int64_t>(p) * J + j;
+  float g[3] = {0.f, 0.f, 0.f};
+  if (g_j3d != nullptr) { g[0] = g_j3d[pj * 3]; g[1] = g_j3d[pj * 3 + 1]; g[2] = g_j3d[pj * 3 + 2]; }
+  if (g_j2d != nullptr) proj_grad(j3d + pj * 3, K + p * 9, g_j2d[pj * 2], g_j2d[pj * 2 + 1], g);
+  if (j == 0 && g_tp != nullptr) { g[0] += g_tp[p * 3]; g[1] += g_tp[p * 3 + 1]; g[2] += g_tp[p * 3 + 2]; }
+  gJ[pj * 3] = g[0]; gJ[pj * 3 + 1] = g[1]; gJ[pj * 3 + 2] = g[2];
+}
+
+// 2. the streaming pass.  part[tile][p][PS]: [g_A (NJ x 12) | g_cf (KT) | sum g_o (3) | sum g_o q^T (9)]
+template <int NJ>
+__global__ void __launch_bounds__(kGThreads, 1)
+body_grad_stream_kernel(const float* __restrict__ PDX, int ldp, int KT, const float* __restrict__ vt,
+                        const float* __restrict__ W, const float* __restrict__ cf, const float* __restrict__ Amat,
+                        const float* __restrict__ xf, const float* __restrict__ K, const float* __restrict__ vout,
+                        const float* __restrict__ g_v3d, const float* __restrict__ g_v2d,
+                        const float* __restrict__ gJ, int J, const int* __restrict__ v2j_ptr,
+                        const int* __restrict__ v2j_jt, const float* __restrict__ v2j_w, int P, int V, int PS,
+                        float* __restrict__ part) {
+  extern __shared__ uint8_t gsm_raw[];
+  GradSmem<NJ>& sm = *reinterpret_cast<GradSmem<NJ>*>(gsm_raw + ((16u - (smem_u32(gsm_raw) & 15u)) & 15u));
+  const int tid = threadIdx.x, tile = blockIdx.x;
+  const int v0 = tile * kGTV, nv = min(kGTV, V - v0), col0 = v0 * 3, ncol = nv * 3;
+  const int n_chunks = (KT + kGRows - 1) / kGRows;
+  const int brow = tid >> 4, bj = tid & 15;  // (row, person) of the g_cf dot product
+
+  for (int i = tid; i < kGTV * NJ; i += kGThreads) {
+    const int v = i / NJ, jj = i - v * NJ;
+    sm.Ws[v][jj] = (v < nv) ? W[static_cast<int64_t>(v0 + v) * NJ + jj] : 0.f;
+  }
+  auto issue = [&](int ch) {
+    float* dst = &sm.stage[ch % kGStages][0][0];
+    for (int idx = tid; idx < kGChunkF4; idx += kGThreads) {
+      const int row = idx / (kGTC / 4), c4 = idx - row * (kGTC / 4);
+      const int k = ch * kGRows + row, col = col0 + c4 * 4;
+      const bool ok = k < KT && col < ldp;  // ldp is a multiple of 4: a float4 is wholly inside or outside
+      cp_async16_zfill(dst + row * kGTC + c4 * 4, ok ? PDX + static_cast<int64_t>(k) * ldp + col : PDX, ok);
+    }
+  };
+
+  for (int pb0 = 0; pb0 < P; pb0 += kGPB) {
+    const int np = min(kGPB, P - pb0);
+    __syncthreads();  // the previous pass is done with every buffer
+    // the first stages of the slab stream while the per-vertex work below runs
+    for (int ch = 0; ch < kGStages - 1; ++ch) {
+      if (ch < n_chunks) issue(ch);
+      cp_async_commit();
+    }
+    for (int i = tid; i < kKTMax * kGPB; i += kGThreads) {
+      const int k = i / kGPB, j = i - k * kGPB;
+      sm.pfs[k][j] = (j < np && k < KT) ? cf[static_cast<int64_t>(pb0 + j) * KT + k] : 0.f;
+    }
+    // ---- per (person, vertex): output gradient, skinning transform, g_vposed
+    for (int i = tid; i < kGPB * kGTV; i += kGThreads) {
+      const int j = i / kGTV, v = i - j * kGTV;
+      float go[3] = {0.f, 0.f, 0.f}, gv[3] = {0.f, 0.f, 0.f};
+      float T[12];
+#pragma unroll
+      for (int q = 0; q < 12; ++q) T[q] = 0.f;
+      if (j < np && v < nv) {
+        const int p = pb0 + j;
+        const int64_t pv = static_cast<int64_t>(p) * V + v0 + v;
+        if (g_v3d != nullptr) { go[0] = g_v3d[pv * 3]; go[1] = g_v3d[pv * 3 + 1]; go[2] = g_v3d[pv * 3 + 2]; }
+        if (g_v2d != nullptr) proj_grad(vout + pv * 3, K + p * 9, g_v2d[pv * 2], g_v2d[pv * 2 + 1], go);
+        for (int e = v2j_ptr[v0 + v]; e < v2j_ptr[v0 + v + 1]; ++e) {
+          const float w = v2j_w[e];
+          const float* gj = gJ + (static_cast<int64_t>(p) * J + v2j_jt[e]) * 3;
+          go[0] = fmaf(w, gj[0], go[0]); go[1] = fmaf(w, gj[1], go[1]); go[2] = fmaf(w, gj[2], go[2]);
+        }
+        const float4* A = reinterpret_cast<const float4*>(Amat + static_cast<int64_t>(p) * NJ * 12);
+#pragma unroll 4
+        for (int jj = 0; jj < NJ; ++jj) {
+          const float w = sm.Ws[v][jj];
+          const float4 a0 = __ldg(A + jj * 3), a1 = __ldg(A + jj * 3 + 1), a2 = __ldg(A + jj * 3 + 2);
+          T[0] = fmaf(w, a0.x, T[0]); T[1] = fmaf(w, a0.y, T[1]); T[2] = fmaf(w, a0.z, T[2]); T[3] = fmaf(w, a0.w, T[3]);
+          T[4] = fmaf(w, a1.x, T[4]); T[5] = fmaf(w, a1.y, T[5]); T[6] = fmaf(w, a1.z, T[6]); T[7] = fmaf(w, a1.w, T[7]);
+          T[8] = fmaf(w, a2.x, T[8]); T[9] = fmaf(w, a2.y, T[9]); T[10] = fmaf(w, a2.z, T[10]); T[11] = fmaf(w, a2.w, T[11]);
+        }
+        const float* X = xf + static_cast<int64_t>(p) * 16;
+        float gq[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) gq[c] = X[c] * go[0] + X[3 + c] * go[1] + X[6 + c] * go[2];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) gv[c] = T[c] * gq[0] + T[4 + c] * gq[1] + T[8 + c] * gq[2];
+      }
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        sm.go[j][v * 3 + c] = go[c];
+        sm.gvp[j][v * 3 + c] = gv[c];
+      }
+#pragma unroll
+      for (int q = 0; q < 12; ++q) sm.Ts[j][v][q] = T[q];
+    }
+
+    // ---- stream the slab: v_posed accumulation (column threads) and g_cf dot products ((row, person) threads)
+    float acc[kGPB];
+#pragma unroll
+    for (int j = 0; j < kGPB; ++j) acc[j] = 0.f;
+    for (int ch = 0; ch < n_chunks; ++ch) {
+      cp_async_wait<kGStages - 2>();
+      __syncthreads();  // chunk ch visible to all; everyone is done with the stage refilled next
+      if (ch + kGStages - 1 < n_chunks) issue(ch + kGStages - 1);
+      cp_async_commit();
+      const float(*stg)[kGTC] = sm.stage[ch % kGStages];
+      if (tid < kGTC) {
+#pragma unroll 4
+        for (int row = 0; row < kGRows; ++row) {
+          const float w = stg[row][tid];
+          const int k = ch * kGRows + row;
+#pragma unroll
+          for (int q = 0; q < kGPB / 4; ++q) {
+            const float4 cc = *reinterpret_cast<const float4*>(&sm.pfs[k][q * 4]);
+            acc[q * 4] = fmaf(cc.x, w, acc[q * 4]);
+            acc[q * 4 + 1] = fmaf(cc.y, w, acc[q * 4 + 1]);
+            acc[q * 4 + 2] = fmaf(cc.z, w, acc[q * 4 + 2]);
+            acc[q * 4 + 3] = fmaf(cc.w, w, acc[q * 4 + 3]);
+          }
+        }
+      }
+      {
+        const float* st = stg[brow];
+        const float* gv = sm.gvp[bj];
+        float s8[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) s8[u] = 0.f;
+#pragma unroll 2
+        for (int c = 0; c < kGTC; c += 8)
+#pragma unroll
+          for (int u = 0; u < 8; ++u) s8[u] = fmaf(st[c + u], gv[c + u], s8[u]);
+        const float s = ((s8[0] + s8[1]) + (s8[2] + s8[3])) + ((s8[4] + s8[5]) + (s8[6] + s8[7]));
+        const int k = ch * kGRows + brow;
+        if (bj < np && k < KT) part[(static_cast<int64_t>(tile) * P + pb0 + bj) * PS + NJ * 12 + k] = s;
+      }
+    }
+    cp_async_wait<0>();
+    if (tid < kGTC) {
+#pragma unroll
+      for (int j = 0; j < kGPB; ++j) sm.vps[j][tid] = (tid < ncol) ? vt[col0 + tid] + acc[j] : 0.f;
+    }
+    __syncthreads();
+    // ---- per (person, vertex): posed vertex q = T [v_posed; 1] and the outer product g_q [v_posed; 1]^T
+    for (int i = tid; i < kGPB * kGTV; i += kGThreads) {
+      const int j = i / kGTV, v = i - j * kGTV;
+      const float* T = sm.Ts[j][v];
+      const float vp[4] = {sm.vps[j][v * 3], sm.vps[j][v * 3 + 1], sm.vps[j][v * 3 + 2], 1.f};
+      float q[3], gq[3];
+      const float* X = xf + static_cast<int64_t>(pb0 + min(j, np - 1)) * 16;
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+        q[r] = T[r * 4] * vp[0] + T[r * 4 + 1] * vp[1] + T[r * 4 + 2] * vp[2] + T[r * 4 + 3];
+        gq[r] = X[r] * sm.go[j][v * 3] + X[3 + r] * sm.go[j][v * 3 + 1] + X[6 + r] * sm.go[j][v * 3 + 2];
+      }
+      float* M = sm.Ts[j][v];
+#pragma unroll
+      for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int s = 0; s < 4; ++s) M[r * 4 + s] = gq[r] * vp[s];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) sm.vps[j][v * 3 + r] = q[r];
+    }
+    __syncthreads();
+    // ---- tile partials, each summed over the tile's vertices in vertex order
+    const int nE = NJ * 12 + 12;
+    for (int i = tid; i < np * nE; i += kGThreads) {
+      const int j = i / nE, e = i - j * nE;
+      float s4[4] = {0.f, 0.f, 0.f, 0.f};
+      int dst;
+      if (e < NJ * 12) {
+        const int jj = e / 12, q = e - jj * 12;
+        for (int v = 0; v < nv; ++v) s4[v & 3] = fmaf(sm.Ws[v][jj], sm.Ts[j][v][q], s4[v & 3]);
+        dst = e;
+      } else {
+        const int e2 = e - NJ * 12;
+        if (e2 < 3) {
+          for (int v = 0; v < nv; ++v) s4[v & 3] += sm.go[j][v * 3 + e2];
+        } else {
+          const int r = (e2 - 3) / 3, c = (e2 - 3) - r * 3;
+          for (int v = 0; v < nv; ++v) s4[v & 3] = fmaf(sm.go[j][v * 3 + r], sm.vps[j][v * 3 + c], s4[v & 3]);
+        }
+        dst = NJ * 12 + KT + e2;
+      }
+      part[(static_cast<int64_t>(tile) * P + pb0 + j) * PS + dst] = (s4[0] + s4[1]) + (s4[2] + s4[3]);
+    }
+  }
+}
+
+// 3. per person: tile sums, placement, A -> G, kinematic chain in reverse, pose features, Rodrigues, J(beta).
+// kRaw: d_rot = d_full_pose [P, NJ, 3], d_transl written; else d_rot = d_rotvec [P, 53, 3], d_loc / d_dist written.
+template <int NJ, int PF, bool kRaw>
+__global__ void __launch_bounds__(256)
+body_grad_person_kernel(const float* __restrict__ rotvec, const float* __restrict__ shape,
+                        const float* __restrict__ expr, int n_expr, const float* __restrict__ Jt,
+                        const float* __restrict__ Jdirs, const int* __restrict__ parents, int num_betas,
+                        int center_idx, int KT, const float* __restrict__ Amat, const float* __restrict__ jposed,
+                        const float* __restrict__ xf, const float* __restrict__ gJ, int J,
+                        const float* __restrict__ part, int tiles, int P, int PS, const float* __restrict__ loc,
+                        const float* __restrict__ dist, const float* __restrict__ K,
+                        const float* __restrict__ g_transl, float* __restrict__ d_rot, float* __restrict__ d_shape,
+                        float* __restrict__ d_expr, float* __restrict__ d_transl, float* __restrict__ d_loc,
+                        float* __restrict__ d_dist) {
+  constexpr int kPSMax = NJ * 12 + kKTMax + 12;
+  __shared__ float red[kPSMax];
+  __shared__ float Rs[NJ][9], GR[NJ][9], Js[NJ][3];
+  __shared__ float gGR[NJ][9], gGt[NJ][3], gJl[NJ][3], gR[NJ][9];
+  __shared__ float beta[32], gcen[3];
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const int L = num_betas + n_expr;
+  for (int e = tid; e < PS; e += blockDim.x) {
+    float s = 0.f;
+    for (int t = 0; t < tiles; ++t) s += part[(static_cast<int64_t>(t) * P + p) * PS + e];
+    red[e] = s;
+  }
+  if (tid < num_betas) beta[tid] = shape[p * num_betas + tid];
+  if (tid >= 32 && tid < 32 + n_expr) beta[num_betas + (tid - 32)] = expr[p * n_expr + (tid - 32)];
+  __syncthreads();
+  float r3[3] = {0.f, 0.f, 0.f};
+  if (tid < NJ) {
+    const int j = tid;
+    const int src = kRaw ? j : full_pose_source(j);
+    if (src >= 0) {
+      const float* rv = rotvec + (static_cast<int64_t>(p) * (kRaw ? NJ : 53) + src) * 3;
+      r3[0] = rv[0]; r3[1] = rv[1]; r3[2] = rv[2];
+    }
+    // the forward's rotation (smplx.lbs.batch_rodrigues), its joints and the chain's rotations G_R = A[:, :3]
+    const float ex = r3[0] + 1e-8f, ey = r3[1] + 1e-8f, ez = r3[2] + 1e-8f;
+    const float ang = sqrtf(ex * ex + ey * ey + ez * ez);
+    const float ax = r3[0] / ang, ay = r3[1] / ang, az = r3[2] / ang;
+    const float s = sinf(ang), c1 = 1.f - cosf(ang);
+    const float Kx[9] = {0.f, -az, ay, az, 0.f, -ax, -ay, ax, 0.f};
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float kk = Kx[r * 3] * Kx[c] + Kx[r * 3 + 1] * Kx[3 + c] + Kx[r * 3 + 2] * Kx[6 + c];
+        Rs[j][r * 3 + c] = ((r == c) ? 1.f : 0.f) + s * Kx[r * 3 + c] + c1 * kk;
+        GR[j][r * 3 + c] = Amat[(static_cast<int64_t>(p) * NJ + j) * 12 + r * 4 + c];
+      }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      float v = Jt[j * 3 + r];
+      for (int l = 0; l < L; ++l) v += Jdirs[(j * 3 + r) * L + l] * beta[l];
+      Js[j][r] = v;
+    }
+  }
+  const float* gJp = gJ + static_cast<int64_t>(p) * J * 3;
+  const float* X = xf + static_cast<int64_t>(p) * 16;
+  const float* jp = jposed + static_cast<int64_t>(p) * NJ * 3;
+  if (tid == NJ) {
+    // placement: every output point o = R_root (x - J_centre) + transl (the pelvis cancels), x the posed LBS point
+    const float* Sv = red + NJ * 12 + KT;
+    float S[3] = {Sv[0], Sv[1], Sv[2]};
+    for (int j = 0; j < NJ; ++j) {
+      S[0] += gJp[j * 3]; S[1] += gJp[j * 3 + 1]; S[2] += gJp[j * 3 + 2];
+    }
+    if (kRaw) {
+      d_transl[p * 3] = S[0]; d_transl[p * 3 + 1] = S[1]; d_transl[p * 3 + 2] = S[2];
+    } else {
+      const float* Mo = Sv + 3;
+      const float* Jc = jp + center_idx * 3;
+      float gRr[9];
+#pragma unroll
+      for (int m = 0; m < 3; ++m)
+#pragma unroll
+        for (int n = 0; n < 3; ++n) gRr[m * 3 + n] = Mo[m * 3 + n] - Sv[m] * Jc[n];
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int m = 0; m < 3; ++m)
+#pragma unroll
+          for (int n = 0; n < 3; ++n) gRr[m * 3 + n] += gJp[j * 3 + m] * (jp[j * 3 + n] - Jc[n]);
+      const float* rv = rotvec + static_cast<int64_t>(p) * 53 * 3;
+      rotvec_grad(rv[0], rv[1], rv[2], 0.f, true, gRr, d_rot + static_cast<int64_t>(p) * 53 * 3);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) gcen[c] = -(X[c] * S[0] + X[3 + c] * S[1] + X[6 + c] * S[2]);
+      // transl = K^-1 [loc, 1] dist (the inverse as loc_to_transl computes it)
+      float gt[3] = {S[0], S[1], S[2]};
+      if (g_transl != nullptr) { gt[0] += g_transl[p * 3]; gt[1] += g_transl[p * 3 + 1]; gt[2] += g_transl[p * 3 + 2]; }
+      const float* m = K + p * 9;
+      const float a = m[0], bb = m[1], c = m[2], d = m[3], e = m[4], f = m[5], g = m[6], h = m[7], i = m[8];
+      const float Ac = e * i - f * h, Bc = -(d * i - f * g), Cc = d * h - e * g;
+      const float rr = 1.0f / (a * Ac + bb * Bc + c * Cc);
+      const float inv[9] = {Ac * rr, -(bb * i - c * h) * rr, (bb * f - c * e) * rr,
+                            Bc * rr, (a * i - c * g) * rr, -(a * f - c * d) * rr,
+                            Cc * rr, -(a * h - bb * g) * rr, (a * e - bb * d) * rr};
+      const float lx = loc[p * 2], ly = loc[p * 2 + 1], dd = dist[p];
+      float gd = 0.f;
+#pragma unroll
+      for (int q = 0; q < 3; ++q) gd += (inv[q * 3] * lx + inv[q * 3 + 1] * ly + inv[q * 3 + 2]) * gt[q];
+      d_dist[p] = gd;
+      d_loc[p * 2] = (inv[0] * gt[0] + inv[3] * gt[1] + inv[6] * gt[2]) * dd;
+      d_loc[p * 2 + 1] = (inv[1] * gt[0] + inv[4] * gt[1] + inv[7] * gt[2]) * dd;
+    }
+  }
+  __syncthreads();
+  if (tid < NJ) {
+    // A_j = [G_R | G_t - G_R J_j], posed joint = G_t
+    const int j = tid;
+    float gx[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) gx[c] = X[c] * gJp[j * 3] + X[3 + c] * gJp[j * 3 + 1] + X[6 + c] * gJp[j * 3 + 2];
+    if (!kRaw && j == center_idx) { gx[0] += gcen[0]; gx[1] += gcen[1]; gx[2] += gcen[2]; }
+    const float* gA = red + j * 12;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      gGt[j][r] = gx[r] + gA[r * 4 + 3];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) gGR[j][r * 3 + c] = gA[r * 4 + c] - gA[r * 4 + 3] * Js[j][c];
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      gJl[j][c] = -(GR[j][c] * gA[3] + GR[j][3 + c] * gA[7] + GR[j][6 + c] * gA[11]);
+  }
+  __syncthreads();
+  if (tid == 0) {
+    // kinematic chain in reverse: G_j = G_par [R_j | J_j - J_par]
+    for (int j = NJ - 1; j >= 1; --j) {
+      const int par = parents[j];
+      const float t[3] = {Js[j][0] - Js[par][0], Js[j][1] - Js[par][1], Js[j][2] - Js[par][2]};
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b)
+          gR[j][a * 3 + b] = GR[par][a] * gGR[j][b] + GR[par][3 + a] * gGR[j][3 + b] + GR[par][6 + a] * gGR[j][6 + b];
+#pragma unroll
+      for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+          gGR[par][r * 3 + c] += gGR[j][r * 3] * Rs[j][c * 3] + gGR[j][r * 3 + 1] * Rs[j][c * 3 + 1] +
+                                 gGR[j][r * 3 + 2] * Rs[j][c * 3 + 2] + gGt[j][r] * t[c];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float u = GR[par][c] * gGt[j][0] + GR[par][3 + c] * gGt[j][1] + GR[par][6 + c] * gGt[j][2];
+        gJl[j][c] += u;
+        gJl[par][c] -= u;
+        gGt[par][c] += gGt[j][c];
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 9; ++q) gR[0][q] = gGR[0][q];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) gJl[0][c] += gGt[0][c];
+  }
+  __syncthreads();
+  if (tid < NJ) {
+    const int j = tid;
+    if (j >= 1) {
+#pragma unroll
+      for (int q = 0; q < 9; ++q) gR[j][q] += red[NJ * 12 + (j - 1) * 9 + q];  // pose feature R_j - I
+    }
+    float gr[3];
+    rotvec_grad(r3[0], r3[1], r3[2], 1e-8f, false, gR[j], gr);
+    const int src = kRaw ? j : full_pose_source(j);
+    if (src >= 0) {
+      float* o = d_rot + (static_cast<int64_t>(p) * (kRaw ? NJ : 53) + src) * 3;
+      o[0] = gr[0]; o[1] = gr[1]; o[2] = gr[2];
+    }
+  }
+  if (tid >= 64 && tid < 64 + L) {
+    // beta enters the blend shapes (cf rows PF..) and the joints J = Jt + Jdirs beta
+    const int l = tid - 64;
+    float s = red[NJ * 12 + PF + l];
+    for (int q = 0; q < NJ * 3; ++q) s = fmaf(Jdirs[q * L + l], gJl[q / 3][q % 3], s);
+    if (l < num_betas) d_shape[p * num_betas + l] = s;
+    else if (d_expr != nullptr) d_expr[p * n_expr + (l - num_betas)] = s;
+  }
+}
+
+__global__ void set_count_kernel(int* count, int P) { *count = P; }
+
+template <int NJ, int PF, int NL, int PB, bool kRaw>
+int body_backward_impl(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* rotvec,
+                       const float* shape, const float* expr, const float* transl, const float* K,
+                       const BodyGrads& g, const float* loc, const float* dist, const float* g_transl, float* d_rot,
+                       float* d_shape, float* d_expr, float* d_transl, float* d_loc, float* d_dist, cudaStream_t st) {
+  const int KT = PF + bm.L, J = NJ + 21 + NL, V = bm.V;
+  MHMR_REQUIRE(KT <= kKTMax, "smplx: too many blend-shape coefficients");
+  MHMR_REQUIRE(bm.num_joints == NJ && bm.pose_feat == PF && bm.n_lmk == NL, "body model / kernel shape mismatch");
+  MHMR_REQUIRE(P <= gs.max_persons, "P exceeds the gradient scratch");
+  const int tiles = (V + kGTV - 1) / kGTV;
+  const int PS = NJ * 12 + KT + 12;
+  set_count_kernel<<<1, 1, 0, st>>>(gs.count, P);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  const bool need_fwd = g.v2d != nullptr || g.j2d != nullptr;  // projections need the forward's points
+  if (need_fwd) {
+    TRY_RC(body_forward_impl<NJ, PF, NL, PB, kRaw>(bm, rotvec, shape, expr, transl, K, gs.count, P, gs.fw, gs.v3d,
+                                                   nullptr, gs.j3d, gs.j2d, gs.tp, st));
+  } else {
+    body_prep_kernel<NJ, PF, kRaw><<<P, 64, 0, st>>>(rotvec, shape, expr, bm.L - bm.num_betas, bm.Jt, bm.Jdirs,
+                                                     bm.parents, gs.count, bm.num_betas, bm.center_idx, KT, gs.fw.cf,
+                                                     gs.fw.Amat, gs.fw.xf, gs.fw.jposed);
+    MHMR_CUDA_CHECK(cudaGetLastError());
+  }
+  body_grad_joints_kernel<<<P, 128, 0, st>>>(gs.j3d, K, g.j3d, g.j2d, g.tp, J, gs.gJ);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  static PerDeviceOnce once;
+  const int smem = static_cast<int>(sizeof(GradSmem<NJ>)) + 16;
+  if (once.first()) {
+    MHMR_CUDA_CHECK(cudaFuncSetAttribute(body_grad_stream_kernel<NJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  }
+  body_grad_stream_kernel<NJ><<<tiles, kGThreads, smem, st>>>(
+      bm.PDX, bm.ldp, KT, bm.vt, bm.lbs_weights_padded, gs.fw.cf, gs.fw.Amat, gs.fw.xf, K, gs.v3d, g.v3d, g.v2d, gs.gJ,
+      J, gs.v2j_ptr, gs.v2j_jt, gs.v2j_w, P, V, PS, gs.part);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  body_grad_person_kernel<NJ, PF, kRaw><<<P, 256, 0, st>>>(
+      rotvec, shape, expr, bm.L - bm.num_betas, bm.Jt, bm.Jdirs, bm.parents, bm.num_betas, bm.center_idx, KT,
+      gs.fw.Amat, gs.fw.jposed, gs.fw.xf, gs.gJ, J, gs.part, tiles, P, PS, loc, dist, K, g_transl, d_rot, d_shape,
+      d_expr, d_transl, d_loc, d_dist);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
+}
+
+}  // namespace
+
+int smplx_grad_init(const SmplxDeviceModel& bm, int max_persons, const std::function<int(void**, size_t)>& alloc,
+                    SmplxGradScratch* gs, cudaStream_t st) {
+  const int V = bm.V, NJ = bm.num_joints, KT = bm.pose_feat + bm.L, NL = bm.n_lmk, J = NJ + 21 + NL;
+  const int Pm = max_persons, tiles = (V + kGTV - 1) / kGTV;
+  // vertex -> output-joint table (vertex-picked joints, then the landmark corners), built on the host in joint order
+  MHMR_CUDA_CHECK(cudaStreamSynchronize(st));
+  std::vector<int32_t> ext(21), tri(3 * NL);
+  std::vector<float> bary(3 * NL);
+  MHMR_CUDA_CHECK(cudaMemcpy(ext.data(), bm.extra_idx, 21 * 4, cudaMemcpyDeviceToHost));
+  if (NL) {
+    MHMR_CUDA_CHECK(cudaMemcpy(tri.data(), bm.lmk_tri, 3 * NL * 4, cudaMemcpyDeviceToHost));
+    MHMR_CUDA_CHECK(cudaMemcpy(bary.data(), bm.lmk_bary, 3 * NL * 4, cudaMemcpyDeviceToHost));
+  }
+  std::vector<std::vector<std::pair<int, float>>> rows(V);
+  for (int e = 0; e < 21; ++e) rows[ext[e]].push_back({NJ + e, 1.f});
+  for (int l = 0; l < NL; ++l)
+    for (int f = 0; f < 3; ++f) rows[tri[l * 3 + f]].push_back({NJ + 21 + l, bary[l * 3 + f]});
+  std::vector<int32_t> rp(V + 1, 0), jt;
+  std::vector<float> w;
+  for (int v = 0; v < V; ++v) {
+    for (const auto& e : rows[v]) { jt.push_back(e.first); w.push_back(e.second); }
+    rp[v + 1] = static_cast<int32_t>(jt.size());
+  }
+  const size_t ne = jt.size();
+  auto f32 = [&](float** p, size_t n) {
+    void* q = nullptr;
+    const int rc = alloc(&q, n * sizeof(float));
+    *p = static_cast<float*>(q);
+    return rc;
+  };
+  auto i32 = [&](int** p, size_t n) {
+    void* q = nullptr;
+    const int rc = alloc(&q, n * sizeof(int));
+    *p = static_cast<int*>(q);
+    return rc;
+  };
+  gs->max_persons = Pm;
+  gs->part_bytes = static_cast<size_t>(tiles) * Pm * (NJ * 12 + KT + 12) * 4;
+  TRY_RC(f32(&gs->fw.cf, static_cast<size_t>(Pm) * KT));
+  TRY_RC(f32(&gs->fw.Amat, static_cast<size_t>(Pm) * NJ * 12));
+  TRY_RC(f32(&gs->fw.xf, static_cast<size_t>(Pm) * 16));
+  TRY_RC(f32(&gs->fw.jposed, static_cast<size_t>(Pm) * NJ * 3));
+  TRY_RC(f32(&gs->v3d, static_cast<size_t>(Pm) * V * 3));
+  TRY_RC(f32(&gs->j3d, static_cast<size_t>(Pm) * J * 3));
+  TRY_RC(f32(&gs->j2d, static_cast<size_t>(Pm) * J * 2));
+  TRY_RC(f32(&gs->tp, static_cast<size_t>(Pm) * 3));
+  TRY_RC(f32(&gs->transl, static_cast<size_t>(Pm) * 3));
+  TRY_RC(f32(&gs->gJ, static_cast<size_t>(Pm) * J * 3));
+  TRY_RC(f32(&gs->part, gs->part_bytes / 4));
+  TRY_RC(i32(&gs->count, 1));
+  TRY_RC(i32(&gs->v2j_ptr, V + 1));
+  TRY_RC(i32(&gs->v2j_jt, ne > 0 ? ne : 1));
+  TRY_RC(f32(&gs->v2j_w, ne > 0 ? ne : 1));
+  MHMR_CUDA_CHECK(cudaMemcpy(gs->v2j_ptr, rp.data(), (V + 1) * 4, cudaMemcpyHostToDevice));
+  if (ne) {
+    MHMR_CUDA_CHECK(cudaMemcpy(gs->v2j_jt, jt.data(), ne * 4, cudaMemcpyHostToDevice));
+    MHMR_CUDA_CHECK(cudaMemcpy(gs->v2j_w, w.data(), ne * 4, cudaMemcpyHostToDevice));
+  }
+  return MHMR_OK;
+}
+
+int smplx_backward(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* rotvec, const float* shape,
+                   const float* expr, const float* loc, const float* dist, const float* K_det, const BodyGrads& g,
+                   const float* g_transl, float* d_rotvec, float* d_shape, float* d_expr, float* d_loc, float* d_dist,
+                   cudaStream_t st) {
+  TRY_RC(loc_to_transl(loc, dist, K_det, P, gs.transl, st));
+  return body_backward_impl<kNJ, kPoseFeat, 51, 16, false>(bm, gs, P, rotvec, shape, expr, gs.transl, K_det, g, loc,
+                                                           dist, g_transl, d_rotvec, d_shape, d_expr, nullptr, d_loc,
+                                                           d_dist, st);
+}
+
+int body_backward_raw(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* full_pose,
+                      const float* betas, const float* expr, const float* transl, const float* K, const BodyGrads& g,
+                      float* d_full_pose, float* d_betas, float* d_expr, float* d_transl, cudaStream_t st) {
+  if (bm.num_joints == 24)
+    return body_backward_impl<24, 207, 0, 8, true>(bm, gs, P, full_pose, betas, expr, transl, K, g, nullptr, nullptr,
+                                                   nullptr, d_full_pose, d_betas, d_expr, d_transl, nullptr, nullptr,
+                                                   st);
+  if (bm.num_joints == kNJ)
+    return body_backward_impl<kNJ, kPoseFeat, 51, 16, true>(bm, gs, P, full_pose, betas, expr, transl, K, g, nullptr,
+                                                            nullptr, nullptr, d_full_pose, d_betas, d_expr, d_transl,
+                                                            nullptr, nullptr, st);
   set_last_error("body model: only SMPL (24 joints) and SMPL-X (55 joints) are instantiated");
   return MHMR_ERR_UNSUPPORTED;
 }

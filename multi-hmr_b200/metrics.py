@@ -193,12 +193,22 @@ class BodyModel:
     def __call__(self, full_pose, betas, transl, K, expression=None):
         """full_pose [P, num_pose_joints, 3] (smplx order), betas [P, num_betas], transl [P, 3], K [P, 3, 3],
         expression [P, 10] (SMPL-X; zeros when None).  Returns v3d [P,V,3], j3d [P,J,3], j2d [P,J,2],
-        transl_pelvis [P,3] on the device."""
-        dev = self.device
+        transl_pelvis [P,3] on the device.  Differentiable in full_pose, betas, transl and expression when grad mode
+        is on and one of them requires grad (`mhmr_body_backward`); gradients with respect to K are not provided."""
         P = int(betas.shape[0])
         if P > self.max_persons:
             raise ValueError(f"{P} persons > max_persons {self.max_persons}")
-        f = lambda t, n: t.to(dev, torch.float32).reshape(P, n).contiguous()
+        if torch.is_grad_enabled():
+            if isinstance(K, torch.Tensor) and K.requires_grad:
+                raise NotImplementedError("BodyModel: gradients with respect to K are not provided")
+            if any(isinstance(t, torch.Tensor) and t.requires_grad for t in (full_pose, betas, transl, expression)):
+                v3d, j3d, j2d, tp = _BodyFunction.apply(self, K, full_pose, betas, transl, expression)
+                return dict(v3d=v3d, j3d=j3d, j2d=j2d, transl_pelvis=tp)
+        return self._forward(*self._inputs(full_pose, betas, transl, K, expression))
+
+    def _inputs(self, full_pose, betas, transl, K, expression):
+        dev, P = self.device, int(betas.shape[0])
+        f = lambda t, n: t.detach().to(dev, torch.float32).reshape(P, n).contiguous()
         fp = f(full_pose, self.num_pose_joints * 3)
         b = f(betas, self.num_betas)
         tr = f(transl, 3)
@@ -206,6 +216,10 @@ class BodyModel:
         ex = None
         if self.kind == "smplx":
             ex = f(expression, 10) if expression is not None else torch.zeros(P, 10, device=dev)
+        return fp, b, tr, Kd, ex
+
+    def _forward(self, fp, b, tr, Kd, ex):
+        dev, P = self.device, int(b.shape[0])
         V, J = self.num_verts, self.num_joints
         out = dict(v3d=torch.empty(P, V, 3, device=dev), j3d=torch.empty(P, J, 3, device=dev),
                    j2d=torch.empty(P, J, 2, device=dev), transl_pelvis=torch.empty(P, 3, device=dev))
@@ -214,6 +228,50 @@ class BodyModel:
                                               ptr(out["v3d"]), None, ptr(out["j3d"]), ptr(out["j2d"]),
                                               ptr(out["transl_pelvis"]), _stream(dev)), "mhmr_body_forward")
         return out
+
+    def _backward(self, fp, b, tr, Kd, ex, g_v3d=None, g_v2d=None, g_j3d=None, g_j2d=None, g_transl_pelvis=None):
+        """`mhmr_body_backward` on converted inputs (see `_inputs`) and fp32 upstream gradients (each None = zero).
+        Returns d_full_pose [P, NJ*3], d_betas [P, num_betas], d_expression [P, 10] (SMPL-X, else None), d_transl."""
+        dev, P = self.device, int(b.shape[0])
+        g = lambda t: None if t is None else t.to(dev, torch.float32).contiguous()
+        d_fp, d_b, d_tr = torch.empty_like(fp), torch.empty_like(b), torch.empty_like(tr)
+        d_ex = torch.empty(P, 10, device=dev) if ex is not None else None
+        with torch.cuda.device(dev):
+            check(self._lib.mhmr_body_backward(self._h, c_int(P), ptr(fp), ptr(b), ptr(ex), ptr(tr), ptr(Kd),
+                                               ptr(g(g_v3d)), ptr(g(g_v2d)), ptr(g(g_j3d)), ptr(g(g_j2d)),
+                                               ptr(g(g_transl_pelvis)), ptr(d_fp), ptr(d_b), ptr(d_ex), ptr(d_tr),
+                                               _stream(dev)), "mhmr_body_backward")
+        return d_fp, d_b, d_ex, d_tr
+
+
+def _grad_like(d, t):
+    """A computed gradient in the shape, dtype and device of the input `t` it belongs to."""
+    return d.reshape(t.shape).to(device=t.device, dtype=t.dtype)
+
+
+class _BodyFunction(torch.autograd.Function):
+    """BodyModel.__call__ with gradients: forward = `mhmr_body_forward`, backward = `mhmr_body_backward`."""
+
+    @staticmethod
+    def forward(ctx, body, K, full_pose, betas, transl, expression):
+        ctx.set_materialize_grads(False)
+        x = body._inputs(full_pose, betas, transl, K, expression)
+        out = body._forward(*x)
+        ctx.body, ctx.x = body, x
+        ctx.orig = (full_pose, betas, transl, expression)
+        return out["v3d"], out["j3d"], out["j2d"], out["transl_pelvis"]
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_v3d, g_j3d, g_j2d, g_tp):
+        d_fp, d_b, d_ex, d_tr = ctx.body._backward(*ctx.x, g_v3d=g_v3d, g_j3d=g_j3d, g_j2d=g_j2d,
+                                                   g_transl_pelvis=g_tp)
+        full_pose, betas, transl, expression = ctx.orig
+        need = ctx.needs_input_grad
+        grads = [_grad_like(d_fp, full_pose) if need[2] else None, _grad_like(d_b, betas) if need[3] else None,
+                 _grad_like(d_tr, transl) if need[4] else None,
+                 _grad_like(d_ex, expression) if need[5] and expression is not None and d_ex is not None else None]
+        return (None, None, *grads)
 
 
 def _center_index(person_center) -> int:

@@ -405,12 +405,46 @@ class Model(_EngineModel):
         return z
 
     def smplx(self, rotvec, shape, loc, dist, K, expression, want_v2d=True):
-        """`SMPL_Layer.forward` (blocks/smpl_layer.py:47-155) for P persons."""
+        """`SMPL_Layer.forward` (blocks/smpl_layer.py:47-155) for P persons.  Differentiable in rotvec, shape, loc,
+        dist and expression when grad mode is on and one of them requires grad (`mhmr_smplx_backward`); gradients
+        with respect to K are not provided."""
+        self.finalize()
+        P = rotvec.shape[0]
+        assert list(rotvec.shape[1:]) == [53, 3] and P <= self.max_persons                       # :67
+        if torch.is_grad_enabled():
+            if isinstance(K, torch.Tensor) and K.requires_grad:
+                raise NotImplementedError("Model.smplx: gradients with respect to K are not provided")
+            if any(isinstance(t, torch.Tensor) and t.requires_grad for t in (rotvec, shape, loc, dist, expression)):
+                v3d, v2d, j3d, j2d, transl, tp = _SmplxFunction.apply(self, K, rotvec, shape, loc, dist, expression)
+                return {"v3d": v3d, "v2d": v2d if want_v2d else None, "j3d": j3d, "j2d": j2d, "transl": transl,
+                        "transl_pelvis": tp[:, None]}
+        return self._smplx_forward(*self._smplx_inputs(rotvec, shape, loc, dist, K, expression), want_v2d)
+
+    def _smplx_inputs(self, rotvec, shape, loc, dist, K, expression):
+        c = lambda a: a.detach().to(self.device, dtype=torch.float32).contiguous()
+        return tuple(map(c, (rotvec, shape, loc, dist, K, expression)))
+
+    def _smplx_backward(self, x, g_v3d=None, g_v2d=None, g_j3d=None, g_j2d=None, g_transl=None,
+                        g_transl_pelvis=None):
+        """`mhmr_smplx_backward` on converted inputs x = (rotvec, shape, loc, dist, K, expression) and fp32 upstream
+        gradients (each None = zero).  Returns d_rotvec [P,53,3], d_shape, d_loc [P,2], d_dist [P], d_expression."""
+        self.finalize()
+        rotvec, shape, loc, dist, K, expression = x
+        P, dev = rotvec.shape[0], self.device
+        g = lambda t: None if t is None else t.to(dev, torch.float32).contiguous()
+        d = [torch.empty_like(t) for t in (rotvec, shape, loc, dist, expression)]
+        with torch.cuda.device(dev):
+            stream = c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            check(self._lib.mhmr_smplx_backward(self._handle, c_int(P), ptr(rotvec), ptr(shape), ptr(expression),
+                                                ptr(loc), ptr(dist), ptr(K), ptr(g(g_v3d)), ptr(g(g_v2d)),
+                                                ptr(g(g_j3d)), ptr(g(g_j2d)), ptr(g(g_transl)),
+                                                ptr(g(g_transl_pelvis)), ptr(d[0]), ptr(d[1]), ptr(d[4]), ptr(d[2]),
+                                                ptr(d[3]), stream), "mhmr_smplx_backward")
+        return tuple(d)
+
+    def _smplx_forward(self, rotvec, shape, loc, dist, K, expression, want_v2d=True):
         self.finalize()
         P, dev, V = rotvec.shape[0], self.device, self.num_verts
-        assert list(rotvec.shape[1:]) == [53, 3] and P <= self.max_persons                       # :67
-        c = lambda a: a.to(dev, dtype=torch.float32).contiguous()
-        rotvec, shape, loc, dist, K, expression = map(c, (rotvec, shape, loc, dist, K, expression))
         f = lambda *s: torch.empty(*s, device=dev)
         out = {"v3d": f(P, V, 3), "v2d": f(P, V, 2) if want_v2d else None, "j3d": f(P, 127, 3), "j2d": f(P, 127, 2),
                "transl": f(P, 3), "transl_pelvis": f(P, 3)}
@@ -422,3 +456,24 @@ class Model(_EngineModel):
                                                ptr(out["transl_pelvis"]), stream), "mhmr_smplx_forward")
         out["transl_pelvis"] = out["transl_pelvis"][:, None]
         return out
+
+
+class _SmplxFunction(torch.autograd.Function):
+    """Model.smplx with gradients: forward = `mhmr_smplx_forward`, backward = `mhmr_smplx_backward`."""
+
+    @staticmethod
+    def forward(ctx, model, K, rotvec, shape, loc, dist, expression):
+        ctx.set_materialize_grads(False)
+        x = model._smplx_inputs(rotvec, shape, loc, dist, K, expression)
+        out = model._smplx_forward(*x, want_v2d=True)
+        ctx.model, ctx.x, ctx.orig = model, x, (rotvec, shape, loc, dist, expression)
+        return out["v3d"], out["v2d"], out["j3d"], out["j2d"], out["transl"], out["transl_pelvis"][:, 0]
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_v3d, g_v2d, g_j3d, g_j2d, g_transl, g_tp):
+        d_rot, d_shape, d_loc, d_dist, d_expr = ctx.model._smplx_backward(
+            ctx.x, g_v3d=g_v3d, g_v2d=g_v2d, g_j3d=g_j3d, g_j2d=g_j2d, g_transl=g_transl, g_transl_pelvis=g_tp)
+        need = ctx.needs_input_grad[2:]
+        like = lambda d, t, n: d.reshape(t.shape).to(device=t.device, dtype=t.dtype) if n else None
+        return (None, None, *(like(d, t, n) for d, t, n in zip((d_rot, d_shape, d_loc, d_dist, d_expr), ctx.orig, need)))
