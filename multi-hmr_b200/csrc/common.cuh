@@ -49,6 +49,13 @@ const char* get_last_error();
     }                                                                                  \
   } while (0)
 
+// Propagates a failed status (variadic: the expression may hold template commas).
+#define TRY(...)                    \
+  do {                              \
+    int rc_ = (__VA_ARGS__);        \
+    if (rc_ != MHMR_OK) return rc_; \
+  } while (0)
+
 // Encode a 2-D row-major tensor map: `rows` x `cols` elements of `elem_bytes`, row pitch
 // `pitch_bytes`; the box is box_rows x box_cols. `swizzle128` selects the 128-byte
 // swizzle (box_cols*elem_bytes must then be 128).

@@ -14,12 +14,6 @@ using namespace mhmr;
 
 namespace {
 
-#define TRY(expr)                       \
-  do {                                  \
-    int rc_ = (expr);                   \
-    if (rc_ != MHMR_OK) return rc_;     \
-  } while (0)
-
 struct DevBuf {
   void* p = nullptr;
   size_t bytes = 0;
@@ -100,7 +94,7 @@ struct mhmr_engine {
   float* Wdec = nullptr;      // [ndec, 1024]
   float* bdec = nullptr;      // [ndec]
   std::vector<HphLayer> hph;
-  SmplxDeviceModel bm;
+  DeviceBody body;   // the SMPL-X layer
 
   // workspaces
   __half *A16 = nullptr, *Xn16 = nullptr, *QKV16 = nullptr, *O16 = nullptr, *H16 = nullptr, *ctx16 = nullptr;
@@ -119,8 +113,6 @@ struct mhmr_engine {
   float *zc = nullptr, *query = nullptr, *vals = nullptr, *dKV = nullptr, *offh = nullptr, *xa = nullptr,
         *qkvp = nullptr, *att = nullptr, *qca = nullptr, *ffh = nullptr, *dec = nullptr, *K_det = nullptr;
   int* one = nullptr;  // device int == 1 (count for load-time skinny launches)
-  SmplxScratch sx;
-  SmplxGradScratch sxg;
   GemmPlan patch_plan, cls0_plan, kv_plan;
   int* h_count = nullptr;  // pinned host copy of the person count
   int r_rows = 0;          // capacity of the refined rows (persons, plus one cls row per image for the Anny head)
@@ -445,7 +437,7 @@ int finalize_head(mhmr_engine* e, cudaStream_t st) {
 }
 
 int finalize_body(mhmr_engine* e, cudaStream_t st) {
-  const int V = e->cfg.num_verts, nb = e->cfg.num_betas, L = nb + 10, Pm = e->cfg.max_persons;
+  const int V = e->cfg.num_verts, nb = e->cfg.num_betas;
   NEEDW(vt, "smplx.v_template", 3ll * V)
   NEEDW(sd, "smplx.shapedirs", 3ll * V * nb)
   NEEDW(ed, "smplx.expr_dirs", 30ll * V)
@@ -457,41 +449,9 @@ int finalize_body(mhmr_engine* e, cudaStream_t st) {
   const int* extra = e->tab("smplx.extra_joints_idxs", 21);
   const int* tri = e->tab("smplx.lmk_tri", 51 * 3);
   if (!parents || !extra || !tri) return MHMR_ERR_STATE;
-  SmplxDeviceModel& bm = e->bm;
-  bm.V = V; bm.L = L; bm.num_betas = nb; bm.center_idx = e->cfg.person_center_idx;
-  bm.ldp = (3 * V + 3) & ~3;
-  float *sfull = nullptr, *PDX = nullptr, *vtp = nullptr, *Jt = nullptr, *Jd = nullptr;
-  TRY(e->alloc(&sfull, static_cast<size_t>(3) * V * L));
-  TRY(repack_f32(sd, nb, 0, sfull, L, 0, 3 * V, nb, false, st));
-  TRY(repack_f32(ed, 10, 0, sfull, L, nb, 3 * V, 10, false, st));
-  TRY(e->alloc(&PDX, static_cast<size_t>(486 + L) * bm.ldp));
-  TRY(smplx_build_pdx(pd, sfull, 486, L, V, bm.ldp, PDX, st));
-  TRY(e->alloc(&vtp, bm.ldp));
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(vtp, vt, 3ll * V * 4, cudaMemcpyDeviceToDevice, st));
-  TRY(e->alloc(&Jt, 55 * 3));
-  TRY(smplx_fold_jreg(jr, vt, 55, V, 3, Jt, st));
-  TRY(e->alloc(&Jd, static_cast<size_t>(55) * 3 * L));
-  TRY(smplx_fold_jreg(jr, sfull, 55, V, 3 * L, Jd, st));
-  // skinning weights padded to whole 72-vertex tiles (the vertex kernel bulk-copies one tile per CTA)
-  const int tv = smplx_tile_verts();
-  const int Vpad = (V + tv - 1) / tv * tv;
-  float* lwp = nullptr;
-  TRY(e->alloc(&lwp, static_cast<size_t>(Vpad) * 55));
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(lwp, lw, 55ll * V * 4, cudaMemcpyDeviceToDevice, st));
-  bm.PDX = PDX; bm.vt = vtp; bm.lbs_weights_padded = lwp; bm.Jt = Jt; bm.Jdirs = Jd;
-  TRY(smplx_make_tmap(&bm));
-  bm.parents = parents; bm.extra_idx = extra; bm.lmk_tri = tri; bm.lmk_bary = bary;
-  TRY(e->alloc(&e->sx.cf, static_cast<size_t>(Pm) * (486 + L)));
-  TRY(e->alloc(&e->sx.Amat, static_cast<size_t>(Pm) * 55 * 12));
-  TRY(e->alloc(&e->sx.xf, static_cast<size_t>(Pm) * 16));
-  TRY(e->alloc(&e->sx.jposed, static_cast<size_t>(Pm) * 55 * 3));
-  // backward scratch of mhmr_smplx_backward and its vertex -> joint table
-  return smplx_grad_init(bm, Pm, [e](void** p, size_t bytes) {
-    uint8_t* q = nullptr;
-    const int rc = e->alloc(&q, bytes);
-    *p = q;
-    return rc;
-  }, &e->sxg, st);
+  // with the backward scratch of mhmr_smplx_backward
+  return body_build(&e->body, 55, V, nb, 10, e->cfg.person_center_idx, e->cfg.max_persons, vt, sd, ed, pd, jr, lw,
+                    parents, extra, tri, bary, st);
 }
 
 // Anny head (multi_hmr_anny/multi_hmr.py:41-95, encoder.py:16-31, hph.py): weights under the checkpoint's own keys.
@@ -757,8 +717,8 @@ int head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float d
                      e->K_det, st));
   {
     ProfScope ps_(e, MHMR_CAT_SMPLX, st);
-    TRY(smplx_forward(e->bm, o->rotvec, o->shape, o->expression, o->transl, e->K_det, count, Pm, e->sx, o->v3d,
-                      o->v2d, o->j3d, o->j2d, o->transl_pelvis, st));
+    TRY(smplx_forward(e->body.bm, o->rotvec, o->shape, o->expression, o->transl, e->K_det, count, Pm, e->body.ws,
+                      o->v3d, o->v2d, o->j3d, o->j2d, o->transl_pelvis, st));
   }
   e->launches += 3;
   return MHMR_OK;
@@ -1040,9 +1000,10 @@ int mhmr_smplx_forward(mhmr_engine* h, int P, const float* rotvec, const float* 
   MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_SMPLX, "mhmr_smplx_forward needs an SMPL-X engine");
   MHMR_REQUIRE(P >= 1 && P <= h->cfg.max_persons, "P exceeds max_persons");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->count + 1, &P, sizeof(int), cudaMemcpyHostToDevice, st));
+  DeviceBody& b = h->body;
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(b.count, &P, sizeof(int), cudaMemcpyHostToDevice, st));
   TRY(loc_to_transl(loc, dist, K_det, P, transl, st));
-  return smplx_forward(h->bm, rotvec, shape, expression, transl, K_det, h->count + 1, P, h->sx, v3d, v2d, j3d, j2d,
+  return smplx_forward(b.bm, rotvec, shape, expression, transl, K_det, b.count, P, b.ws, v3d, v2d, j3d, j2d,
                        transl_pelvis, st);
 }
 
@@ -1059,8 +1020,8 @@ int mhmr_smplx_backward(mhmr_engine* h, int P, const float* rotvec, const float*
                "null argument");
   BodyGrads g;
   g.v3d = g_v3d; g.v2d = g_v2d; g.j3d = g_j3d; g.j2d = g_j2d; g.tp = g_transl_pelvis;
-  return smplx_backward(h->bm, h->sxg, P, rotvec, shape, expression, loc, dist, K_det, g, g_transl, d_rotvec, d_shape,
-                        d_expression, d_loc, d_dist, static_cast<cudaStream_t>(stream));
+  return smplx_backward(h->body.bm, h->body.gs, P, rotvec, shape, expression, loc, dist, K_det, g, g_transl, d_rotvec,
+                        d_shape, d_expression, d_loc, d_dist, static_cast<cudaStream_t>(stream));
 }
 
 int mhmr_last_launch_count(mhmr_engine* h) { return h != nullptr ? h->launches : 0; }

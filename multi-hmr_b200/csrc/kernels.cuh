@@ -1,6 +1,6 @@
 // Host-callable launchers of the non-GEMM kernels (one translation unit each).
 #pragma once
-#include <functional>
+#include <vector>
 
 #include "common.cuh"
 
@@ -171,10 +171,6 @@ struct SmplxGradScratch {
 struct BodyGrads {
   const float *v3d = nullptr, *v2d = nullptr, *j3d = nullptr, *j2d = nullptr, *tp = nullptr;
 };
-// Allocates through `alloc(&ptr, bytes)` (owned by the caller's handle) and uploads the vertex -> joint table built
-// from bm's extra_idx / lmk tables; synchronises `st`.
-int smplx_grad_init(const SmplxDeviceModel& bm, int max_persons, const std::function<int(void**, size_t)>& alloc,
-                    SmplxGradScratch* gs, cudaStream_t st);
 // Placed layer: d_rotvec [P,53,3], d_shape [P,num_betas], d_expr [P,10] (nullable), d_loc [P,2], d_dist [P].
 int smplx_backward(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* rotvec, const float* shape,
                    const float* expr, const float* loc, const float* dist, const float* K_det, const BodyGrads& g,
@@ -184,5 +180,42 @@ int smplx_backward(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, cons
 int body_backward_raw(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* full_pose,
                       const float* betas, const float* expr, const float* transl, const float* K, const BodyGrads& g,
                       float* d_full_pose, float* d_betas, float* d_expr, float* d_transl, cudaStream_t st);
+
+// ---- body.cu: a body model on the device ----------------------------------------------------------
+// The folded tables, the forward and backward scratch and the person count of one SMPL / SMPL-X layer, in zero-filled
+// device allocations it owns and frees.
+struct DeviceBody {
+  SmplxDeviceModel bm;
+  SmplxScratch ws;
+  SmplxGradScratch gs;
+  int* count = nullptr;  // device person count of a forward
+  std::vector<void*> allocs;
+  DeviceBody() = default;
+  DeviceBody(const DeviceBody&) = delete;
+  DeviceBody& operator=(const DeviceBody&) = delete;
+  ~DeviceBody() {
+    for (void* p : allocs) cudaFree(p);
+  }
+  template <typename T>
+  int alloc(T** out, size_t n, cudaStream_t st) {
+    void* p = nullptr;
+    MHMR_CUDA_CHECK(cudaMalloc(&p, n * sizeof(T)));
+    allocs.push_back(p);
+    MHMR_CUDA_CHECK(cudaMemsetAsync(p, 0, n * sizeof(T), st));
+    *out = static_cast<T*>(p);
+    return MHMR_OK;
+  }
+};
+// Loads a body model of `joints` kinematic joints (24: SMPL; 55: SMPL-X with 51 face landmarks) and V vertices into
+// `b`, with scratch for max_persons.  The float arrays are device memory the folding kernels read; the integer tables
+// (parents, extra_idx [21], lmk_tri [51, 3]) are read with cudaMemcpyDefault and checked on the host before `b` keeps
+// device copies of them.  Synchronises `st`.
+int body_build(DeviceBody* b, int joints, int V, int num_betas, int num_expr, int center_idx, int max_persons,
+               const float* v_template, const float* shapedirs, const float* expr_dirs, const float* posedirs,
+               const float* J_regressor, const float* lbs_weights, const int32_t* parents, const int32_t* extra_idx,
+               const int32_t* lmk_tri, const float* lmk_bary, cudaStream_t st);
+// (smplx_lbs.cu) Allocates b->gs through b and uploads the vertex -> joint table built from b->bm's extra_idx / lmk
+// tables; synchronises `st`.
+int smplx_grad_init(DeviceBody* b, int max_persons, cudaStream_t st);
 
 }  // namespace mhmr

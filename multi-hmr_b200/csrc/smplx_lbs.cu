@@ -586,12 +586,6 @@ int body_forward_raw(const SmplxDeviceModel& bm, const float* full_pose, const f
 // ================================================================================================
 namespace {
 
-#define TRY_RC(...)                 \
-  do {                              \
-    int rc_ = (__VA_ARGS__);        \
-    if (rc_ != MHMR_OK) return rc_; \
-  } while (0)
-
 constexpr int kGTV = 80;            // vertices per CTA: 131 tiles for V = 10475 on 132 SMs
 constexpr int kGTC = kGTV * 3;       // 240 columns
 constexpr int kGThreads = 256;
@@ -1076,8 +1070,8 @@ int body_backward_impl(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, 
   MHMR_CUDA_CHECK(cudaGetLastError());
   const bool need_fwd = g.v2d != nullptr || g.j2d != nullptr;  // projections need the forward's points
   if (need_fwd) {
-    TRY_RC(body_forward_impl<NJ, PF, NL, PB, kRaw>(bm, rotvec, shape, expr, transl, K, gs.count, P, gs.fw, gs.v3d,
-                                                   nullptr, gs.j3d, gs.j2d, gs.tp, st));
+    TRY(body_forward_impl<NJ, PF, NL, PB, kRaw>(bm, rotvec, shape, expr, transl, K, gs.count, P, gs.fw, gs.v3d,
+                                                nullptr, gs.j3d, gs.j2d, gs.tp, st));
   } else {
     body_prep_kernel<NJ, PF, kRaw><<<P, 64, 0, st>>>(rotvec, shape, expr, bm.L - bm.num_betas, bm.Jt, bm.Jdirs,
                                                      bm.parents, gs.count, bm.num_betas, bm.center_idx, KT, gs.fw.cf,
@@ -1105,8 +1099,9 @@ int body_backward_impl(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, 
 
 }  // namespace
 
-int smplx_grad_init(const SmplxDeviceModel& bm, int max_persons, const std::function<int(void**, size_t)>& alloc,
-                    SmplxGradScratch* gs, cudaStream_t st) {
+int smplx_grad_init(DeviceBody* b, int max_persons, cudaStream_t st) {
+  const SmplxDeviceModel& bm = b->bm;
+  SmplxGradScratch* gs = &b->gs;
   const int V = bm.V, NJ = bm.num_joints, KT = bm.pose_feat + bm.L, NL = bm.n_lmk, J = NJ + 21 + NL;
   const int Pm = max_persons, tiles = (V + kGTV - 1) / kGTV;
   // vertex -> output-joint table (vertex-picked joints, then the landmark corners), built on the host in joint order
@@ -1129,40 +1124,30 @@ int smplx_grad_init(const SmplxDeviceModel& bm, int max_persons, const std::func
     rp[v + 1] = static_cast<int32_t>(jt.size());
   }
   const size_t ne = jt.size();
-  auto f32 = [&](float** p, size_t n) {
-    void* q = nullptr;
-    const int rc = alloc(&q, n * sizeof(float));
-    *p = static_cast<float*>(q);
-    return rc;
-  };
-  auto i32 = [&](int** p, size_t n) {
-    void* q = nullptr;
-    const int rc = alloc(&q, n * sizeof(int));
-    *p = static_cast<int*>(q);
-    return rc;
-  };
   gs->max_persons = Pm;
   gs->part_bytes = static_cast<size_t>(tiles) * Pm * (NJ * 12 + KT + 12) * 4;
-  TRY_RC(f32(&gs->fw.cf, static_cast<size_t>(Pm) * KT));
-  TRY_RC(f32(&gs->fw.Amat, static_cast<size_t>(Pm) * NJ * 12));
-  TRY_RC(f32(&gs->fw.xf, static_cast<size_t>(Pm) * 16));
-  TRY_RC(f32(&gs->fw.jposed, static_cast<size_t>(Pm) * NJ * 3));
-  TRY_RC(f32(&gs->v3d, static_cast<size_t>(Pm) * V * 3));
-  TRY_RC(f32(&gs->j3d, static_cast<size_t>(Pm) * J * 3));
-  TRY_RC(f32(&gs->j2d, static_cast<size_t>(Pm) * J * 2));
-  TRY_RC(f32(&gs->tp, static_cast<size_t>(Pm) * 3));
-  TRY_RC(f32(&gs->transl, static_cast<size_t>(Pm) * 3));
-  TRY_RC(f32(&gs->gJ, static_cast<size_t>(Pm) * J * 3));
-  TRY_RC(f32(&gs->part, gs->part_bytes / 4));
-  TRY_RC(i32(&gs->count, 1));
-  TRY_RC(i32(&gs->v2j_ptr, V + 1));
-  TRY_RC(i32(&gs->v2j_jt, ne > 0 ? ne : 1));
-  TRY_RC(f32(&gs->v2j_w, ne > 0 ? ne : 1));
-  MHMR_CUDA_CHECK(cudaMemcpy(gs->v2j_ptr, rp.data(), (V + 1) * 4, cudaMemcpyHostToDevice));
+  TRY(b->alloc(&gs->fw.cf, static_cast<size_t>(Pm) * KT, st));
+  TRY(b->alloc(&gs->fw.Amat, static_cast<size_t>(Pm) * NJ * 12, st));
+  TRY(b->alloc(&gs->fw.xf, static_cast<size_t>(Pm) * 16, st));
+  TRY(b->alloc(&gs->fw.jposed, static_cast<size_t>(Pm) * NJ * 3, st));
+  TRY(b->alloc(&gs->v3d, static_cast<size_t>(Pm) * V * 3, st));
+  TRY(b->alloc(&gs->j3d, static_cast<size_t>(Pm) * J * 3, st));
+  TRY(b->alloc(&gs->j2d, static_cast<size_t>(Pm) * J * 2, st));
+  TRY(b->alloc(&gs->tp, static_cast<size_t>(Pm) * 3, st));
+  TRY(b->alloc(&gs->transl, static_cast<size_t>(Pm) * 3, st));
+  TRY(b->alloc(&gs->gJ, static_cast<size_t>(Pm) * J * 3, st));
+  TRY(b->alloc(&gs->part, gs->part_bytes / 4, st));
+  TRY(b->alloc(&gs->count, 1, st));
+  TRY(b->alloc(&gs->v2j_ptr, V + 1, st));
+  TRY(b->alloc(&gs->v2j_jt, ne > 0 ? ne : 1, st));
+  TRY(b->alloc(&gs->v2j_w, ne > 0 ? ne : 1, st));
+  // on `st`, after the zero-fills; the host tables live until the synchronisation
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(gs->v2j_ptr, rp.data(), (V + 1) * 4, cudaMemcpyHostToDevice, st));
   if (ne) {
-    MHMR_CUDA_CHECK(cudaMemcpy(gs->v2j_jt, jt.data(), ne * 4, cudaMemcpyHostToDevice));
-    MHMR_CUDA_CHECK(cudaMemcpy(gs->v2j_w, w.data(), ne * 4, cudaMemcpyHostToDevice));
+    MHMR_CUDA_CHECK(cudaMemcpyAsync(gs->v2j_jt, jt.data(), ne * 4, cudaMemcpyHostToDevice, st));
+    MHMR_CUDA_CHECK(cudaMemcpyAsync(gs->v2j_w, w.data(), ne * 4, cudaMemcpyHostToDevice, st));
   }
+  MHMR_CUDA_CHECK(cudaStreamSynchronize(st));
   return MHMR_OK;
 }
 
@@ -1170,7 +1155,7 @@ int smplx_backward(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, cons
                    const float* expr, const float* loc, const float* dist, const float* K_det, const BodyGrads& g,
                    const float* g_transl, float* d_rotvec, float* d_shape, float* d_expr, float* d_loc, float* d_dist,
                    cudaStream_t st) {
-  TRY_RC(loc_to_transl(loc, dist, K_det, P, gs.transl, st));
+  TRY(loc_to_transl(loc, dist, K_det, P, gs.transl, st));
   return body_backward_impl<kNJ, kPoseFeat, 51, 16, false>(bm, gs, P, rotvec, shape, expr, gs.transl, K_det, g, loc,
                                                            dist, g_transl, d_rotvec, d_shape, d_expr, nullptr, d_loc,
                                                            d_dist, st);

@@ -18,6 +18,7 @@ import torch
 
 from . import _lib
 from ._lib import c_int, c_void_p, check, ptr
+from .model import BODY_TABLES, body_model_arrays
 
 # train.py:402-403 (SPIN's constants.py): the 14 LSP joints of the 17 H36M joints
 H36M_TO_J17 = [6, 5, 4, 1, 2, 3, 16, 15, 14, 11, 12, 13, 8, 10, 0, 7, 9]
@@ -156,26 +157,17 @@ class BodyModel:
         dev = torch.device(device)
         self.kind, self.device, self.max_persons = kind, dev, int(max_persons)
         nb = int(num_betas if num_betas is not None else (11 if kind == "smplx" else 10))
-        sd = bm["shapedirs"]
-        if sd.shape[-1] < nb:  # the 11th (kid) component of the neutral_11 layer
-            sd = torch.cat([sd, bm["shapedirs_extra"][..., : nb - sd.shape[-1]]], dim=-1)
-        f32 = lambda t: torch.as_tensor(t).to(dev, torch.float32).contiguous()
-        i32 = lambda t: torch.as_tensor(t).to(dev, torch.int32).contiguous()
-        V = int(bm["v_template"].shape[0])
+        arrays = {k: torch.as_tensor(v).to(dev, torch.int32 if k in BODY_TABLES else torch.float32).contiguous()
+                  for k, v in body_model_arrays(bm, nb, landmarks=kind == "smplx").items()}
+        V = int(arrays["v_template"].shape[0])
         self.num_verts, self.num_betas = V, nb
-        arrays = dict(vt=f32(bm["v_template"]), sd=f32(sd[..., :nb]), pd=f32(bm["posedirs"]),
-                      jr=f32(bm["J_regressor"]), lw=f32(bm["lbs_weights"]), par=i32(bm["parents"]),
-                      ext=i32(bm["extra_joints_idxs"]))
-        if kind == "smplx":
-            faces = torch.as_tensor(bm["faces"]).long()
-            arrays.update(ed=f32(bm["expr_dirs"]), tri=i32(faces[torch.as_tensor(bm["lmk_faces_idx"]).long()]),
-                          bary=f32(bm["lmk_bary_coords"]))
-        a = lambda k: ptr(arrays.get(k))
+        a = lambda *ks: [ptr(arrays.get(k)) for k in ks]
         h = c_void_p()
         with torch.cuda.device(dev):
             check(lib.mhmr_body_create(c_int(1 if kind == "smplx" else 0), c_int(V), c_int(nb), c_int(self.max_persons),
-                                       a("vt"), a("sd"), a("ed"), a("pd"), a("jr"), a("lw"), a("par"), a("ext"),
-                                       a("tri"), a("bary"), _stream(dev), ctypes.byref(h)), "mhmr_body_create")
+                                       *a("v_template", "shapedirs", "expr_dirs", "posedirs", "J_regressor",
+                                          "lbs_weights", "parents", "extra_joints_idxs", "lmk_tri", "lmk_bary_coords"),
+                                       _stream(dev), ctypes.byref(h)), "mhmr_body_create")
         self._h = h
         self._lib = lib
         nj_out, nj = ctypes.c_int(), ctypes.c_int()

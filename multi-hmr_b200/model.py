@@ -39,6 +39,25 @@ assert len(KINEMATIC_JOINTS) == 55
 # the 72 non-kinematic names of JOINT_NAMES[:127] (vertex-picked joints and face landmarks): valid in the
 # reference (utils/humans.py:25-26), not supported as a person centre here
 DEFAULT_PERSONS_PER_IMAGE = 16
+# the integer tables among body_model_arrays' entries; the others are fp32
+BODY_TABLES = ("parents", "extra_joints_idxs", "lmk_tri")
+
+
+def body_model_arrays(bm: dict, num_betas: int, landmarks: bool = True) -> dict:
+    """The arrays a body-model loader takes (the engine's `smplx.*` weights and tables, `mhmr_body_create`) from a
+    body-model dict (`synth.make_body_model`, `api.body_model_from_smplx_npz`, ...): shapedirs with `num_betas`
+    columns, the 11th (kid) component taken from `shapedirs_extra`; with `landmarks` (SMPL-X) also the expression
+    directions and the landmark triangles faces[lmk_faces_idx] with their barycentric coordinates."""
+    sd = torch.as_tensor(bm["shapedirs"])
+    if sd.shape[-1] < num_betas:
+        sd = torch.cat([sd, torch.as_tensor(bm["shapedirs_extra"])[..., : num_betas - sd.shape[-1]]], dim=-1)
+    out = {k: bm[k] for k in ("v_template", "posedirs", "J_regressor", "lbs_weights", "parents", "extra_joints_idxs")}
+    out["shapedirs"] = sd[..., :num_betas]
+    if landmarks:
+        faces = torch.as_tensor(bm["faces"]).long()
+        out.update(expr_dirs=bm["expr_dirs"], lmk_tri=faces[torch.as_tensor(bm["lmk_faces_idx"]).long()],
+                   lmk_bary_coords=bm["lmk_bary_coords"])
+    return out
 
 
 class _Config(ctypes.Structure):
@@ -303,21 +322,8 @@ class Model(_EngineModel):
 
     def _upload_extras(self):
         self._set_weight("camera.freq_bands", torch.linspace(1.0, 32.0, 16))       # blocks/camera_embed.py:46
-        bm = self._bm
-        nb = self.num_betas
-        sdirs = bm["shapedirs"]
-        if sdirs.shape[-1] < nb:
-            sdirs = torch.cat([sdirs, bm["shapedirs_extra"][..., : nb - sdirs.shape[-1]]], dim=-1)
-        self._set_weight("smplx.v_template", bm["v_template"])
-        self._set_weight("smplx.shapedirs", sdirs[..., :nb])
-        self._set_weight("smplx.expr_dirs", bm["expr_dirs"])
-        self._set_weight("smplx.posedirs", bm["posedirs"])
-        self._set_weight("smplx.J_regressor", bm["J_regressor"])
-        self._set_weight("smplx.lbs_weights", bm["lbs_weights"])
-        self._set_weight("smplx.lmk_bary_coords", bm["lmk_bary_coords"])
-        self._set_table("smplx.parents", bm["parents"])
-        self._set_table("smplx.extra_joints_idxs", bm["extra_joints_idxs"])
-        self._set_table("smplx.lmk_tri", bm["faces"][bm["lmk_faces_idx"]])
+        for k, v in body_model_arrays(self._bm, self.num_betas).items():
+            (self._set_table if k in BODY_TABLES else self._set_weight)("smplx." + k, v)
 
     # ------------------------------------------------------------------ forward
     def _alloc_outputs(self, B, want_v2d, want_z):
