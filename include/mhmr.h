@@ -498,6 +498,51 @@ int mhmr_render_info(const mhmr_render* h, int* num_faces, int* num_verts, int* 
  * (growing frees the old buffer, which waits for the device).  One call at a time per handle. */
 int mhmr_render_forward(mhmr_render* h, const mhmr_render_args* a, void* stream);
 
+/* Several topologies in one z-buffer.  A handle made by mhmr_render_create_topologies holds, besides the body mesh,
+ * `num_topologies` extra face arrays (topology t: topo_num_faces[t] faces over topo_num_verts[t] vertices, its faces
+ * in `topo_faces` after those of topologies 0..t-1, indices local to the topology), each with its own normal CSR.
+ * The depth key's low word holds (mesh, face); face_bits is sized for the largest topology.  With num_topologies 0
+ * this is mhmr_render_create. */
+int mhmr_render_create_topologies(const int32_t* faces, int num_faces, int num_verts, int num_topologies,
+                                  const int32_t* topo_faces, const int32_t* topo_num_faces,
+                                  const int32_t* topo_num_verts, void* stream, mhmr_render** out);
+#define MHMR_RENDER_MAX_PROPS 16
+typedef struct mhmr_render_extra {
+  int num_props;                /* extra meshes ("props") drawn next to the persons, <= MHMR_RENDER_MAX_PROPS     */
+  const int32_t* prop_topology; /* HOST [num_props]: topology of each prop                                        */
+  const float* prop_verts;      /* [sum of the props' vertex counts, 3] back to back, world coordinates            */
+  const float* prop_colors;     /* [num_props, 3] base colours in [0, 1]                                          */
+  const uint8_t* prop_visible;  /* [views, num_props]: nonzero draws prop j into view b; NULL = everywhere         */
+  const float* view_alpha;      /* [views] blend alpha of each view; NULL = args->alpha                           */
+  const int32_t* view_background; /* [views] background image of each view; NULL = args->view_image             */
+} mhmr_render_extra;
+/* mhmr_render_forward plus props, per-view alpha and backgrounds.  Mesh m of the key is person m for m <
+ * max_persons and prop m - max_persons after; max_persons + num_props must fit the key next to the face index.  The
+ * person map (args->person) holds that mesh index. */
+int mhmr_render_forward_extra(mhmr_render* h, const mhmr_render_args* a, const mhmr_render_extra* e, void* stream);
+
+/* Camera poses of the demo's views, on the device (demo.py:160-241 create_rotating_video, utils/render.py:407
+ * render_side_views), one CTA per image.  Per image, the views are: the photo's own camera (identity); if n_frames
+ * >= 2, the orbit frames i = 0..n_frames-1 of the sweeps y by +angle_range, y by -angle_range and x by
+ * +angle_range degrees about the centroid of the image's first person ([R | c - R c]); if side, lookAt poses of the
+ * displaced, side and bird's-eye views.  The first person is the first listed (person_image order) or, with `transl`,
+ * the smallest transl z (ties to the first).  Arithmetic in fp64, rounded once to fp32. */
+typedef struct mhmr_render_pose_args {
+  int images, max_persons, num_verts;
+  const int32_t* count;         /* [1] persons, read on the device                                                */
+  const int32_t* person_image;  /* [max_persons]                                                                  */
+  const float* verts;           /* [max_persons, num_verts, 3]                                                    */
+  const float* transl_pelvis;   /* [max_persons, 3]: the side views look at the median pelvis z                   */
+  const float* transl;          /* [max_persons, 3] or NULL: closest first by transl z (Anny's order)             */
+  int n_frames;                 /* 0 (no orbit) or >= 2                                                           */
+  double angle_range;           /* degrees                                                                        */
+  int side;
+  float* pose;                  /* out [images, views per image, 3, 4]                                            */
+  uint8_t* nonempty;            /* out [images]: 1 when the image has a person                                    */
+  int32_t* rank;                /* out [max_persons]: position of the person in its image's list, -1 past count   */
+} mhmr_render_pose_args;
+int mhmr_render_view_poses(const mhmr_render_pose_args* a, void* stream);
+
 /* Kernel launches enqueued by the last mhmr_forward (bench.py's `gpu_launches`). */
 int mhmr_last_launch_count(mhmr_engine* h);
 

@@ -58,13 +58,36 @@ class RenderArgs(ctypes.Structure):
                 ("overlay", c_void_p), ("depth", c_void_p), ("person", c_void_p)]
 
 
+class RenderExtra(ctypes.Structure):
+    """`mhmr_render_extra` of include/mhmr.h."""
+
+    _fields_ = [("num_props", c_int), ("prop_topology", c_void_p), ("prop_verts", c_void_p),
+                ("prop_colors", c_void_p), ("prop_visible", c_void_p), ("view_alpha", c_void_p),
+                ("view_background", c_void_p)]
+
+
+class RenderPoseArgs(ctypes.Structure):
+    """`mhmr_render_pose_args` of include/mhmr.h."""
+
+    _fields_ = [("images", c_int), ("max_persons", c_int), ("num_verts", c_int), ("count", c_void_p),
+                ("person_image", c_void_p), ("verts", c_void_p), ("transl_pelvis", c_void_p), ("transl", c_void_p),
+                ("n_frames", c_int), ("angle_range", ctypes.c_double), ("side", c_int), ("pose", c_void_p),
+                ("nonempty", c_void_p), ("rank", c_void_p)]
+
+
 def _declare_render(lib) -> None:
     P = ctypes.POINTER
     lib.mhmr_render_create.argtypes = [c_void_p, c_int, c_int, c_void_p, P(c_void_p)]
+    lib.mhmr_render_create_topologies.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                                  c_void_p, P(c_void_p)]
     lib.mhmr_render_destroy.argtypes = [c_void_p]
     lib.mhmr_render_info.argtypes = [c_void_p, P(c_int), P(c_int), P(c_int)]
     lib.mhmr_render_forward.argtypes = [c_void_p, P(RenderArgs), c_void_p]
-    for f in (lib.mhmr_render_create, lib.mhmr_render_destroy, lib.mhmr_render_info, lib.mhmr_render_forward):
+    lib.mhmr_render_forward_extra.argtypes = [c_void_p, P(RenderArgs), P(RenderExtra), c_void_p]
+    lib.mhmr_render_view_poses.argtypes = [P(RenderPoseArgs), c_void_p]
+    for f in (lib.mhmr_render_create, lib.mhmr_render_create_topologies, lib.mhmr_render_destroy,
+              lib.mhmr_render_info, lib.mhmr_render_forward, lib.mhmr_render_forward_extra,
+              lib.mhmr_render_view_poses):
         f.restype = c_int
 
 

@@ -266,6 +266,33 @@ def overlay_human_meshes(humans, faces, K, model, img_pil, unique_color=False, a
     return arr, _color
 
 
+def create_rotating_video(humans, faces, K, model, img_pil_visu, unique_color=False, alpha=0.8, fn=None, n_frames=20,
+                          angle_range=60):
+    """demo.py:188-241: the frames of the rotating video of one image's persons, as a list of uint8 [H,W,3] arrays
+    (None without persons): the overlay on the photo, then orbits about the first person's centroid (y by
+    +angle_range, y by -angle_range, x by +angle_range) over white, each sweep forth and back, the overlay between.
+    All distinct frames come from one render call on the device.  Writing the video is the caller's: `fn` must
+    be None."""
+    from .render import PALETTE, _humans_dict, _person_colors, renderer_for
+
+    if fn is not None:
+        raise NotImplementedError("create_rotating_video returns the frames; encode them to a video file yourself")
+    if len(humans) == 0:
+        return None
+    _color = [PALETTE[0] for _ in range(len(humans))] if unique_color else list(PALETTE)
+    photo = np.asarray(img_pil_visu)
+    if photo.dtype != np.uint8:
+        raise ValueError("img_pil_visu must be an 8-bit RGB image")
+    dev = torch.device("cuda")
+    t = _humans_dict(humans, dev, "verts_smplx" if "verts_smplx" in humans[0] else "v3d")  # demo.py:195
+    r = renderer_for(faces, t["v3d"].shape[1], dev)
+    cols = torch.tensor(np.asarray(_person_colors(_color, len(humans)), np.float64)[:, :3], dtype=torch.float32)
+    out = r.render_views(t, torch.from_numpy(np.ascontiguousarray(photo[..., :3]))[None].to(dev),
+                         torch.as_tensor(K)[:1], orbit=(n_frames, angle_range), alpha=alpha, colors=cols)
+    seq = torch.cat([out["overlay"], out["orbit"][0]]).cpu().numpy()
+    return [seq[i] for i in out["frame_order"]]
+
+
 def forward_model(model, input_image, camera_parameters, det_thresh=0.3, nms_kernel_size=1):
     """One forward on an image batch and its intrinsics (demo.py:108-126).  The reference wraps the call in
     no_grad + fp16 autocast; here precision is fixed by the kernels (fp16 tensor-core operands, fp32

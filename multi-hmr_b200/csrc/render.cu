@@ -257,6 +257,73 @@ __global__ void __launch_bounds__(256) render_raster_big_kernel(Params a) {
   }
 }
 
+// ---- props: extra meshes of other topologies in the same z-buffer ------------------------------------------------
+// Prop j is mesh P + j of the key.  Its topology's faces and CSR sit in the handle's concatenated topology arrays;
+// the per-prop offsets travel by value.
+struct Props {
+  int n, total_faces, total_verts;
+  int face_off[MHMR_RENDER_MAX_PROPS], nf[MHMR_RENDER_MAX_PROPS];   // into faces (in faces), of the topology
+  int ptr_off[MHMR_RENDER_MAX_PROPS], nv[MHMR_RENDER_MAX_PROPS];    // into csr_ptr, vertices of the topology
+  int vert_off[MHMR_RENDER_MAX_PROPS], fsum[MHMR_RENDER_MAX_PROPS]; // into verts / normals; faces of props < j
+  const int* faces;
+  const int* csr_ptr;
+  const int* csr_ent;
+  const float* verts;
+  const float* colors;
+  const unsigned char* visible;
+  float* normals;
+};
+
+__device__ __forceinline__ int prop_of_vertex(const Props& q, int i) {
+  int j = 0;
+  while (j + 1 < q.n && q.vert_off[j + 1] <= i) ++j;
+  return j;
+}
+
+__device__ __forceinline__ int prop_of_face(const Props& q, int i) {
+  int j = 0;
+  while (j + 1 < q.n && q.fsum[j + 1] <= i) ++j;
+  return j;
+}
+
+// Vertex normals of the props, as render_prep_kernel computes the persons'.
+__global__ void render_prop_normals_kernel(Props q) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= q.total_verts) return;
+  const int j = prop_of_vertex(q, i), v = i - q.vert_off[j];
+  const float* vp = q.verts + static_cast<size_t>(q.vert_off[j]) * 3;
+  const int* faces = q.faces + 3ll * q.face_off[j];
+  const int* ptr = q.csr_ptr + q.ptr_off[j];
+  float3 acc = make_float3(0.f, 0.f, 0.f);
+  for (int e = ptr[v]; e < ptr[v + 1]; ++e) {
+    const int ent = q.csr_ent[e], f = ent / 3, corner = ent % 3;
+    const int* fc = faces + 3 * f;
+    const float3 p0 = load3(vp + 3 * fc[corner]), p1 = load3(vp + 3 * fc[(corner + 1) % 3]),
+                 p2 = load3(vp + 3 * fc[(corner + 2) % 3]);
+    const float3 fn = cross3(sub3(p1, p0), sub3(p2, p0));
+    const float3 u = sub3(p1, p0), w = sub3(p2, p0);
+    const float ang = atan2f(sqrtf(dot3(fn, fn)), dot3(u, w));
+    const float3 un = normalize3(fn);
+    acc.x = fmaf(ang, un.x, acc.x); acc.y = fmaf(ang, un.y, acc.y); acc.z = fmaf(ang, un.z, acc.z);
+  }
+  const float3 n = normalize3(acc);
+  float* out = q.normals + static_cast<size_t>(i) * 3;
+  out[0] = n.x; out[1] = n.y; out[2] = n.z;
+}
+
+// One CTA per (prop face, view): props are few faces, often large on screen (a glyph next to the camera).
+__global__ void __launch_bounds__(128) render_prop_raster_kernel(Params a, Props q) {
+  const int b = blockIdx.y, j = prop_of_face(q, blockIdx.x), f = blockIdx.x - q.fsum[j];
+  if (q.visible && !q.visible[static_cast<size_t>(b) * q.n + j]) return;
+  const Cam c = load_cam(a.K, a.pose, b);
+  if (!(c.fx > 0.f) || !(c.fy > 0.f)) return;
+  Tri T;
+  if (!tri_setup(q.verts + static_cast<size_t>(q.vert_off[j]) * 3, q.faces + 3ll * (q.face_off[j] + f), c, a.W, a.H,
+                 T))
+    return;
+  raster_box(a, T, c, b, (static_cast<unsigned int>(a.P + j) << a.fbits) | f, threadIdx.x, blockDim.x);
+}
+
 // ---- 4. shading + composite -------------------------------------------------------------------------------------
 struct Shade {
   const unsigned char* images;
@@ -265,6 +332,8 @@ struct Shade {
   unsigned char* overlay;
   float* depth;
   int* person;
+  const float* view_alpha;      // kExtra only: per-view alpha, or null
+  const int* view_background;   // kExtra only: per-view background image, or null
 };
 
 // pyrender's metallic-roughness fragment shader (the glTF reference BRDF) for one white directional light along the
@@ -300,14 +369,18 @@ __device__ __forceinline__ float3 shade_pbr(float3 n, float3 v, float3 base, flo
   return make_float3(out[0], out[1], out[2]);
 }
 
-__global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s) {
+// kExtra: props, per-view alpha and backgrounds (mhmr_render_forward_extra); without, the one-topology path.
+template <bool kExtra>
+__global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s, Props q) {
   const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   const long long hw = static_cast<long long>(a.H) * a.W;
   if (i >= a.views * hw) return;
   const int b = static_cast<int>(i / hw), pix = static_cast<int>(i % hw), y = pix / a.W, x = pix % a.W;
   const unsigned long long* keys = a.keys + b * hw;
   const unsigned long long key = keys[pix];
-  const unsigned char* bg = s.images + (static_cast<size_t>(a.view_image[b]) * hw + pix) * 3;
+  const int bg_image = kExtra && s.view_background ? s.view_background[b] : a.view_image[b];
+  const float alpha = kExtra && s.view_alpha ? s.view_alpha[b] : s.alpha;
+  const unsigned char* bg = s.images + (static_cast<size_t>(bg_image) * hw + pix) * 3;
   unsigned char* out = s.overlay + i * 3;
   if (key == kEmpty) {  // fg = 0: the blend returns the photo exactly
     out[0] = bg[0]; out[1] = bg[1]; out[2] = bg[2];
@@ -330,6 +403,15 @@ __global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s) {
   const Cam c = load_cam(a.K, a.pose, b);
   const float* vp = a.verts + static_cast<size_t>(p) * a.V * 3;
   const int* fc = a.faces + 3 * f;
+  const float* vn_base = a.normals + static_cast<size_t>(p) * a.V * 3;
+  const float* col = s.colors + 3 * p;
+  if (kExtra && p >= a.P) {
+    const int j = p - a.P;
+    vp = q.verts + static_cast<size_t>(q.vert_off[j]) * 3;
+    fc = q.faces + 3ll * (q.face_off[j] + f);
+    vn_base = q.normals + static_cast<size_t>(q.vert_off[j]) * 3;
+    col = q.colors + 3 * j;
+  }
   Tri T;
   tri_setup(vp, fc, c, a.W, a.H, T);
   const float rx = ray_x(c, x), ry = ray_y(c, y);
@@ -342,7 +424,7 @@ __global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s) {
     float3 acc = make_float3(0.f, 0.f, 0.f);
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-      const float3 vn = load3(a.normals + (static_cast<size_t>(p) * a.V + fc[k]) * 3);
+      const float3 vn = load3(vn_base + static_cast<size_t>(fc[k]) * 3);
       const float w = e[k] * inv;
       acc.x = fmaf(w, vn.x, acc.x); acc.y = fmaf(w, vn.y, acc.y); acc.z = fmaf(w, vn.z, acc.z);
     }
@@ -351,18 +433,154 @@ __global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s) {
     n = normalize3(cross3(sub3(T.p[1], T.p[0]), sub3(T.p[2], T.p[0])));
   }
   const float3 v = normalize3(make_float3(-rx * z, -ry * z, -z));
-  const float* col = s.colors + 3 * p;
   const float3 rgb = shade_pbr(n, v, make_float3(col[0], col[1], col[2]), s.intensity, s.metallic, s.roughness);
   const float rgbv[3] = {rgb.x, rgb.y, rgb.z};
 #pragma unroll
   for (int ch = 0; ch < 3; ++ch) {
     const float r8 = rintf(rgbv[ch] * 255.f);
     const float im = static_cast<float>(bg[ch]);
-    const float o = fg * (s.alpha * r8 + (1.f - s.alpha) * im) + (1.f - fg) * im;
+    const float o = fg * (alpha * r8 + (1.f - alpha) * im) + (1.f - fg) * im;
     out[ch] = static_cast<unsigned char>(fminf(fmaxf(o, 0.f), 255.f));
   }
   if (s.depth) s.depth[i] = z;
   if (s.person) s.person[i] = p;
+}
+
+// ---- view poses of the demo (demo.py:160-241, utils/render.py:329-448) ------------------------------------------
+constexpr int kPoseThreads = 256;
+constexpr int kMaxPosePersons = 4096;
+
+__device__ void put_pose(float* out, const double (&R)[9], const double (&t)[3]) {
+  for (int r = 0; r < 3; ++r) {
+    for (int k = 0; k < 3; ++k) out[4 * r + k] = static_cast<float>(R[3 * r + k]);
+    out[4 * r + 3] = static_cast<float>(t[r]);
+  }
+}
+
+// utils/render.py:lookAt with up (0, -1, 0) and normalisation v / (|v| + 1e-13), then OPENCV_TO_OPENGL @ view:
+// rows x, -y, z_forward of the camera frame and t = -R eye.
+__device__ void look_at(const double (&eye)[3], const double (&at)[3], float* out) {
+  auto normalize = [](double (&v)[3]) {
+    const double l = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]) + 1e-13;
+    v[0] = v[0] / l; v[1] = v[1] / l; v[2] = v[2] / l;
+  };
+  double z[3] = {at[0] - eye[0], at[1] - eye[1], at[2] - eye[2]};
+  normalize(z);
+  const double up[3] = {0.0, -1.0, 0.0};
+  double x[3] = {z[1] * up[2] - up[1] * z[2], z[2] * up[0] - up[2] * z[0], z[0] * up[1] - up[0] * z[1]};
+  normalize(x);
+  const double y[3] = {x[1] * z[2] - z[1] * x[2], x[2] * z[0] - z[2] * x[0], x[0] * z[1] - z[0] * x[1]};
+  const double R[9] = {x[0], x[1], x[2], -y[0], -y[1], -y[2], z[0], z[1], z[2]};
+  double t[3];
+  for (int r = 0; r < 3; ++r) t[r] = -(R[3 * r] * eye[0] + R[3 * r + 1] * eye[1] + R[3 * r + 2] * eye[2]);
+  put_pose(out, R, t);
+}
+
+struct PoseArgs {
+  int images, P, V, n_frames, side, vpi;
+  double angle_range;
+  const int* count;
+  const int* person_image;
+  const float* verts;
+  const float* transl_pelvis;
+  const float* transl;
+  float* pose;
+  unsigned char* nonempty;
+  int* rank;
+};
+
+// One CTA per image.  Each thread takes persons p strided and counts, over all persons q of the image, those listed
+// before p (its rank: list order, or stable by transl z) and those with a smaller pelvis depth (its slot in the
+// sorted depths, ties by index): O(n^2 / threads) per image, no serial sort.  All threads then sum the first
+// person's vertices in fp64, strided, and reduce in a fixed-order tree: the centroid is bitwise repeatable.
+__global__ void __launch_bounds__(kPoseThreads) render_pose_kernel(PoseArgs a) {
+  extern __shared__ double sh[];  // [3][kPoseThreads] partial sums, then [P] sorted depths
+  __shared__ int s_first, s_cnt;
+  double* zs = sh + 3 * kPoseThreads;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int n = min(max(*a.count, 0), a.P);
+  if (b == 0)
+    for (int p = tid; p < a.P; p += blockDim.x)
+      if (p >= n || a.person_image[p] < 0 || a.person_image[p] >= a.images) a.rank[p] = -1;
+  if (tid == 0) {
+    s_first = -1;
+    s_cnt = 0;
+  }
+  __syncthreads();
+  for (int p = tid; p < n; p += blockDim.x) {
+    if (a.person_image[p] != b) continue;
+    const float zp = a.transl ? a.transl[3 * p + 2] : 0.f;
+    const float tp = a.transl_pelvis ? a.transl_pelvis[3 * p + 2] : 0.f;
+    int r = 0, slot = 0;
+    for (int q = 0; q < n; ++q) {
+      if (a.person_image[q] != b) continue;
+      if (a.transl) {
+        const float zq = a.transl[3 * q + 2];
+        r += zq < zp || (zq == zp && q < p);
+      } else {
+        r += q < p;
+      }
+      if (a.transl_pelvis) {
+        const float tq = a.transl_pelvis[3 * q + 2];
+        slot += tq < tp || (tq == tp && q < p);
+      }
+    }
+    a.rank[p] = r;
+    if (r == 0) s_first = p;  // the ranks of an image are a permutation: one writer
+    if (a.transl_pelvis) zs[slot] = static_cast<double>(tp);
+    atomicAdd(&s_cnt, 1);
+  }
+  __syncthreads();
+  if (tid == 0) a.nonempty[b] = s_cnt > 0 ? 1 : 0;
+  const int first = s_first, cnt = s_cnt;
+  double acc[3] = {0.0, 0.0, 0.0};
+  if (first >= 0) {
+    const float* vp = a.verts + static_cast<size_t>(first) * a.V * 3;
+    for (int v = tid; v < a.V; v += blockDim.x)
+      for (int k = 0; k < 3; ++k) acc[k] += static_cast<double>(vp[3 * v + k]);
+  }
+  for (int k = 0; k < 3; ++k) sh[k * kPoseThreads + tid] = acc[k];
+  __syncthreads();
+  for (int s = kPoseThreads / 2; s > 0; s >>= 1) {
+    if (tid < s)
+      for (int k = 0; k < 3; ++k) sh[k * kPoseThreads + tid] += sh[k * kPoseThreads + tid + s];
+    __syncthreads();
+  }
+  if (tid != 0) return;
+  float* out = a.pose + static_cast<size_t>(b) * a.vpi * 12;
+  const double I[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, zero[3] = {0, 0, 0};
+  for (int w = 0; w < a.vpi; ++w) put_pose(out + 12 * w, I, zero);
+  if (cnt == 0) return;
+  const double c[3] = {sh[0] / a.V, sh[kPoseThreads] / a.V, sh[2 * kPoseThreads] / a.V};
+  int w = 1;
+  if (a.n_frames >= 2) {
+    const double kDeg = 3.141592653589793 / 180.0;  // np.deg2rad
+    for (int sweep = 0; sweep < 3; ++sweep) {
+      const double range = sweep == 1 ? -a.angle_range : a.angle_range;
+      for (int i = 0; i < a.n_frames; ++i, ++w) {
+        const double th = range * i / (a.n_frames - 1) * kDeg, co = cos(th), si = sin(th);
+        double R[9];
+        if (sweep < 2) {
+          const double Ry[9] = {co, 0, si, 0, 1, 0, -si, 0, co};
+          for (int k = 0; k < 9; ++k) R[k] = Ry[k];
+        } else {
+          const double Rx[9] = {1, 0, 0, 0, co, -si, 0, si, co};
+          for (int k = 0; k < 9; ++k) R[k] = Rx[k];
+        }
+        double t[3];
+        for (int r = 0; r < 3; ++r) t[r] = c[r] - (R[3 * r] * c[0] + R[3 * r + 1] * c[1] + R[3 * r + 2] * c[2]);
+        put_pose(out + 12 * w, R, t);
+      }
+    }
+  }
+  if (a.side) {
+    const double zt = (cnt % 2) ? zs[cnt / 2] : (zs[cnt / 2 - 1] + zs[cnt / 2]) / 2.0;  // np.median
+    const double e0[3] = {2.0, -1.0, -2.0}, t0[3] = {0.0, 0.0, 3.0};
+    const double e1[3] = {2.2 * zt, 0.0, zt}, e2[3] = {0.0, -2.0 * zt, zt - 0.001}, tz[3] = {0.0, 0.0, zt};
+    look_at(e0, t0, out + 12 * w);
+    look_at(e1, tz, out + 12 * (w + 1));
+    look_at(e2, tz, out + 12 * (w + 2));
+  }
 }
 
 }  // namespace
@@ -378,10 +596,18 @@ struct mhmr_render {
   size_t key_cap = 0;
   float* normals = nullptr;
   size_t normal_cap = 0;
+  // extra topologies: faces (local indices) and CSR back to back; per topology, host offsets
+  int* topo_faces = nullptr;
+  int* topo_ptr = nullptr;
+  int* topo_ent = nullptr;
+  float* prop_normals = nullptr;
+  size_t prop_normal_cap = 0;
+  std::vector<int> topo_face_off, topo_nf, topo_ptr_off, topo_nv;
   ~mhmr_render() {
     for (void* p : {static_cast<void*>(faces), static_cast<void*>(csr_ptr), static_cast<void*>(csr_ent),
                     static_cast<void*>(queue), static_cast<void*>(queue_count), static_cast<void*>(keys),
-                    static_cast<void*>(normals)})
+                    static_cast<void*>(normals), static_cast<void*>(topo_faces), static_cast<void*>(topo_ptr),
+                    static_cast<void*>(topo_ent), static_cast<void*>(prop_normals)})
       if (p) cudaFree(p);
   }
 };
@@ -399,17 +625,45 @@ int grow(T** buf, size_t* cap, size_t n) {
   return MHMR_OK;
 }
 
+// vertex -> incident (face, corner) entries, faces in increasing order; ptr values offset by `base`
+void build_csr(const int32_t* hf, int F, int V, int base, std::vector<int32_t>& ptr, std::vector<int32_t>& ent) {
+  const size_t p0 = ptr.size(), e0 = ent.size();
+  ptr.resize(p0 + V + 1, 0);
+  ent.resize(e0 + 3ll * F);
+  for (int i = 0; i < 3 * F; ++i) ++ptr[p0 + hf[i] + 1];
+  for (int v = 0; v < V; ++v) ptr[p0 + v + 1] += ptr[p0 + v];
+  std::vector<int32_t> fill(ptr.begin() + p0, ptr.begin() + p0 + V);
+  for (int i = 0; i < 3 * F; ++i) ent[e0 + fill[hf[i]]++] = i;
+  for (size_t i = p0; i < ptr.size(); ++i) ptr[i] += base;
+}
+
+int render_build_topologies(mhmr_render* h, const int32_t* topo_faces, int total_faces, cudaStream_t st) {
+  std::vector<int32_t> hf(3ll * total_faces), ptr, ent;
+  MHMR_CUDA_CHECK(cudaMemcpy(hf.data(), topo_faces, 12ll * total_faces, cudaMemcpyDefault));
+  for (size_t t = 0; t < h->topo_nf.size(); ++t) {
+    const int32_t* f = hf.data() + 3ll * h->topo_face_off[t];
+    for (int i = 0; i < 3 * h->topo_nf[t]; ++i)
+      MHMR_REQUIRE(f[i] >= 0 && f[i] < h->topo_nv[t], "topology face vertex index outside [0, its num_verts)");
+    h->topo_ptr_off.push_back(static_cast<int>(ptr.size()));
+    build_csr(f, h->topo_nf[t], h->topo_nv[t], static_cast<int>(ent.size()), ptr, ent);
+  }
+  MHMR_CUDA_CHECK(cudaMalloc(&h->topo_faces, 12ll * total_faces));
+  MHMR_CUDA_CHECK(cudaMalloc(&h->topo_ptr, 4ll * ptr.size()));
+  MHMR_CUDA_CHECK(cudaMalloc(&h->topo_ent, 4ll * ent.size()));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->topo_faces, hf.data(), 12ll * total_faces, cudaMemcpyHostToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->topo_ptr, ptr.data(), 4ll * ptr.size(), cudaMemcpyHostToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->topo_ent, ent.data(), 4ll * ent.size(), cudaMemcpyHostToDevice, st));
+  MHMR_CUDA_CHECK(cudaStreamSynchronize(st));
+  return MHMR_OK;
+}
+
 int render_build(mhmr_render* h, const int32_t* faces, cudaStream_t st) {
   const int F = h->F, V = h->V;
   std::vector<int32_t> hf(3ll * F);
   MHMR_CUDA_CHECK(cudaMemcpy(hf.data(), faces, 12ll * F, cudaMemcpyDefault));
   for (int32_t v : hf) MHMR_REQUIRE(v >= 0 && v < V, "face vertex index outside [0, num_verts)");
-  // vertex -> incident (face, corner) entries, faces in increasing order
-  std::vector<int32_t> ptr(V + 1, 0), ent(3ll * F);
-  for (int32_t v : hf) ++ptr[v + 1];
-  for (int v = 0; v < V; ++v) ptr[v + 1] += ptr[v];
-  std::vector<int32_t> fill(ptr.begin(), ptr.end() - 1);
-  for (int i = 0; i < 3 * F; ++i) ent[fill[hf[i]]++] = i;
+  std::vector<int32_t> ptr, ent;
+  build_csr(hf.data(), F, V, 0, ptr, ent);
   MHMR_CUDA_CHECK(cudaMalloc(&h->faces, 12ll * F));
   MHMR_CUDA_CHECK(cudaMalloc(&h->csr_ptr, 4ll * (V + 1)));
   MHMR_CUDA_CHECK(cudaMalloc(&h->csr_ent, 12ll * F));
@@ -426,23 +680,46 @@ int render_build(mhmr_render* h, const int32_t* faces, cudaStream_t st) {
 
 extern "C" {
 
-int mhmr_render_create(const int32_t* faces, int num_faces, int num_verts, void* stream, mhmr_render** out) {
+int mhmr_render_create_topologies(const int32_t* faces, int num_faces, int num_verts, int num_topologies,
+                                  const int32_t* topo_faces, const int32_t* topo_num_faces,
+                                  const int32_t* topo_num_verts, void* stream, mhmr_render** out) {
   MHMR_REQUIRE(out != nullptr, "null output handle");
   *out = nullptr;
   MHMR_REQUIRE(faces != nullptr, "null faces");
   MHMR_REQUIRE(num_faces >= 1 && num_verts >= 3, "need at least one face and three vertices");
+  MHMR_REQUIRE(num_topologies >= 0, "negative topology count");
+  MHMR_REQUIRE(num_topologies == 0 || (topo_faces && topo_num_faces && topo_num_verts), "null topology argument");
+  long long max_faces = num_faces, total = 0;
+  for (int t = 0; t < num_topologies; ++t) {
+    MHMR_REQUIRE(topo_num_faces[t] >= 1 && topo_num_verts[t] >= 3,
+                 "a topology needs at least one face and three vertices");
+    max_faces = std::max<long long>(max_faces, topo_num_faces[t]);
+    total += topo_num_faces[t];
+  }
+  MHMR_REQUIRE(total < (1ll << 31) / 3, "too many topology faces");
   int fbits = 0;
-  while ((1ll << fbits) < num_faces) ++fbits;
-  MHMR_REQUIRE(fbits <= 24, "at most 2^24 faces (the depth key keeps 32 bits for person and face)");
+  while ((1ll << fbits) < max_faces) ++fbits;
+  MHMR_REQUIRE(fbits <= 24, "at most 2^24 faces (the depth key keeps 32 bits for mesh and face)");
   auto* h = new mhmr_render();
   h->F = num_faces; h->V = num_verts; h->fbits = fbits; h->nnz = 3 * num_faces;
-  const int rc = render_build(h, faces, static_cast<cudaStream_t>(stream));
+  for (int t = 0, off = 0; t < num_topologies; off += topo_num_faces[t++]) {
+    h->topo_face_off.push_back(off);
+    h->topo_nf.push_back(topo_num_faces[t]);
+    h->topo_nv.push_back(topo_num_verts[t]);
+  }
+  int rc = render_build(h, faces, static_cast<cudaStream_t>(stream));
+  if (rc == MHMR_OK && num_topologies > 0)
+    rc = render_build_topologies(h, topo_faces, static_cast<int>(total), static_cast<cudaStream_t>(stream));
   if (rc != MHMR_OK) {
     delete h;
     return rc;
   }
   *out = h;
   return MHMR_OK;
+}
+
+int mhmr_render_create(const int32_t* faces, int num_faces, int num_verts, void* stream, mhmr_render** out) {
+  return mhmr_render_create_topologies(faces, num_faces, num_verts, 0, nullptr, nullptr, nullptr, stream, out);
 }
 
 int mhmr_render_destroy(mhmr_render* h) {
@@ -458,12 +735,30 @@ int mhmr_render_info(const mhmr_render* h, int* num_faces, int* num_verts, int* 
   return MHMR_OK;
 }
 
-int mhmr_render_forward(mhmr_render* h, const mhmr_render_args* a, void* stream) {
+int mhmr_render_forward_extra(mhmr_render* h, const mhmr_render_args* a, const mhmr_render_extra* e,
+                              void* stream) {
   MHMR_REQUIRE(h != nullptr && a != nullptr, "null renderer or arguments");
   MHMR_REQUIRE(a->views >= 1 && a->H >= 1 && a->W >= 1, "views, H and W must be positive");
   MHMR_REQUIRE(a->max_persons >= 1, "max_persons must be positive");
-  MHMR_REQUIRE(static_cast<long long>(a->max_persons) <= (1ll << (32 - h->fbits)),
+  const int nprops = e ? e->num_props : 0;
+  MHMR_REQUIRE(nprops >= 0 && nprops <= MHMR_RENDER_MAX_PROPS, "at most MHMR_RENDER_MAX_PROPS props");
+  MHMR_REQUIRE(static_cast<long long>(a->max_persons) + nprops <= (1ll << (32 - h->fbits)),
                "max_persons does not fit the depth key next to the face index");
+  Props q{};
+  if (nprops > 0) {
+    MHMR_REQUIRE(e->prop_topology && e->prop_verts && e->prop_colors, "null prop argument");
+    q.n = nprops;
+    for (int j = 0; j < nprops; ++j) {
+      const int t = e->prop_topology[j];
+      MHMR_REQUIRE(t >= 0 && t < static_cast<int>(h->topo_nf.size()), "prop topology outside the handle's");
+      q.face_off[j] = h->topo_face_off[t]; q.nf[j] = h->topo_nf[t];
+      q.ptr_off[j] = h->topo_ptr_off[t]; q.nv[j] = h->topo_nv[t];
+      q.vert_off[j] = q.total_verts; q.fsum[j] = q.total_faces;
+      q.total_verts += q.nv[j]; q.total_faces += q.nf[j];
+    }
+    q.faces = h->topo_faces; q.csr_ptr = h->topo_ptr; q.csr_ent = h->topo_ent;
+    q.verts = e->prop_verts; q.colors = e->prop_colors; q.visible = e->prop_visible;
+  }
   MHMR_REQUIRE(static_cast<long long>(a->views) * a->max_persons <= 65535, "views x max_persons exceeds 65535");
   MHMR_REQUIRE(a->images && a->view_image && a->K && a->verts && a->person_image && a->count && a->colors &&
                    a->overlay,
@@ -474,6 +769,10 @@ int mhmr_render_forward(mhmr_render* h, const mhmr_render_args* a, void* stream)
   if (grow(&h->keys, &h->key_cap, npix) != MHMR_OK) return MHMR_ERR_CUDA;
   if (a->smooth && grow(&h->normals, &h->normal_cap, static_cast<size_t>(a->max_persons) * h->V * 3) != MHMR_OK)
     return MHMR_ERR_CUDA;
+  if (nprops > 0 && a->smooth &&
+      grow(&h->prop_normals, &h->prop_normal_cap, static_cast<size_t>(q.total_verts) * 3) != MHMR_OK)
+    return MHMR_ERR_CUDA;
+  q.normals = h->prop_normals;
   Params p;
   p.views = a->views; p.H = a->H; p.W = a->W; p.P = a->max_persons; p.F = h->F; p.V = h->V; p.fbits = h->fbits;
   p.smooth = a->smooth ? 1 : 0;
@@ -485,6 +784,8 @@ int mhmr_render_forward(mhmr_render* h, const mhmr_render_args* a, void* stream)
   s.images = a->images; s.colors = a->colors; s.alpha = a->alpha; s.intensity = a->intensity;
   s.metallic = a->metallic; s.roughness = a->roughness; s.overlay = a->overlay; s.depth = a->depth;
   s.person = a->person;
+  s.view_alpha = e ? e->view_alpha : nullptr;
+  s.view_background = e ? e->view_background : nullptr;
   const int sms = device_sm_count();
   const size_t prep_work = npix + (a->smooth ? static_cast<size_t>(a->max_persons) * h->V : 0);
   const int prep_blocks = static_cast<int>(std::min<size_t>((prep_work + 255) / 256, static_cast<size_t>(sms) * 16));
@@ -492,9 +793,50 @@ int mhmr_render_forward(mhmr_render* h, const mhmr_render_args* a, void* stream)
   MHMR_CUDA_CHECK(cudaGetLastError());
   render_raster_kernel<<<dim3((h->F + 127) / 128, a->views * a->max_persons), 128, 0, st>>>(p);
   MHMR_CUDA_CHECK(cudaGetLastError());
+  if (nprops > 0) {
+    if (a->smooth) {
+      render_prop_normals_kernel<<<(q.total_verts + 255) / 256, 256, 0, st>>>(q);
+      MHMR_CUDA_CHECK(cudaGetLastError());
+    }
+    render_prop_raster_kernel<<<dim3(q.total_faces, a->views), 128, 0, st>>>(p, q);
+    MHMR_CUDA_CHECK(cudaGetLastError());
+  }
   render_raster_big_kernel<<<sms * 8, 256, 0, st>>>(p);
   MHMR_CUDA_CHECK(cudaGetLastError());
-  render_shade_kernel<<<static_cast<unsigned>((npix + 255) / 256), 256, 0, st>>>(p, s);
+  const unsigned shade_blocks = static_cast<unsigned>((npix + 255) / 256);
+  if (e)
+    render_shade_kernel<true><<<shade_blocks, 256, 0, st>>>(p, s, q);
+  else
+    render_shade_kernel<false><<<shade_blocks, 256, 0, st>>>(p, s, q);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  return MHMR_OK;
+}
+
+int mhmr_render_forward(mhmr_render* h, const mhmr_render_args* a, void* stream) {
+  return mhmr_render_forward_extra(h, a, nullptr, stream);
+}
+
+int mhmr_render_view_poses(const mhmr_render_pose_args* a, void* stream) {
+  MHMR_REQUIRE(a != nullptr, "null arguments");
+  MHMR_REQUIRE(a->images >= 1 && a->max_persons >= 1 && a->num_verts >= 1,
+               "images, max_persons and num_verts must be positive");
+  MHMR_REQUIRE(a->max_persons <= kMaxPosePersons, "at most 4096 persons");
+  MHMR_REQUIRE(a->n_frames == 0 || a->n_frames >= 2, "n_frames must be 0 (no orbit) or at least 2");
+  MHMR_REQUIRE(a->n_frames <= 10000, "n_frames above 10000");
+  MHMR_REQUIRE(a->count && a->person_image && a->verts && a->pose && a->nonempty && a->rank, "null argument");
+  MHMR_REQUIRE(!a->side || a->transl_pelvis, "the side views need transl_pelvis");
+  PoseArgs p;
+  p.images = a->images; p.P = a->max_persons; p.V = a->num_verts; p.n_frames = a->n_frames;
+  p.side = a->side ? 1 : 0;
+  p.vpi = 1 + 3 * a->n_frames + 3 * p.side;
+  p.angle_range = a->angle_range;
+  p.count = a->count; p.person_image = a->person_image; p.verts = a->verts; p.transl_pelvis = a->transl_pelvis;
+  p.transl = a->transl; p.pose = a->pose; p.nonempty = a->nonempty; p.rank = a->rank;
+  const size_t smem = sizeof(double) * (3 * kPoseThreads + a->max_persons);
+  if (smem > 48 * 1024)
+    MHMR_CUDA_CHECK(cudaFuncSetAttribute(render_pose_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         static_cast<int>(smem)));
+  render_pose_kernel<<<a->images, kPoseThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }

@@ -6,6 +6,8 @@ per-kernel times from torch.profiler in a separate pass.  Prints the card name a
 Workloads: an 896 x 896 image with 4 persons; a 1920 x 1080 photo with 20 persons (the size demo.py renders at);
 a 20-frame rotating view of one image with 3 persons in one call (demo.py:160-195).  Meshes are seeded blob people
 (`synth.make_blob_people`) of 18 432 faces each, close to SMPL-X's 20 908, between 3 and 8 m from the camera.
+Then two `Renderer.render_views` workloads (see `view_workloads`; `--skip-views` leaves them out).  `--dump x.npz`
+saves the one-topology outputs, to compare builds bit for bit.
 """
 import argparse
 import json
@@ -49,11 +51,49 @@ def workloads():
     return out
 
 
+def view_workloads(res, args, dev):
+    """Renderer.render_views: the demo orbit of one 1920 x 1080 photo with 3 persons (n_frames 20, angle_range 60:
+    61 distinct views), and a batch of 8 images at 896 x 896 with 4 persons each taking the overlay, a 20-frame orbit
+    and the three side views (with the camera glyph) in one call."""
+    from multihmr_b200.render import Renderer, camera_glyph
+
+    for name, (W, H, B, n, side) in {"demo_orbit_1920x1080_3p": (1920, 1080, 1, 3, False),
+                                     "views_896_8x4p": (896, 896, 8, 4, True)}.items():
+        f = max(W, H) / (2 * np.tan(np.radians(30)))
+        verts, faces = _people(n * B, W, H, f, seed=len(name))
+        P = n * B
+        r = Renderer(faces, dev, topologies=camera_glyph()[0])
+        t = {"v3d": torch.from_numpy(verts).to(dev),
+             "det_idx": torch.arange(P, dtype=torch.int32, device=dev).div(n, rounding_mode="floor").expand(3, P)
+             .contiguous(), "count": torch.full((1,), P, dtype=torch.int32, device=dev),
+             "transl_pelvis": torch.from_numpy(verts.mean(1)).to(dev)}
+        photos = torch.randint(0, 256, (B, H, W, 3), dtype=torch.uint8, device=dev)
+        K = torch.tensor([[f, 0, W / 2], [0, f, H / 2], [0, 0, 1]], dtype=torch.float32).expand(B, 3, 3).to(dev)
+        kw = dict(orbit=(20, 60), side=side, alpha=0.8)
+        for _ in range(args.warmup):
+            r.render_views(t, photos, K, **kw)
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        calls = max(args.calls // 10, 10)
+        e0.record()
+        for _ in range(calls):
+            r.render_views(t, photos, K, **kw)
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / calls
+        views = B * (1 + 60 + (3 if side else 0))
+        res["workloads"][name] = {"ms_per_call": round(ms, 4), "ms_per_view": round(ms / views, 4), "views": views,
+                                  "persons": P, "faces_per_person": int(faces.shape[0]), "calls": calls}
+        print(f"{name}: {ms:.3f} ms per call, {ms / views:.4f} ms per view ({views} views)")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--skip-views", action="store_true", help="only the three one-topology workloads")
+    ap.add_argument("--dump", default=None, help="write the one-topology outputs of each workload to this .npz")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_render needs a CUDA device")
@@ -64,15 +104,20 @@ def main():
     res = {"gpu": q, "calls": args.calls, "workloads": {}}
     print(f"GPU: {q}")
     dev = torch.device("cuda")
+    dumps = {}
     for name, w in workloads().items():
         r = Renderer(w["faces"], dev)
-        imgs = torch.randint(0, 256, (1, w["H"], w["W"], 3), dtype=torch.uint8, device=dev)
+        imgs = torch.randint(0, 256, (1, w["H"], w["W"], 3), dtype=torch.uint8, device=dev,
+                             generator=torch.Generator(dev).manual_seed(len(name)))
         verts = torch.from_numpy(w["verts"]).to(dev)
         P = verts.shape[0]
         kw = dict(person_image=torch.zeros(P, dtype=torch.int32, device=dev),
                   count=torch.full((1,), P, dtype=torch.int32, device=dev), view_image=[0] * w["views"],
                   pose=w["pose"], alpha=0.8)
         K = w["K"].to(dev)
+        if args.dump:
+            o = r.render(verts, K, imgs, depth=True, index=True, **kw)
+            dumps.update({f"{name}_{k}": v.cpu().numpy() for k, v in o.items()})
         for _ in range(args.warmup):
             r.render(verts, K, imgs, **kw)
         torch.cuda.synchronize()
@@ -98,6 +143,10 @@ def main():
                                   "views": w["views"], "persons": P, "faces_per_person": int(w["faces"].shape[0]),
                                   "kernel_ms_per_call": kern}
         print(f"{name}: {ms:.3f} ms per call, {ms / w['views']:.3f} ms per view; kernels {kern}")
+    if args.dump:
+        np.savez_compressed(args.dump, **dumps)
+    if not args.skip_views:
+        view_workloads(res, args, dev)
     line = json.dumps(res)
     print(line)
     if args.out:
