@@ -352,6 +352,10 @@ int mhmr_anny_place(mhmr_engine* h, int P, int V, const float* bone_poses, const
 
 /* Stage-level entry: backbone only (blocks/dinov2.py:16-26): x [B,3,S,S] -> z [B,N,D] fp32. */
 int mhmr_vit_forward(mhmr_engine* h, const float* x, int B, float* z, void* stream);
+/* Stage-level entry: the bulk pass of mhmr_vit_forward stopped after its patch embedding and first `layers` blocks
+ * (0 <= layers <= depth): out [B,T,D] fp32 residual stream, cls row first.  Folded LayerNorm: hi + lo of the
+ * two-term fp16 stream; MHMR_LN_FOLD=0: the fp32 stream. */
+int mhmr_op_vit_stream(mhmr_engine* h, const float* x, int B, int layers, float* out, void* stream);
 /* Stage-level entry: SMPL-X layer only (blocks/smpl_layer.py:47-155) for P persons (device pointers):
  * rotvec [P,53,3], shape [P,nb], expression [P,10], loc [P,2], dist [P], K_det [P,3,3]. */
 int mhmr_smplx_forward(mhmr_engine* h, int P, const float* rotvec, const float* shape,

@@ -567,8 +567,12 @@ int run_plan(mhmr_engine* e, int cat, GemmPlan& plan, int M, cudaStream_t st) {
   return MHMR_OK;
 }
 
-int vit_forward(mhmr_engine* e, const ImgSrc& x, int B, float* z_out, cudaStream_t st) {
+// The bulk pass.  With stream_out (stage entry mhmr_op_vit_stream) it stops after the first `layers` blocks and writes
+// the residual stream [B, T, D] fp32 instead of the final norm; the product path runs all blocks.
+int vit_forward(mhmr_engine* e, const ImgSrc& x, int B, float* z_out, cudaStream_t st, int layers = -1,
+                float* stream_out = nullptr) {
   const int D = e->D, N = e->N, T = e->T, M = B * T;
+  if (layers < 0) layers = e->depth;
   if (x.u8 != nullptr) {
     LAUNCH(MHMR_CAT_MISC, im2col_u8_patch14(x.u8, x.lut, e->A16, B, e->cfg.img_size, 592, st));
   } else {
@@ -576,14 +580,14 @@ int vit_forward(mhmr_engine* e, const ImgSrc& x, int B, float* z_out, cudaStream
   }
   LAUNCH(MHMR_CAT_MISC, cls_rows(e->X, e->cls_pos, B, T, D, st));
   TRY(run_plan(e, MHMR_CAT_GEMM_OTHER, e->patch_plan, B * N, st));
-  for (int l = 0; l < e->depth; ++l) {
+  // the folded chain enters as the two-term stream (hi, lo) + row statistics
+  if (e->ln_fold)
+    LAUNCH(MHMR_CAT_LAYERNORM, split_rowstats(e->X, e->Xn16, e->Xlo, D, e->ln_stats, e->ln_slots, M, D, st));
+  for (int l = 0; l < layers; ++l) {
     VitLayer& L = e->vit[l];
     // norm1 / norm2: folded into qkv / fc1 (statistics + raw fp16 rows come from the previous epilogue), or kernels
-    if (!e->ln_fold) {
+    if (!e->ln_fold)
       LAUNCH(MHMR_CAT_LAYERNORM, layernorm(e->X, L.ln1_g, L.ln1_b, e->Xn16, D, nullptr, 0, M, D, 1e-6f, 0, 0, st));
-    } else if (l == 0) {
-      LAUNCH(MHMR_CAT_LAYERNORM, split_rowstats(e->X, e->Xn16, e->Xlo, D, e->ln_stats, e->ln_slots, M, D, st));
-    }
     TRY(run_plan(e, MHMR_CAT_GEMM_QKV, L.qkv, M, st));
     LAUNCH(MHMR_CAT_ATTENTION, attention_forward(e->QKV16, 3 * D, L.O16, D, B, T, D, st));
     TRY(run_plan(e, MHMR_CAT_GEMM_PROJ, L.proj, M, st));
@@ -591,6 +595,15 @@ int vit_forward(mhmr_engine* e, const ImgSrc& x, int B, float* z_out, cudaStream
       LAUNCH(MHMR_CAT_LAYERNORM, layernorm(e->X, L.ln2_g, L.ln2_b, e->Xn16, D, nullptr, 0, M, D, 1e-6f, 0, 0, st));
     TRY(run_plan(e, MHMR_CAT_GEMM_FC1, L.fc1, M, st));
     TRY(run_plan(e, MHMR_CAT_GEMM_FC2, L.fc2, M, st));
+  }
+  if (stream_out != nullptr) {
+    const int64_t n = static_cast<int64_t>(M) * D;
+    if (e->ln_fold) {
+      LAUNCH(MHMR_CAT_MISC, merge_split(e->Xn16, e->Xlo, stream_out, n, st));
+    } else {
+      MHMR_CUDA_CHECK(cudaMemcpyAsync(stream_out, e->X, n * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    return MHMR_OK;
   }
   // final norm, cls dropped: fp32 features (head query side, optional user copy) + fp16 context columns
   if (e->ln_fold) {
@@ -989,6 +1002,17 @@ int mhmr_vit_forward(mhmr_engine* h, const float* x, int B, float* z, void* stre
   ImgSrc src;
   src.f32 = x;
   return vit_forward(h, src, B, z, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_op_vit_stream(mhmr_engine* h, const float* x, int B, int layers, float* out, void* stream) {
+  MHMR_REQUIRE(h != nullptr && x != nullptr && out != nullptr, "null argument");
+  if (!h->finalized) { set_last_error("mhmr_op_vit_stream before mhmr_finalize"); return MHMR_ERR_STATE; }
+  MHMR_REQUIRE(B >= 1 && B <= h->cfg.max_batch, "batch exceeds max_batch");
+  MHMR_REQUIRE(layers >= 0 && layers <= h->depth, "layers outside [0, depth]");
+  h->launches = 0;
+  ImgSrc src;
+  src.f32 = x;
+  return vit_forward(h, src, B, nullptr, static_cast<cudaStream_t>(stream), layers, out);
 }
 
 int mhmr_smplx_forward(mhmr_engine* h, int P, const float* rotvec, const float* shape,

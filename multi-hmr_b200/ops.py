@@ -387,6 +387,20 @@ def cls_gather(x, T, B, D, xlo=None):
     return out
 
 
+def vit_stream(model, x, layers):
+    """The residual stream of `model`'s bulk pass after its patch embedding and first `layers` blocks: x [B,3,S,S]
+    (normalised fp32) -> fp32 [B, T, D], cls row first.  On the folded-LayerNorm path it is hi + lo of the two-term
+    fp16 stream the next block reads."""
+    model.finalize()
+    x = x.to(model.device, dtype=torch.float32).contiguous()
+    B = x.shape[0]
+    out = torch.empty(B, 1 + model.res * model.res, model.embed_dim, device=model.device)
+    with torch.cuda.device(model.device):
+        rc = _lib.load().mhmr_op_vit_stream(model._handle, ptr(x), c_int(B), c_int(layers), ptr(out), stream_ptr())
+    check(rc, "mhmr_op_vit_stream")
+    return out
+
+
 def anny_gather(z32, pos, det_b, det_y, det_x, count, max_persons, res, zc, xa, xr=None, norm=(None, None)):
     """Anny decoder inputs: zc [Pm, D] (bulk row, or the final norm of xr), xa [Pm, dim] = pos[cell]."""
     _cuda(z32, pos, zc, xa, xr, *norm)

@@ -21,7 +21,8 @@ EPS = 1e-6
 
 
 def r16(t):
-    return t.to(torch.float16).to(torch.float32)
+    """fp16 rounding of t, kept in t's dtype (the study runs in fp32 on the CPU and in fp64 in the tests)"""
+    return t.to(torch.float16).to(t.dtype)
 
 
 def split16(t):
@@ -30,10 +31,11 @@ def split16(t):
     return hi + r16(t - hi)
 
 
-def ln_linear(x, g, b, w, bias, mode, shift=None, qa=r16, qw=r16):
+def ln_linear(x, g, b, w, bias, mode, shift=None, qa=None, qw=None):
     """Linear(LayerNorm(x)) with the engine's rounding points.  mode: 'exact' | 'sep' | 'fold' | 'fold_shift'.
-    qa / qw round the folded GEMM's operands (fp16 by default)."""
+    qa / qw round the folded GEMM's operands (fp16 by default: r16 as it is when called)."""
     D = x.shape[-1]
+    qa, qw = qa or r16, qw or r16
     if mode == "exact":
         return F.linear(F.layer_norm(x, (D,), g, b, EPS), w, bias)
     if mode == "sep":
@@ -57,12 +59,14 @@ def attention(q, k, v):
     return torch.matmul(r16(p), v) / p.sum(dim=-1, keepdim=True)
 
 
-def forward(x_img, sd, name, pre, mode, o_in=None, mlp8=None, keep_cls=False):
+def forward(x_img, sd, name, pre, mode, o_in=None, mlp8=None, keep_cls=False, attn=None, taps=None):
     """mode 'sep' / 'fold' / 'fold_shift': bulk pass, returns (z, [O16 per layer], stats).  mode 'refine': fp32
     stream fed with the given attention outputs.  mlp8 = (fc1 A, fc1 W, fc2 A, fc2 W): the 'fold' bulk pass rounds
     the operands of fc1 (raw stream, folded W') and fc2 (GELU output, W2) with these functions instead of fp16
     (tools/precision_study.py --fp8).
-    keep_cls: z keeps the final-normed cls row in front."""
+    keep_cls: z keeps the final-normed cls row in front.  attn: attention(q, k, v) in place of `attention` (the same
+    arithmetic in another loop order).  taps: {layers: None} is filled with the residual stream [B, T, D] after the
+    patch embedding (layers = 0) and after each listed number of blocks."""
     cfg = dinov2_ref.ARCHS[name]
     H = cfg["num_heads"]
     if mode == "refine" or mode == "exact":
@@ -76,6 +80,8 @@ def forward(x_img, sd, name, pre, mode, o_in=None, mlp8=None, keep_cls=False):
     outs, ratios = [], []
     if mode.startswith("fold"):
         x = split16(x)
+    if taps is not None and 0 in taps:
+        taps[0] = x
     shift = x.mean(-1, keepdim=True)
     for i in range(cfg["depth"]):
         p = f"{pre}blocks.{i}."
@@ -92,7 +98,7 @@ def forward(x_img, sd, name, pre, mode, o_in=None, mlp8=None, keep_cls=False):
             if mode == "exact":
                 o = F.scaled_dot_product_attention(qkv[0], qkv[1], qkv[2])
             else:
-                o = r16(attention(qkv[0], qkv[1], qkv[2]))
+                o = r16((attn or attention)(qkv[0], qkv[1], qkv[2]))
             o = o.transpose(1, 2).reshape(B, T, D)
             outs.append(o)
         full = mode in ("refine", "exact")
@@ -101,7 +107,7 @@ def forward(x_img, sd, name, pre, mode, o_in=None, mlp8=None, keep_cls=False):
         x = x + sd[p + "ls1.gamma"] * F.linear(o, wp if full else r16(wp), sd[p + "attn.proj.bias"])
         if mode.startswith("fold"):
             x = split16(x)
-        qa1, qw1, qa2, qw2 = (r16,) * 4 if mlp8 is None else mlp8
+        qa1, qw1, qa2, qw2 = (None, None, r16, r16) if mlp8 is None else mlp8
         h = ln_linear(x, sd[p + "norm2.weight"], sd[p + "norm2.bias"], sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"],
                       "exact" if full else mode, shift, qa1, qw1)
         h = F.gelu(h)
@@ -110,6 +116,8 @@ def forward(x_img, sd, name, pre, mode, o_in=None, mlp8=None, keep_cls=False):
         x = x + sd[p + "ls2.gamma"] * F.linear(h if full else qa2(h), w2 if full else qw2(w2), sd[p + "mlp.fc2.bias"])
         if mode.startswith("fold"):
             x = split16(x)
+        if taps is not None and i + 1 in taps:
+            taps[i + 1] = x
     z = F.layer_norm(x, (D,), sd[pre + "norm.weight"], sd[pre + "norm.bias"], EPS)
     z = z if keep_cls else z[:, 1:]
     return z, outs, ratios
