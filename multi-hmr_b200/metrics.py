@@ -12,12 +12,10 @@ The three protocols of the reference README ("Evaluating BEDLAM-val / EHF-test /
           H36M joints of J_regressor_h36m"""
 from __future__ import annotations
 
-import ctypes
-
 import torch
 
 from . import _lib
-from ._lib import c_int, c_void_p, check, ptr
+from ._lib import call, stream
 from .model import BODY_TABLES, body_model_arrays
 
 # train.py:402-403 (SPIN's constants.py): the 14 LSP joints of the 17 H36M joints
@@ -54,15 +52,10 @@ def compute_prf1(count, miss, fp):
     return 100.0 * precision, 100.0 * recall, 100.0 * f1
 
 
-def _stream(dev):
-    return c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def match_2d_greedy(pred_j2d: torch.Tensor, gt_j2d: torch.Tensor, valid_mask: torch.Tensor | None = None,
                     iou_thresh: float = 0.05):
     """utils/training.py:25-147 on the device.  pred_j2d [P,J,2], gt_j2d [G,J,2] (CUDA, fp32).  Returns device tensors
     (pairs [min(P,G),2] int32, n_pairs [1] int32, pred_to_gt [P] int32, gt_to_pred [G] int32)."""
-    lib = _lib.load()
     dev = gt_j2d.device
     assert dev.type == "cuda", "the evaluation kernels need CUDA tensors (no CPU fallback)"
     P, G, J = int(pred_j2d.shape[0]), int(gt_j2d.shape[0]), int(gt_j2d.shape[1])
@@ -74,16 +67,13 @@ def match_2d_greedy(pred_j2d: torch.Tensor, gt_j2d: torch.Tensor, valid_mask: to
     p2g = torch.full((max(P, 1),), -1, device=dev, dtype=torch.int32)
     g2p = torch.full((G,), -1, device=dev, dtype=torch.int32)
     with torch.cuda.device(dev):
-        check(lib.mhmr_eval_match_2d(ptr(pred), ptr(gt), ptr(vm), c_int(P), c_int(G), c_int(J),
-                                     ctypes.c_float(iou_thresh), ptr(pairs), ptr(n_pairs), ptr(p2g), ptr(g2p),
-                                     _stream(dev)), "mhmr_eval_match_2d")
+        call("mhmr_eval_match_2d", pred, gt, vm, P, G, J, iou_thresh, pairs, n_pairs, p2g, g2p, stream(dev))
     return pairs, n_pairs, p2g[:P], g2p
 
 
 def points_error(pred, gt, pairs, n_pairs, pred_center=None, gt_center=None):
     """Mean point error (mm) and Procrustes-aligned mean point error (mm) of the matched pairs
     (train.py:387-394, :419-427).  pred [P,n,3], gt [G,n,3]; returns two device tensors [pairs.shape[0]]."""
-    lib = _lib.load()
     dev = gt.device
     n = int(gt.shape[1])
     assert pred.shape[1] == n, "prediction and ground truth need the same number of points"
@@ -94,8 +84,7 @@ def points_error(pred, gt, pairs, n_pairs, pred_center=None, gt_center=None):
     err = torch.zeros(M, device=dev)
     pa = torch.zeros(M, device=dev)
     with torch.cuda.device(dev):
-        check(lib.mhmr_eval_points_error(ptr(pred), ptr(pc), ptr(gt), ptr(gc), ptr(pairs), ptr(n_pairs), c_int(M),
-                                         c_int(n), ptr(err), ptr(pa), _stream(dev)), "mhmr_eval_points_error")
+        call("mhmr_eval_points_error", pred, pc, gt, gc, pairs, n_pairs, M, n, err, pa, stream(dev))
     return err, pa
 
 
@@ -122,7 +111,6 @@ def regress(A: CSR, X, pairs, n_pairs, side: int, center=None, rows=None, root: 
     """out[m] = A[rows] . (X[s] - center[s]) (minus the root row's result when root >= 0), s = pairs[m, side], for the
     matched pairs m < n_pairs still on the device (`mhmr_eval_regress`).  X [*, N, 3]; returns out [M, R_out, 3] and,
     when K [*, 3, 3] is given, the projection out2d [M, R_out, 2]."""
-    lib = _lib.load()
     dev = X.device
     R, N = A.shape
     assert X.shape[1] == N, f"regressor takes {N} points, got {X.shape[1]}"
@@ -139,9 +127,8 @@ def regress(A: CSR, X, pairs, n_pairs, side: int, center=None, rows=None, root: 
     Kd = None if K is None else K.to(dev, torch.float32).reshape(-1, 9).contiguous()
     out2d = None if K is None else torch.zeros(M, R_out, 2, device=dev)
     with torch.cuda.device(dev):
-        check(lib.mhmr_eval_regress(ptr(A.rowptr), ptr(A.col), ptr(A.val), c_int(R), c_int(N), ptr(r), c_int(R_out),
-                                    c_int(root), ptr(X), ptr(c), ptr(pairs), c_int(side), ptr(n_pairs), c_int(M),
-                                    ptr(Kd), ptr(out), ptr(out2d), _stream(dev)), "mhmr_eval_regress")
+        call("mhmr_eval_regress", A.rowptr, A.col, A.val, R, N, r, R_out, root, X, c, pairs, side, n_pairs, M, Kd, out,
+             out2d, stream(dev))
     return out, out2d
 
 
@@ -153,7 +140,6 @@ class BodyModel:
 
     def __init__(self, bm: dict, kind: str, num_betas: int | None = None, max_persons: int = 48, device="cuda"):
         assert kind in ("smpl", "smplx"), kind
-        lib = _lib.load()
         dev = torch.device(device)
         self.kind, self.device, self.max_persons = kind, dev, int(max_persons)
         nb = int(num_betas if num_betas is not None else (11 if kind == "smplx" else 10))
@@ -161,24 +147,23 @@ class BodyModel:
                   for k, v in body_model_arrays(bm, nb, landmarks=kind == "smplx").items()}
         V = int(arrays["v_template"].shape[0])
         self.num_verts, self.num_betas = V, nb
-        a = lambda *ks: [ptr(arrays.get(k)) for k in ks]
-        h = c_void_p()
+        keys = ("v_template", "shapedirs", "expr_dirs", "posedirs", "J_regressor", "lbs_weights", "parents",
+                "extra_joints_idxs", "lmk_tri", "lmk_bary_coords")
+        h = torch.zeros(1, dtype=torch.int64)
         with torch.cuda.device(dev):
-            check(lib.mhmr_body_create(c_int(1 if kind == "smplx" else 0), c_int(V), c_int(nb), c_int(self.max_persons),
-                                       *a("v_template", "shapedirs", "expr_dirs", "posedirs", "J_regressor",
-                                          "lbs_weights", "parents", "extra_joints_idxs", "lmk_tri", "lmk_bary_coords"),
-                                       _stream(dev), ctypes.byref(h)), "mhmr_body_create")
-        self._h = h
-        self._lib = lib
-        nj_out, nj = ctypes.c_int(), ctypes.c_int()
-        check(lib.mhmr_body_info(h, None, ctypes.byref(nj_out), ctypes.byref(nj), None, None), "mhmr_body_info")
-        self.num_joints, self.num_pose_joints = nj_out.value, nj.value
+            call("mhmr_body_create", 1 if kind == "smplx" else 0, V, nb, self.max_persons,
+                 *(arrays.get(k) for k in keys), stream(dev), h)
+        self._h = h.item()
+        self._lib = _lib.load()
+        nj_out, nj = torch.zeros(1, dtype=torch.int32), torch.zeros(1, dtype=torch.int32)
+        call("mhmr_body_info", self._h, None, nj_out, nj, None, None)
+        self.num_joints, self.num_pose_joints = nj_out.item(), nj.item()
         # smplx J_regressor (EHF joints = J_regressor @ vertices, train.py:73)
         self.j_regressor = CSR(bm["J_regressor"], dev)
 
     def __del__(self):
         h = getattr(self, "_h", None)
-        if h is not None and h.value:
+        if h:
             self._lib.mhmr_body_destroy(h)
             self._h = None
 
@@ -216,9 +201,8 @@ class BodyModel:
         out = dict(v3d=torch.empty(P, V, 3, device=dev), j3d=torch.empty(P, J, 3, device=dev),
                    j2d=torch.empty(P, J, 2, device=dev), transl_pelvis=torch.empty(P, 3, device=dev))
         with torch.cuda.device(dev):
-            check(self._lib.mhmr_body_forward(self._h, c_int(P), ptr(fp), ptr(b), ptr(ex), ptr(tr), ptr(Kd),
-                                              ptr(out["v3d"]), None, ptr(out["j3d"]), ptr(out["j2d"]),
-                                              ptr(out["transl_pelvis"]), _stream(dev)), "mhmr_body_forward")
+            call("mhmr_body_forward", self._h, P, fp, b, ex, tr, Kd, out["v3d"], None, out["j3d"], out["j2d"],
+                 out["transl_pelvis"], stream(dev))
         return out
 
     def _backward(self, fp, b, tr, Kd, ex, g_v3d=None, g_v2d=None, g_j3d=None, g_j2d=None, g_transl_pelvis=None):
@@ -229,10 +213,8 @@ class BodyModel:
         d_fp, d_b, d_tr = torch.empty_like(fp), torch.empty_like(b), torch.empty_like(tr)
         d_ex = torch.empty(P, 10, device=dev) if ex is not None else None
         with torch.cuda.device(dev):
-            check(self._lib.mhmr_body_backward(self._h, c_int(P), ptr(fp), ptr(b), ptr(ex), ptr(tr), ptr(Kd),
-                                               ptr(g(g_v3d)), ptr(g(g_v2d)), ptr(g(g_j3d)), ptr(g(g_j2d)),
-                                               ptr(g(g_transl_pelvis)), ptr(d_fp), ptr(d_b), ptr(d_ex), ptr(d_tr),
-                                               _stream(dev)), "mhmr_body_backward")
+            call("mhmr_body_backward", self._h, P, fp, b, ex, tr, Kd, g(g_v3d), g(g_v2d), g(g_j3d), g(g_j2d),
+                 g(g_transl_pelvis), d_fp, d_b, d_ex, d_tr, stream(dev))
         return d_fp, d_b, d_ex, d_tr
 
 

@@ -9,7 +9,6 @@ and the built extension are required, otherwise construction / forward raise.
 """
 from __future__ import annotations
 
-import ctypes
 import math
 from types import SimpleNamespace
 
@@ -17,7 +16,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from ._lib import c_int, c_int64, c_void_p, check, ptr
+from ._lib import call, stream
 
 ARCH_ID = {"dinov2_vits14": 0, "dinov2_vitb14": 1, "dinov2_vitl14": 2}
 EMBED_DIM = {"dinov2_vits14": 384, "dinov2_vitb14": 768, "dinov2_vitl14": 1024}
@@ -60,18 +59,9 @@ def body_model_arrays(bm: dict, num_betas: int, landmarks: bool = True) -> dict:
     return out
 
 
-class _Config(ctypes.Structure):
-    _fields_ = [(n, c_int) for n in ("arch", "img_size", "max_batch", "max_persons", "xat_depth",
-                                     "xat_num_heads", "num_betas", "person_center_idx", "num_verts",
-                                     "refine_central", "head", "xat_dim", "xat_mlp_dim", "num_joints")]
-
-
-_OUT_FIELDS = ("scores_map", "count", "det_idx", "det_score", "offset", "loc", "dist_pp", "dist", "rotmat",
-               "rotvec", "shape", "expression", "transl", "transl_pelvis", "v3d", "v2d", "j3d", "j2d", "z")
-
-
-class _Outputs(ctypes.Structure):
-    _fields_ = [(n, c_void_p) for n in _OUT_FIELDS]
+# the engine's structs under the names the hand-written binding gave them
+_Config, _Outputs = _lib.structs()["mhmr_config"], _lib.structs()["mhmr_outputs"]
+_OUT_FIELDS = _Outputs.field_names()
 
 
 def interpolate_pos_embed(pos_embed: torch.Tensor, grid: int) -> torch.Tensor:
@@ -99,7 +89,7 @@ class _EngineModel:
     _POS_EMBED_KEY = ""    # the backbone's pos_embed, interpolated to the working grid at upload
     _SKIPPED_KEYS = ()     # state-dict keys the engine does not read
     _ENTRY = ""            # forward entry of the C-ABI; "_u8" appended for uint8 images
-    _OUT_STRUCT = None     # ctypes struct of that entry's output pointers, one field per output tensor
+    _OUTPUTS = ""          # the header struct of that entry's output pointers, one field per output tensor
     PROFILE_CATEGORIES = ("misc", "layernorm", "gemm_qkv", "attention", "gemm_proj", "gemm_fc1", "gemm_fc2",
                           "gemm_other", "head", "smplx", "refine")
 
@@ -153,7 +143,7 @@ class _EngineModel:
 
     # ------------------------------------------------------------------ load-time packing
     def _head_config(self) -> dict:
-        """The `_Config` fields of the head (all but arch, sizes, capacities and refine_central)."""
+        """The `mhmr_config` fields of the head (all but arch, sizes, capacities and refine_central)."""
         raise NotImplementedError
 
     def _upload_extras(self):
@@ -161,18 +151,18 @@ class _EngineModel:
 
     def _set_weight(self, key, t):
         t = t.detach().to(torch.float32).contiguous()
-        check(self._lib.mhmr_set_weight(self._handle, key.encode(), ptr(t), c_int64(t.numel())), f"set_weight({key})")
+        call("mhmr_set_weight", self._handle, key.encode(), t, t.numel())
 
     def finalize(self):
         if self._finalized:
             return self
         with torch.cuda.device(self.device):
-            cfg = _Config(arch=ARCH_ID[self.backbone_name], img_size=self.img_size, max_batch=self.max_batch,
-                          max_persons=self.max_persons, refine_central=1 if self.refine_central else 0,
-                          **self._head_config())
-            h = c_void_p()
-            check(self._lib.mhmr_create(ctypes.byref(cfg), ctypes.byref(h)), "mhmr_create")
-            self._handle = h
+            cfg = _lib.struct("mhmr_config", arch=ARCH_ID[self.backbone_name], img_size=self.img_size,
+                              max_batch=self.max_batch, max_persons=self.max_persons,
+                              refine_central=1 if self.refine_central else 0, **self._head_config())
+            h = torch.zeros(1, dtype=torch.int64)
+            call("mhmr_create", cfg, h)
+            self._handle = h.item()
             for k, v in self._state.items():
                 if k == self._POS_EMBED_KEY:
                     v = interpolate_pos_embed(v.cpu(), self.res)
@@ -180,7 +170,7 @@ class _EngineModel:
                     continue
                 self._set_weight(k, v)
             self._upload_extras()
-            check(self._lib.mhmr_finalize(self._handle), "mhmr_finalize")
+            call("mhmr_finalize", self._handle)
         self._finalized = True
         return self
 
@@ -224,37 +214,35 @@ class _EngineModel:
         number of persons."""
         if isinstance(det_thresh, list):
             det_thresh = det_thresh[0]                                               # model.py:614-615
-        o = self._OUT_STRUCT(*[ptr(t[n]).value if t[n] is not None else None for n, _ in self._OUT_STRUCT._fields_])
+        o = _lib.struct(self._OUTPUTS, **t)
         fP = 0
         if fidx is not None:
             fP = int(fidx.shape[1])
             fidx = fidx.to(self.device).contiguous()
-        stream = c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-        args = (ptr(K), c_int(x.shape[0]), ctypes.c_float(float(det_thresh)), c_int(int(nms_kernel_size)), ptr(fidx),
-                c_int(fP), ctypes.byref(o), stream)
+        s = stream(self.device)
+        args = (K, x.shape[0], float(det_thresh), int(nms_kernel_size), fidx, fP, o, s)
         if fused:
             from .preprocess import device_table
-            entry = self._ENTRY + "_u8"
-            check(getattr(self._lib, entry)(self._handle, ptr(x), ptr(device_table(self.device)), *args), entry)
+            call(self._ENTRY + "_u8", self._handle, x, device_table(self.device), *args)
         else:
-            check(getattr(self._lib, self._ENTRY)(self._handle, ptr(x), *args), self._ENTRY)
-        n = c_int(0)
-        check(self._lib.mhmr_sync_count(self._handle, stream, ctypes.byref(n)), "mhmr_sync_count")
+            call(self._ENTRY, self._handle, x, *args)
+        n = torch.zeros(1, dtype=torch.int32)
+        call("mhmr_sync_count", self._handle, s, n)
         self.last_outputs = t
-        return int(n.value)
+        return n.item()
 
     def last_launch_count(self) -> int:
-        return int(self._lib.mhmr_last_launch_count(self._handle))
+        return call("mhmr_last_launch_count", self._handle)
 
     def set_profiling(self, enable: bool):
         self.finalize()
-        check(self._lib.mhmr_set_profiling(self._handle, c_int(1 if enable else 0)), "mhmr_set_profiling")
+        call("mhmr_set_profiling", self._handle, 1 if enable else 0)
 
     def get_profile(self) -> dict:
         """{category: (device ms summed over launches, launches)} since profiling was enabled / last read."""
         n = len(self.PROFILE_CATEGORIES)
-        ms, cnt = (ctypes.c_float * n)(), (ctypes.c_int * n)()
-        check(self._lib.mhmr_get_profile(self._handle, ms, cnt), "mhmr_get_profile")
+        ms, cnt = torch.zeros(n), torch.zeros(n, dtype=torch.int32)
+        call("mhmr_get_profile", self._handle, ms, cnt)
         return {c: (float(ms[i]), int(cnt[i])) for i, c in enumerate(self.PROFILE_CATEGORIES)}
 
 
@@ -266,7 +254,7 @@ class Model(_EngineModel):
     _POS_EMBED_KEY = "backbone.encoder.pos_embed"
     _SKIPPED_KEYS = ("backbone.encoder.mask_token", "x_attention_head.init_betas_kid", "x_attention_head.init_expression")
     _ENTRY = "mhmr_forward"
-    _OUT_STRUCT = _Outputs
+    _OUTPUTS = "mhmr_outputs"
 
     def __init__(self, backbone="dinov2_vitb14", pretrained_backbone=False, img_size=896,
                  camera_embedding="geometric", camera_embedding_num_bands=16,
@@ -309,7 +297,7 @@ class Model(_EngineModel):
     # ------------------------------------------------------------------ load-time packing
     def _set_table(self, key, t):
         t = t.detach().to(torch.int32).contiguous().cpu()
-        check(self._lib.mhmr_set_table_i32(self._handle, key.encode(), ptr(t), c_int64(t.numel())), f"set_table({key})")
+        call("mhmr_set_table_i32", self._handle, key.encode(), t, t.numel())
 
     def finalize(self):
         if not self._finalized and not hasattr(self, "_bm"):
@@ -406,8 +394,7 @@ class Model(_EngineModel):
         B = x.shape[0]
         z = torch.empty(B, self.res * self.res, self.embed_dim, device=self.device)
         with torch.cuda.device(self.device):
-            stream = c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-            check(self._lib.mhmr_vit_forward(self._handle, ptr(x), c_int(B), ptr(z), stream), "mhmr_vit_forward")
+            call("mhmr_vit_forward", self._handle, x, B, z, stream(self.device))
         return z
 
     def smplx(self, rotvec, shape, loc, dist, K, expression, want_v2d=True):
@@ -440,12 +427,8 @@ class Model(_EngineModel):
         g = lambda t: None if t is None else t.to(dev, torch.float32).contiguous()
         d = [torch.empty_like(t) for t in (rotvec, shape, loc, dist, expression)]
         with torch.cuda.device(dev):
-            stream = c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            check(self._lib.mhmr_smplx_backward(self._handle, c_int(P), ptr(rotvec), ptr(shape), ptr(expression),
-                                                ptr(loc), ptr(dist), ptr(K), ptr(g(g_v3d)), ptr(g(g_v2d)),
-                                                ptr(g(g_j3d)), ptr(g(g_j2d)), ptr(g(g_transl)),
-                                                ptr(g(g_transl_pelvis)), ptr(d[0]), ptr(d[1]), ptr(d[4]), ptr(d[2]),
-                                                ptr(d[3]), stream), "mhmr_smplx_backward")
+            call("mhmr_smplx_backward", self._handle, P, rotvec, shape, expression, loc, dist, K, g(g_v3d), g(g_v2d),
+                 g(g_j3d), g(g_j2d), g(g_transl), g(g_transl_pelvis), d[0], d[1], d[4], d[2], d[3], stream(dev))
         return tuple(d)
 
     def _smplx_forward(self, rotvec, shape, loc, dist, K, expression, want_v2d=True):
@@ -455,11 +438,8 @@ class Model(_EngineModel):
         out = {"v3d": f(P, V, 3), "v2d": f(P, V, 2) if want_v2d else None, "j3d": f(P, 127, 3), "j2d": f(P, 127, 2),
                "transl": f(P, 3), "transl_pelvis": f(P, 3)}
         with torch.cuda.device(dev):
-            stream = c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            check(self._lib.mhmr_smplx_forward(self._handle, c_int(P), ptr(rotvec), ptr(shape), ptr(expression),
-                                               ptr(loc), ptr(dist), ptr(K), ptr(out["v3d"]), ptr(out["v2d"]),
-                                               ptr(out["j3d"]), ptr(out["j2d"]), ptr(out["transl"]),
-                                               ptr(out["transl_pelvis"]), stream), "mhmr_smplx_forward")
+            call("mhmr_smplx_forward", self._handle, P, rotvec, shape, expression, loc, dist, K, out["v3d"], out["v2d"],
+                 out["j3d"], out["j2d"], out["transl"], out["transl_pelvis"], stream(dev))
         out["transl_pelvis"] = out["transl_pelvis"][:, None]
         return out
 

@@ -9,21 +9,13 @@ after it (centre bone, translation, projection) runs in the sm_90a kernels behin
 """
 from __future__ import annotations
 
-import ctypes
-
 import torch
 
-from ._lib import c_int, c_void_p, check, ptr
+from ._lib import call, stream
 from .model import ARCH_ID, PATCH_SIZE, _EngineModel
 
 ANNY_SHAPE_KEYS = ("age", "gender", "weight", "height", "muscle", "proportions")   # multi_hmr.py:171
-_OUT_FIELDS = ("scores_map", "logits", "count", "det_idx", "K_regressed", "fov", "K_det", "offset", "loc", "dist",
-               "dist_pp", "shape", "rotmat", "rotmat_homo", "rotvec", "transl", "z")
 HEAD_ANNY = 1
-
-
-class _AnnyOutputs(ctypes.Structure):
-    _fields_ = [(n, c_void_p) for n in _OUT_FIELDS]
 
 
 def create_anny_body_model():
@@ -44,7 +36,7 @@ class ModelAnny(_EngineModel):
     _POS_EMBED_KEY = "encoder.backbone.pos_embed"
     _SKIPPED_KEYS = ("encoder.backbone.mask_token", "eye")
     _ENTRY = "mhmr_forward_anny"
-    _OUT_STRUCT = _AnnyOutputs
+    _OUTPUTS = "mhmr_anny_outputs"
 
     def __init__(self, img_size=896, backbone="dinov2_vits14", pretrained_backbone=False, xat_dim=512, xat_depth=8,
                  xat_heads=16, xat_dim_head=32, xat_mlp_dim=4 * 512, xat_dropout=0.0, person_center="head",
@@ -112,10 +104,8 @@ class ModelAnny(_EngineModel):
         res = {"v3d": v3d, "j3d": f(P, J, 3), "j2d": f(P, J, 2), "v2d": f(P, V, 2) if want_v2d else None,
                "transl_pelvis": f(P, 3)}
         with torch.cuda.device(dev):
-            stream = c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            check(self._lib.mhmr_anny_place(self._handle, c_int(P), c_int(V), ptr(bones), ptr(t["transl"]),
-                                            ptr(t["K_det"]), ptr(v3d), ptr(res["j3d"]), ptr(res["v2d"]),
-                                            ptr(res["j2d"]), ptr(res["transl_pelvis"]), stream), "mhmr_anny_place")
+            call("mhmr_anny_place", self._handle, P, V, bones, t["transl"], t["K_det"], v3d, res["j3d"], res["v2d"],
+                 res["j2d"], res["transl_pelvis"], stream(dev))
         return res
 
     def forward(self, x, K=None, idx=None, is_training=False, det_thresh=0.3, nms_kernel_size=3, *args, **kwargs):

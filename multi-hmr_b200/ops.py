@@ -7,8 +7,7 @@ from __future__ import annotations
 
 import torch
 
-from . import _lib
-from ._lib import c_float, c_int, c_int64, check, ptr, stream_ptr
+from ._lib import call, stream
 
 EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RELU_F16, EPI_LS_RESID_F32, EPI_ROWADD_F32, EPI_BIAS_F32 = range(6)
 
@@ -27,12 +26,8 @@ def gemm_f16(a, w, epilogue, out, bias=None, gamma=None, rowadd=None, rows_in=0,
     assert a.stride(1) == 1 and w.stride(1) == 1 and out.stride(1) == 1
     M, K = a.shape
     N = w.shape[0]
-    lib = _lib.load()
-    rc = lib.mhmr_op_gemm_f16(ptr(a), c_int64(a.stride(0)), ptr(w), c_int64(w.stride(0)), c_int(M), c_int(N),
-                              c_int(K), c_int(epilogue), ptr(bias), ptr(gamma), ptr(rowadd), ptr(out),
-                              c_int64(out.stride(0)), c_int(rows_in), c_int(rows_out), c_int(row_off),
-                              c_int(block_n), stream_ptr())
-    check(rc, "mhmr_op_gemm_f16")
+    call("mhmr_op_gemm_f16", a, a.stride(0), w, w.stride(0), M, N, K, epilogue, bias, gamma, rowadd, out, out.stride(0),
+         rows_in, rows_out, row_off, block_n, stream())
     return out
 
 
@@ -47,11 +42,8 @@ def resid_ln_linear_f16(a, wp, bp, ls, x, ln_g, ln_b, w, b, gelu=False):
     N = w.shape[0]
     assert x.shape == (M, D) and w.shape == (N, D)
     out = torch.empty(M, N, device=a.device, dtype=torch.float16)
-    rc = _lib.load().mhmr_op_resid_ln_linear_f16(
-        ptr(a), c_int64(a.stride(0)), ptr(wp), c_int64(wp.stride(0)), ptr(bp), ptr(ls), ptr(x), c_int(M), c_int(D),
-        c_int(Ka), ptr(ln_g), ptr(ln_b), ptr(w), ptr(b), c_int(N), c_int(1 if gelu else 0), ptr(out),
-        c_int64(out.stride(0)), stream_ptr())
-    check(rc, "mhmr_op_resid_ln_linear_f16")
+    call("mhmr_op_resid_ln_linear_f16", a, a.stride(0), wp, wp.stride(0), bp, ls, x, M, D, Ka, ln_g, ln_b, w, b, N,
+         1 if gelu else 0, out, out.stride(0), stream())
     return out
 
 
@@ -62,8 +54,7 @@ def normalize_u8(img_u8, lut):
     assert lut.dtype == torch.float32 and tuple(lut.shape) == (3, 256) and lut.is_contiguous()
     B, H, W, _ = img_u8.shape
     out = torch.empty(B, 3, H, W, device=img_u8.device, dtype=torch.float32)
-    rc = _lib.load().mhmr_op_normalize_u8(ptr(img_u8), ptr(lut), ptr(out), c_int(B), c_int(H), c_int(W), stream_ptr())
-    check(rc, "mhmr_op_normalize_u8")
+    call("mhmr_op_normalize_u8", img_u8, lut, out, B, H, W, stream())
     return out
 
 
@@ -73,10 +64,7 @@ def attention(qkv, B, T, D, out=None):
     assert qkv.dtype == torch.float16 and qkv.shape == (B * T, 3 * D) and qkv.stride(1) == 1
     if out is None:
         out = torch.empty(B * T, D, device=qkv.device, dtype=torch.float16)
-    lib = _lib.load()
-    rc = lib.mhmr_op_attention(ptr(qkv), c_int64(qkv.stride(0)), ptr(out), c_int64(out.stride(0)), c_int(B),
-                               c_int(T), c_int(D), stream_ptr())
-    check(rc, "mhmr_op_attention")
+    call("mhmr_op_attention", qkv, qkv.stride(0), out, out.stride(0), B, T, D, stream())
     return out
 
 
@@ -99,11 +87,8 @@ def skinny_linear(x, count, max_persons, K, w, out, bias=None, ln=None, act=0, r
     _f32(x, w, out, bias, resid)
     _i32(count)
     g, b, eps = ln if ln is not None else (None, None, 0.0)
-    rc = _lib.load().mhmr_op_skinny_linear(
-        ptr(x), c_int(x.stride(0)), ptr(count), c_int(max_persons), c_int(K), ptr(w), c_int(w.stride(0)), ptr(bias),
-        c_int(w.shape[0]), ptr(g), ptr(b), c_float(eps), c_int(act), ptr(resid),
-        c_int(resid.stride(0) if resid is not None else 0), ptr(out), c_int(out.stride(0)), c_int(cols), stream_ptr())
-    check(rc, "mhmr_op_skinny_linear")
+    call("mhmr_op_skinny_linear", x, x.stride(0), count, max_persons, K, w, w.stride(0), bias, w.shape[0], g, b, eps,
+         act, resid, resid.stride(0) if resid is not None else 0, out, out.stride(0), cols, stream())
     return out
 
 
@@ -114,9 +99,8 @@ def hph_self_attn(qkv, det_b, img_off, count, max_persons, heads, out=None):
     _i32(det_b, img_off, count)
     if out is None:
         out = torch.zeros(max_persons, heads * 32, device=qkv.device)
-    rc = _lib.load().mhmr_op_hph_self_attn(ptr(qkv), c_int(qkv.stride(0)), ptr(det_b), ptr(img_off), ptr(count),
-                                           c_int(max_persons), c_int(heads), ptr(out), c_int(out.stride(0)), stream_ptr())
-    check(rc, "mhmr_op_hph_self_attn")
+    call("mhmr_op_hph_self_attn", qkv, qkv.stride(0), det_b, img_off, count, max_persons, heads, out, out.stride(0),
+         stream())
     return out
 
 
@@ -127,10 +111,8 @@ def hph_cross_attn(q, kv, k_col, v_col, det_b, count, max_persons, heads, N, out
     _i32(det_b, count)
     if out is None:
         out = torch.zeros(max_persons, heads * 32, device=q.device)
-    rc = _lib.load().mhmr_op_hph_cross_attn(ptr(q), c_int(q.stride(0)), ptr(kv), c_int64(kv.stride(0)), c_int(k_col),
-                                            c_int(v_col), ptr(det_b), ptr(count), c_int(max_persons), c_int(heads),
-                                            c_int(N), ptr(out), c_int(out.stride(0)), stream_ptr())
-    check(rc, "mhmr_op_hph_cross_attn")
+    call("mhmr_op_hph_cross_attn", q, q.stride(0), kv, kv.stride(0), k_col, v_col, det_b, count, max_persons, heads, N,
+         out, out.stride(0), stream())
     return out
 
 
@@ -147,10 +129,9 @@ def detect(scores, nms_k, thresh, max_persons):
          "det_score": torch.full((cap,), -1.0, device=dev), "count": torch.full((1,), -1, dtype=torch.int32, device=dev),
          "count_clamped": torch.full((1,), -1, dtype=torch.int32, device=dev),
          "img_off": torch.full((B + 1,), -1, dtype=torch.int32, device=dev)}
-    rc = _lib.load().mhmr_op_detect(ptr(scores), c_int(B), c_int(res), c_int(nms_k), c_float(thresh), c_int(max_persons),
-                                    *(ptr(o[k]) for k in ("scores_out", "det_b", "det_y", "det_x", "det_score", "count",
-                                                          "count_clamped", "img_off")), stream_ptr())
-    check(rc, "mhmr_op_detect")
+    call("mhmr_op_detect", scores, B, res, nms_k, thresh, max_persons,
+         *(o[k] for k in ("scores_out", "det_b", "det_y", "det_x", "det_score", "count", "count_clamped", "img_off")),
+         stream())
     return o
 
 
@@ -169,12 +150,10 @@ def person_post(dec, num_betas, offset, K, det_b, det_y, det_x, count, max_perso
     o = {"rotmat": _zeros(dev, Pm, 53, 3, 3), "rotvec": _zeros(dev, Pm, 53, 3), "shape": _zeros(dev, Pm, num_betas),
          "expression": _zeros(dev, Pm, 10), "dist_pp": _zeros(dev, Pm), "dist": _zeros(dev, Pm),
          "loc": _zeros(dev, Pm, 2), "transl": _zeros(dev, Pm, 3), "K_det": _zeros(dev, Pm, 3, 3)}
-    rc = _lib.load().mhmr_op_person_post(
-        ptr(dec), c_int(dec.stride(0)), c_int(num_betas), ptr(offset), ptr(K),
-        c_int(K.shape[0]), ptr(det_b), ptr(det_y), ptr(det_x), ptr(count), c_int(Pm), c_float(focal_norm),
-        *(ptr(o[k]) for k in ("rotmat", "rotvec", "shape", "expression", "dist_pp", "dist", "loc", "transl", "K_det")),
-        stream_ptr())
-    check(rc, "mhmr_op_person_post")
+    call("mhmr_op_person_post", dec, dec.stride(0), num_betas, offset, K, K.shape[0], det_b, det_y, det_x, count, Pm,
+         focal_norm,
+         *(o[k] for k in ("rotmat", "rotvec", "shape", "expression", "dist_pp", "dist", "loc", "transl", "K_det")),
+         stream())
     return o
 
 
@@ -192,13 +171,9 @@ def anny_person_post(hid, w2, b2, fov_max, K, img_size, rot6d, J, useful, shape,
     o = {"fov": _zeros(dev, B), "K_regressed": _zeros(dev, B, 3, 3), "K_use": _zeros(dev, B, 3, 3),
          "rotmat": _zeros(dev, Pm, J, 3, 3), "rotmat_homo": _zeros(dev, Pm, J, 4, 4), "rotvec": _zeros(dev, Pm, J, 3),
          "dist": _zeros(dev, Pm), "loc": _zeros(dev, Pm, 2), "transl": _zeros(dev, Pm, 3), "K_det": _zeros(dev, Pm, 3, 3)}
-    rc = _lib.load().mhmr_op_anny_person_post(
-        ptr(hid), c_int(D), ptr(w2), ptr(b2), ptr(fov_max), ptr(K), c_int(B),
-        c_int(img_size), ptr(o["fov"]), ptr(o["K_regressed"]), ptr(o["K_use"]), ptr(rot6d), c_int(rot6d.stride(0)),
-        c_int(J), ptr(useful), ptr(shape), c_int(shape.shape[1]), ptr(offset), ptr(dist_pp),
-        ptr(det_b), ptr(det_y), ptr(det_x), ptr(count), c_int(Pm),
-        *(ptr(o[k]) for k in ("rotmat", "rotmat_homo", "rotvec", "dist", "loc", "transl", "K_det")), stream_ptr())
-    check(rc, "mhmr_op_anny_person_post")
+    call("mhmr_op_anny_person_post", hid, D, w2, b2, fov_max, K, B, img_size, o["fov"], o["K_regressed"], o["K_use"],
+         rot6d, rot6d.stride(0), J, useful, shape, shape.shape[1], offset, dist_pp, det_b, det_y, det_x, count, Pm,
+         *(o[k] for k in ("rotmat", "rotmat_homo", "rotvec", "dist", "loc", "transl", "K_det")), stream())
     o["shape"] = shape
     return o
 
@@ -215,10 +190,7 @@ def refine_chain(layers, o16, rowidx, count, x):
     assert all(layers[k].is_contiguous() for k in keys)
     depth, R, D = o16.shape
     assert x.shape[1] == D and rowidx.shape[0] >= x.shape[0]
-    rc = _lib.load().mhmr_op_refine_chain(c_int(depth), c_int(D), ptr(count), c_int(x.shape[0]),
-                                          *(ptr(layers[k]) for k in keys), ptr(o16), c_int64(R), ptr(rowidx), ptr(x),
-                                          stream_ptr())
-    check(rc, "mhmr_op_refine_chain")
+    call("mhmr_op_refine_chain", depth, D, count, x.shape[0], *(layers[k] for k in keys), o16, R, rowidx, x, stream())
     return x
 
 
@@ -240,9 +212,7 @@ def im2col_patch14(img, A, lut=None):
     u8 = img.dtype == torch.uint8
     assert (lut is not None) == u8 and (img.dtype == torch.float32 or u8)
     B, S = img.shape[0], img.shape[2] if u8 else img.shape[3]
-    rc = _lib.load().mhmr_op_im2col_patch14(ptr(None if u8 else img), ptr(img if u8 else None), ptr(lut), c_int(B),
-                                            c_int(S), ptr(A), c_int(A.stride(0)), stream_ptr())
-    check(rc, "mhmr_op_im2col_patch14")
+    call("mhmr_op_im2col_patch14", None if u8 else img, img if u8 else None, lut, B, S, A, A.stride(0), stream())
     return A
 
 
@@ -255,11 +225,8 @@ def layernorm(x, gamma, beta, out16=None, out32=None, eps=1e-6, rows_in=0, skip=
     for o in (out16, out32):
         assert o is None or o.stride(1) == 1
     M, D = x.shape
-    rc = _lib.load().mhmr_op_layernorm(ptr(x), ptr(xlo), ptr(gamma), ptr(beta), ptr(out16),
-                                       c_int64(out16.stride(0) if out16 is not None else 0), ptr(out32),
-                                       c_int64(out32.stride(0) if out32 is not None else 0), c_int(M), c_int(D),
-                                       c_float(eps), c_int(rows_in), c_int(skip), stream_ptr())
-    check(rc, "mhmr_op_layernorm")
+    call("mhmr_op_layernorm", x, xlo, gamma, beta, out16, out16.stride(0) if out16 is not None else 0, out32,
+         out32.stride(0) if out32 is not None else 0, M, D, eps, rows_in, skip, stream())
 
 
 def split_rowstats(x, hi, lo, stats):
@@ -268,9 +235,7 @@ def split_rowstats(x, hi, lo, stats):
     _contig(x, stats)
     assert hi.dtype == lo.dtype == torch.float16 and hi.stride() == lo.stride() and hi.stride(1) == 1
     M, D = x.shape
-    rc = _lib.load().mhmr_op_split_rowstats(ptr(x), ptr(hi), ptr(lo), c_int64(hi.stride(0)), ptr(stats),
-                                            c_int(stats.shape[1]), c_int(M), c_int(D), stream_ptr())
-    check(rc, "mhmr_op_split_rowstats")
+    call("mhmr_op_split_rowstats", x, hi, lo, hi.stride(0), stats, stats.shape[1], M, D, stream())
 
 
 def fold_ln_linear(w, bias, ln_g, ln_b):
@@ -280,9 +245,7 @@ def fold_ln_linear(w, bias, ln_g, ln_b):
     N, K = w.shape
     w16 = torch.empty(N, K, device=w.device, dtype=torch.float16)
     b2 = torch.empty(N, device=w.device)
-    rc = _lib.load().mhmr_op_fold_ln_linear(ptr(w), ptr(bias), ptr(ln_g), ptr(ln_b), ptr(w16), ptr(b2), c_int(N),
-                                            c_int(K), stream_ptr())
-    check(rc, "mhmr_op_fold_ln_linear")
+    call("mhmr_op_fold_ln_linear", w, bias, ln_g, ln_b, w16, b2, N, K, stream())
     return w16, b2
 
 
@@ -298,13 +261,10 @@ def gemm_internal(a, w, epilogue, block_n, out=None, bias=None, gamma=None, hi=N
     assert hi is None or (hi.dtype == lo.dtype == torch.float16 and hi.stride() == lo.stride() and hi.stride(1) == 1)
     M, K = a.shape
     N = w.shape[0]
-    rc = _lib.load().mhmr_op_gemm_internal(
-        ptr(a), c_int64(a.stride(0)), ptr(w), c_int64(w.stride(0)), c_int(M), c_int(N), c_int(K), c_int(epilogue),
-        ptr(bias), ptr(gamma), ptr(hi), ptr(lo), c_int64(hi.stride(0) if hi is not None else 0), ptr(stats),
-        c_int(stats.shape[1] if stats is not None else 0), ptr(rowadd), c_int(rows_in), c_int(rows_out),
-        c_int(row_off), ptr(out), c_int64(out.stride(0) if out is not None else 0), c_int(block_n),
-        c_int(0 if m_run is None else m_run), stream_ptr())
-    check(rc, "mhmr_op_gemm_internal")
+    call("mhmr_op_gemm_internal", a, a.stride(0), w, w.stride(0), M, N, K, epilogue, bias, gamma, hi, lo,
+         hi.stride(0) if hi is not None else 0, stats, stats.shape[1] if stats is not None else 0, rowadd, rows_in,
+         rows_out, row_off, out, out.stride(0) if out is not None else 0, block_n, 0 if m_run is None else m_run,
+         stream())
     return out
 
 
@@ -315,9 +275,7 @@ def camera_ctx(K, freqs, ctx, res, col0, pad_cols):
     assert ctx.dtype == torch.float16 and ctx.stride(1) == 1
     B = K.shape[0]
     kinv = torch.empty(B, 3, 3, device=K.device)
-    rc = _lib.load().mhmr_op_camera_ctx(ptr(K), c_int(B), ptr(freqs), ptr(kinv), ptr(ctx), c_int64(ctx.stride(0)),
-                                        c_int(res), c_int(col0), c_int(pad_cols), stream_ptr())
-    check(rc, "mhmr_op_camera_ctx")
+    call("mhmr_op_camera_ctx", K, B, freqs, kinv, ctx, ctx.stride(0), res, col0, pad_cols, stream())
     return kinv
 
 
@@ -326,9 +284,8 @@ def rowdot_sigmoid(hid, D, w, b, scores, logits=None, clamp=True):
     _cuda(hid, w, b, scores, logits)
     _contig(w, b, scores, logits)
     assert hid.dtype == torch.float16 and hid.stride(1) == 1
-    rc = _lib.load().mhmr_op_rowdot_sigmoid(ptr(hid), c_int64(hid.stride(0)), ptr(w), ptr(b), ptr(scores), ptr(logits),
-                                            c_int(1 if clamp else 0), c_int(scores.numel()), c_int(D), stream_ptr())
-    check(rc, "mhmr_op_rowdot_sigmoid")
+    call("mhmr_op_rowdot_sigmoid", hid, hid.stride(0), w, b, scores, logits, 1 if clamp else 0, scores.numel(), D,
+         stream())
 
 
 def person_gather(z32, kinv, freqs, cq_x, cq_y, cv_x, cv_y, det_b, det_y, det_x, count, max_persons, res, zc, query,
@@ -340,11 +297,8 @@ def person_gather(z32, kinv, freqs, cq_x, cq_y, cv_x, cv_y, det_b, det_y, det_x,
     _i32(det_b, det_y, det_x, count)
     assert query.stride() == vals.stride()
     D = z32.shape[-1]
-    rc = _lib.load().mhmr_op_person_gather(
-        ptr(z32), ptr(xr), ptr(norm[0]), ptr(norm[1]), ptr(kinv), ptr(freqs), ptr(cq_x), ptr(cq_y), ptr(cv_x),
-        ptr(cv_y), ptr(det_b), ptr(det_y), ptr(det_x), ptr(count), c_int(max_persons), c_int(res), c_int(D), ptr(zc),
-        ptr(query), ptr(vals), c_int(query.stride(0)), stream_ptr())
-    check(rc, "mhmr_op_person_gather")
+    call("mhmr_op_person_gather", z32, xr, norm[0], norm[1], kinv, freqs, cq_x, cq_y, cv_x, cv_y, det_b, det_y, det_x,
+         count, max_persons, res, D, zc, query, vals, query.stride(0), stream())
 
 
 def refine_prepare(img, rowadd, det_b, det_y, det_x, count, max_persons, rowidx, patch, xr, lut=None, n_cls=0,
@@ -357,11 +311,8 @@ def refine_prepare(img, rowadd, det_b, det_y, det_x, count, max_persons, rowidx,
     assert patch.stride(1) == 1
     u8 = img.dtype == torch.uint8
     S = img.shape[2] if u8 else img.shape[3]
-    rc = _lib.load().mhmr_op_refine_prepare(
-        ptr(None if u8 else img), ptr(img if u8 else None), ptr(lut), c_int(S), ptr(rowadd), c_int(xr.shape[1]),
-        ptr(det_b), ptr(det_y), ptr(det_x), ptr(count), c_int(max_persons), c_int(n_cls), ptr(cls_pos), ptr(rows_out),
-        ptr(rowidx), ptr(patch), c_int(patch.stride(0)), ptr(xr), stream_ptr())
-    check(rc, "mhmr_op_refine_prepare")
+    call("mhmr_op_refine_prepare", None if u8 else img, img if u8 else None, lut, S, rowadd, xr.shape[1], det_b, det_y,
+         det_x, count, max_persons, n_cls, cls_pos, rows_out, rowidx, patch, patch.stride(0), xr, stream())
 
 
 def kv_add_rows(kv, dkv, det_b, det_y, det_x, count, max_persons, res):
@@ -370,10 +321,8 @@ def kv_add_rows(kv, dkv, det_b, det_y, det_x, count, max_persons, res):
     _f32(kv, dkv)
     _contig(dkv)
     _i32(det_b, det_y, det_x, count)
-    rc = _lib.load().mhmr_op_kv_add_rows(ptr(kv), c_int64(kv.stride(0)), ptr(dkv), c_int(dkv.shape[1]), ptr(det_b),
-                                         ptr(det_y), ptr(det_x), ptr(count), c_int(max_persons), c_int(res),
-                                         stream_ptr())
-    check(rc, "mhmr_op_kv_add_rows")
+    call("mhmr_op_kv_add_rows", kv, kv.stride(0), dkv, dkv.shape[1], det_b, det_y, det_x, count, max_persons, res,
+         stream())
 
 
 def cls_gather(x, T, B, D, xlo=None):
@@ -381,9 +330,7 @@ def cls_gather(x, T, B, D, xlo=None):
     _cuda(x, xlo)
     assert x.stride(1) == 1 and (xlo is None or xlo.stride() == x.stride())
     out = torch.empty(B, D, device=x.device)
-    rc = _lib.load().mhmr_op_cls_gather(ptr(x), ptr(xlo), c_int64(x.stride(0)), c_int(T), c_int(B), c_int(D), ptr(out),
-                                        stream_ptr())
-    check(rc, "mhmr_op_cls_gather")
+    call("mhmr_op_cls_gather", x, xlo, x.stride(0), T, B, D, out, stream())
     return out
 
 
@@ -396,8 +343,7 @@ def vit_stream(model, x, layers):
     B = x.shape[0]
     out = torch.empty(B, 1 + model.res * model.res, model.embed_dim, device=model.device)
     with torch.cuda.device(model.device):
-        rc = _lib.load().mhmr_op_vit_stream(model._handle, ptr(x), c_int(B), c_int(layers), ptr(out), stream_ptr())
-    check(rc, "mhmr_op_vit_stream")
+        call("mhmr_op_vit_stream", model._handle, x, B, layers, out, stream())
     return out
 
 
@@ -406,10 +352,8 @@ def anny_gather(z32, pos, det_b, det_y, det_x, count, max_persons, res, zc, xa, 
     _cuda(z32, pos, zc, xa, xr, *norm)
     _contig(z32, pos, zc, xa, xr, *norm)
     _i32(det_b, det_y, det_x, count)
-    rc = _lib.load().mhmr_op_anny_gather(ptr(z32), ptr(xr), ptr(norm[0]), ptr(norm[1]), ptr(pos), ptr(det_b),
-                                         ptr(det_y), ptr(det_x), ptr(count), c_int(max_persons), c_int(res),
-                                         c_int(z32.shape[-1]), c_int(xa.shape[1]), ptr(zc), ptr(xa), stream_ptr())
-    check(rc, "mhmr_op_anny_gather")
+    call("mhmr_op_anny_gather", z32, xr, norm[0], norm[1], pos, det_b, det_y, det_x, count, max_persons, res,
+         z32.shape[-1], xa.shape[1], zc, xa, stream())
 
 
 def anny_place(bone_poses, transl, K_det, center, v3d, j3d, j2d, transl_pelvis, v2d=None):
@@ -418,7 +362,4 @@ def anny_place(bone_poses, transl, K_det, center, v3d, j3d, j2d, transl_pelvis, 
     _contig(bone_poses, transl, K_det, v3d, j3d, j2d, transl_pelvis, v2d)
     P, J = bone_poses.shape[:2]
     V = v3d.shape[1]
-    rc = _lib.load().mhmr_op_anny_place(ptr(bone_poses), ptr(transl), ptr(K_det), c_int(center), c_int(P), c_int(V),
-                                        c_int(J), ptr(v3d), ptr(j3d), ptr(v2d), ptr(j2d), ptr(transl_pelvis),
-                                        stream_ptr())
-    check(rc, "mhmr_op_anny_place")
+    call("mhmr_op_anny_place", bone_poses, transl, K_det, center, P, V, J, v3d, j3d, v2d, j2d, transl_pelvis, stream())

@@ -12,6 +12,9 @@ from __future__ import annotations
 import torch
 import torch.distributed as dist
 
+from . import _lib
+from ._lib import call
+
 # per-person record layout (fp32): [global image index, score, loc(2), transl(3), transl_pelvis(3),
 # rotvec(159), expression(10), shape(nb), v3d(3V), j3d(381), j2d(254)]
 FIELDS = (("img", 1), ("scores", 1), ("loc", 2), ("transl", 3), ("transl_pelvis", 3), ("rotvec", 159),
@@ -112,26 +115,16 @@ class RecordGather:
 
     # ---- CUDA path -------------------------------------------------------------------------------
     def _init_cuda(self):
-        import ctypes
-
-        from . import _lib
-        self._ct, self._lib_mod = ctypes, _lib
-        self.lib = _lib.load()
-        self.lib.mhmr_record_block_bytes.restype = ctypes.c_int64
         dev = self.model.device
         uid = torch.zeros(128, dtype=torch.uint8)
         if self.rank == 0:
-            buf = (ctypes.c_char * 128)()
-            _lib.check(self.lib.mhmr_nccl_unique_id(buf), "mhmr_nccl_unique_id")
-            uid = torch.frombuffer(bytearray(buf.raw), dtype=torch.uint8).clone()
+            call("mhmr_nccl_unique_id", uid)
         uid = uid.to(dev)
         dist.broadcast(uid, src=0, group=self.group)
-        raw = bytes(uid.cpu().numpy().tobytes())
-        comm = ctypes.c_void_p()
+        comm = torch.zeros(1, dtype=torch.int64)
         with torch.cuda.device(dev):
-            _lib.check(self.lib.mhmr_comm_create(raw, ctypes.c_int(self.world), ctypes.c_int(self.rank),
-                                                 ctypes.byref(comm)), "mhmr_comm_create")
-        self._comm = comm
+            call("mhmr_comm_create", uid.cpu(), self.world, self.rank, comm)
+        self._comm = comm.item()
         self.stream = torch.cuda.Stream(device=dev)
         self._bufs = {}
 
@@ -143,17 +136,12 @@ class RecordGather:
         return self._bufs[capacity]
 
     def _enqueue_cuda(self, t, img_offset, capacity):
-        from .model import _OUT_FIELDS, _Outputs
-        ct, lib, check = self._ct, self.lib, self._lib_mod.check
         block, out = self._buffers(capacity)
-        o = _Outputs(*[ct.c_void_p(t[n].data_ptr()) if t.get(n) is not None else None for n in _OUT_FIELDS])
-        sp = ct.c_void_p(self.stream.cuda_stream)
+        o = _lib.struct("mhmr_outputs", **t)
+        s = self.stream.cuda_stream
         with torch.cuda.device(self.model.device):
-            check(lib.mhmr_pack_records(ct.byref(o), ct.c_int(self.Pm), ct.c_int(self.nb), ct.c_int(self.V),
-                                        ct.c_int(img_offset), ct.c_int(capacity), ct.c_void_p(block.data_ptr()), sp),
-                  "mhmr_pack_records")
-            check(lib.mhmr_allgather_records(self._comm, ct.c_void_p(block.data_ptr()), ct.c_void_p(out.data_ptr()),
-                                             ct.c_int64(block.numel() * 4), sp), "mhmr_allgather_records")
+            call("mhmr_pack_records", o, self.Pm, self.nb, self.V, img_offset, capacity, block, s)
+            call("mhmr_allgather_records", self._comm, block, out, block.numel() * 4, s)
         return out
 
     # ---- public ------------------------------------------------------------------------------------
@@ -198,7 +186,7 @@ class RecordGather:
     def close(self):
         if self._comm is not None:
             self.wait()
-            self.lib.mhmr_comm_destroy(self._comm)
+            _lib.load().mhmr_comm_destroy(self._comm)
             self._comm = None
 
 

@@ -16,15 +16,13 @@ its framebuffer; this renderer does not, so silhouette pixels can differ from a 
 from __future__ import annotations
 
 import colorsys
-import ctypes
 import hashlib
-from ctypes import c_int, c_void_p
 
 import numpy as np
 import torch
 
 from . import _lib
-from ._lib import check, ptr
+from ._lib import call, stream
 
 ZNEAR, ZFAR = 0.05, 100.0
 
@@ -40,10 +38,6 @@ def _palette(n: int = 40) -> list[tuple[float, float, float]]:
 
 
 PALETTE = _palette()
-
-
-def _stream(dev):
-    return c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _faces(faces) -> torch.Tensor:
@@ -153,27 +147,25 @@ class Renderer:
         self.topologies = topo
         self.topology_verts = [int(t.max()) + 1 for t in topo]
         self._lib = _lib.load()
-        h = c_void_p()
+        h = torch.zeros(1, dtype=torch.int64)
         with torch.cuda.device(dev):
             if topo:
                 tf = torch.cat(topo).contiguous()
                 nf = torch.tensor([t.shape[0] for t in topo], dtype=torch.int32)
                 nv = torch.tensor(self.topology_verts, dtype=torch.int32)
-                check(self._lib.mhmr_render_create_topologies(ptr(self.faces), self.num_faces, V, len(topo), ptr(tf),
-                                                              ptr(nf), ptr(nv), _stream(dev), ctypes.byref(h)),
-                      "mhmr_render_create_topologies")
+                call("mhmr_render_create_topologies", self.faces, self.num_faces, V, len(topo), tf, nf, nv,
+                     stream(dev), h)
             else:
-                check(self._lib.mhmr_render_create(ptr(self.faces), self.num_faces, V, _stream(dev),
-                                                   ctypes.byref(h)), "mhmr_render_create")
-        self._h = h
+                call("mhmr_render_create", self.faces, self.num_faces, V, stream(dev), h)
+        self._h = h.item()
         self._glyph = self._palette = None
-        fb = c_int()
-        check(self._lib.mhmr_render_info(h, None, None, ctypes.byref(fb)), "mhmr_render_info")
-        self.face_bits = fb.value
+        fb = torch.zeros(1, dtype=torch.int32)
+        call("mhmr_render_info", self._h, None, None, fb)
+        self.face_bits = fb.item()
 
     def __del__(self):
         h = getattr(self, "_h", None)
-        if h is not None and h.value:
+        if h:
             self._lib.mhmr_render_destroy(h)
             self._h = None
 
@@ -243,23 +235,20 @@ class Renderer:
         out = {"overlay": torch.empty(B, H, W, 3, dtype=torch.uint8, device=dev),
                "depth": torch.empty(B, H, W, dtype=torch.float32, device=dev) if depth else None,
                "index": torch.empty(B, H, W, dtype=torch.int32, device=dev) if index else None}
-        args = _lib.RenderArgs(B, H, W, images.data_ptr(), vi.data_ptr(), K.data_ptr(),
-                               pose.data_ptr() if pose is not None else None, verts.data_ptr(), Pm,
-                               person_image.data_ptr(), count.data_ptr(), colors.data_ptr(), float(alpha),
-                               float(intensity), float(metallic), float(roughness), int(bool(smooth)),
-                               out["overlay"].data_ptr(), out["depth"].data_ptr() if depth else None,
-                               out["index"].data_ptr() if index else None)
+        args = _lib.struct("mhmr_render_args", views=B, H=H, W=W, images=images, view_image=vi, K=K, pose=pose,
+                           verts=verts, max_persons=Pm, person_image=person_image, count=count, colors=colors,
+                           alpha=float(alpha), intensity=float(intensity), metallic=float(metallic),
+                           roughness=float(roughness), smooth=int(bool(smooth)), overlay=out["overlay"],
+                           depth=out["depth"], person=out["index"])
         with torch.cuda.device(dev):
             if extra is None:
-                check(self._lib.mhmr_render_forward(self._h, ctypes.byref(args), _stream(dev)),
-                      "mhmr_render_forward")
+                call("mhmr_render_forward", self._h, args, stream(dev))
             else:
-                check(self._lib.mhmr_render_forward_extra(self._h, ctypes.byref(args), ctypes.byref(extra[0]),
-                                                          _stream(dev)), "mhmr_render_forward_extra")
+                call("mhmr_render_forward_extra", self._h, args, extra[0], stream(dev))
         return {k: v for k, v in out.items() if v is not None}
 
     def _extra(self, B, N, props, prop_visible, view_alpha, view_background):
-        """(RenderExtra, tensors it points to).  props: [(topology, verts [V_t,3], colour)]."""
+        """(mhmr_render_extra, tensors it points to).  props: [(topology, verts [V_t,3], colour)]."""
         dev = self.device
         n = len(props)
         keep = []
@@ -289,8 +278,8 @@ class Renderer:
             if vb.shape[0] != B:
                 raise ValueError(f"view_background must hold {B} image indices")
         keep += [topo, pv, pc, vis, va, vb]
-        p = lambda t: t.data_ptr() if t is not None else None
-        return _lib.RenderExtra(n, topo.data_ptr(), p(pv), p(pc), p(vis), p(va), p(vb)), keep
+        return _lib.struct("mhmr_render_extra", num_props=n, prop_topology=topo, prop_verts=pv, prop_colors=pc,
+                           prop_visible=vis, view_alpha=va, view_background=vb), keep
 
     def glyph_props(self):
         """The device props of `camera_glyph()` for a renderer created with its topologies (the first three)."""
@@ -350,11 +339,11 @@ class Renderer:
         rank = torch.empty(Pm, dtype=torch.int32, device=dev)
         if side and P and tp is None:
             raise ValueError("the side views need t['transl_pelvis']")
-        pa = _lib.RenderPoseArgs(B, Pm, self.num_verts, count.data_ptr(), person_image.data_ptr(), verts.data_ptr(),
-                                 tp.data_ptr() if tp is not None else None, tr.data_ptr() if tr is not None else None,
-                                 nf, ar, int(bool(side)), pose.data_ptr(), nonempty.data_ptr(), rank.data_ptr())
+        pa = _lib.struct("mhmr_render_pose_args", images=B, max_persons=Pm, num_verts=self.num_verts, count=count,
+                         person_image=person_image, verts=verts, transl_pelvis=tp, transl=tr, n_frames=nf,
+                         angle_range=ar, side=int(bool(side)), pose=pose, nonempty=nonempty, rank=rank)
         with torch.cuda.device(dev):
-            check(self._lib.mhmr_render_view_poses(ctypes.byref(pa), _stream(dev)), "mhmr_render_view_poses")
+            call("mhmr_render_view_poses", pa, stream(dev))
         if colors is None:
             if self._palette is None:
                 self._palette = torch.tensor(PALETTE, dtype=torch.float32).to(dev)

@@ -1,7 +1,5 @@
 """CPU: the Anny variant's oracle restatement against the goldens of the unmodified reference, the synthetic Anny
 assets, and the validation of the Anny engine configuration."""
-import ctypes
-
 import pytest
 import torch
 
@@ -70,19 +68,20 @@ def test_sincos_table_layout():
 
 def test_create_validates_anny_config_without_gpu():
     from multihmr_b200 import _lib
-    from multihmr_b200.model import _Config
 
     lib = _lib.load()
-    h = ctypes.c_void_p()
+    h = torch.zeros(1, dtype=torch.int64)
+    base = dict(arch=0, img_size=224, max_batch=2, max_persons=8, xat_depth=8, xat_num_heads=16, num_betas=11,
+                person_center_idx=9, num_verts=0, refine_central=1, head=1, xat_dim=512, xat_mlp_dim=2048,
+                num_joints=163)
 
-    def rc(*fields):
-        return lib.mhmr_create(ctypes.byref(_Config(*fields)), ctypes.byref(h))
+    def rc(**change):
+        return lib.mhmr_create(_lib.struct("mhmr_config", **{**base, **change}), h)
 
-    base = [0, 224, 2, 8, 8, 16, 11, 9, 0, 1]
-    assert rc(*base, 1, 500, 2048, 163) == -2                         # xat_dim not a multiple of 32
-    assert rc(*base, 1, 512, 0, 163) == -2                            # no FeedForward width
-    assert rc(*base, 2, 512, 2048, 163) == -2                         # unknown head kind
-    assert rc(*base[:7], 163, 0, 1, 1, 512, 2048, 163) == -2          # centre bone out of range
+    assert rc(xat_dim=500) == -2                                      # xat_dim not a multiple of 32
+    assert rc(xat_mlp_dim=0) == -2                                    # no FeedForward width
+    assert rc(head=2) == -2                                           # unknown head kind
+    assert rc(person_center_idx=163) == -2                            # centre bone out of range
     assert b"person_center" in lib.mhmr_last_error()
-    assert rc(*base, 1, 512, 2048, 163) == 0
-    assert lib.mhmr_destroy(h) == 0
+    assert rc() == 0
+    assert lib.mhmr_destroy(h.item()) == 0

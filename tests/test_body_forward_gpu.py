@@ -26,12 +26,6 @@ CAP = 80
 V_SWEEP = (5, 71, 72, 73, 144, 145, "real")
 
 
-def _stream():
-    from ctypes import c_void_p
-
-    return c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _canvases(shapes, P, cap, dev):
     """{name: (flat canvas, [P, *shape] view)}: GUARD sentinels, cap persons' rows of sentinels, GUARD sentinels."""
     out = {}
@@ -57,9 +51,7 @@ def _body(bm, kind, nb, dev, cap=CAP):
 
 def raw_forward(body, pose, betas, transl, K, expr, with_v2d=True):
     """mhmr_body_forward into sentinel canvases; returns the outputs (guards checked)."""
-    from ctypes import c_int
-
-    from multihmr_b200._lib import check, ptr
+    from multihmr_b200._lib import call, stream
 
     P = int(betas.shape[0])
     fp, b, tr, Kd, ex = body._inputs(pose, betas, transl, K, expr)
@@ -68,27 +60,23 @@ def raw_forward(body, pose, betas, transl, K, expr, with_v2d=True):
     if not with_v2d:
         shapes.pop("v2d")
     cv = _canvases(shapes, P, body.max_persons, body.device)
-    o = lambda k: ptr(cv[k][1]) if k in cv else None
-    check(body._lib.mhmr_body_forward(body._h, c_int(P), ptr(fp), ptr(b), ptr(ex), ptr(tr), ptr(Kd), o("v3d"),
-                                      o("v2d"), o("j3d"), o("j2d"), o("transl_pelvis"), _stream()),
-          "mhmr_body_forward")
+    o = lambda k: cv[k][1] if k in cv else None
+    call("mhmr_body_forward", body._h, P, fp, b, ex, tr, Kd, o("v3d"), o("v2d"), o("j3d"), o("j2d"), o("transl_pelvis"),
+         stream())
     torch.cuda.synchronize()
     _check_guards(cv, P)
     return {k: v[1] for k, v in cv.items()}
 
 
 def placed_forward(m, rotvec, shape, loc, dist, K, expr):
-    from ctypes import c_int
-
-    from multihmr_b200._lib import check, ptr
+    from multihmr_b200._lib import call, stream
 
     m.finalize()
     x = m._smplx_inputs(rotvec, shape, loc, dist, K, expr)
     P, V = int(rotvec.shape[0]), m.num_verts
     shapes = dict(v3d=(V, 3), v2d=(V, 2), j3d=(127, 3), j2d=(127, 2), transl=(3,), transl_pelvis=(3,))
     cv = _canvases(shapes, P, m.max_persons, m.device)
-    check(m._lib.mhmr_smplx_forward(m._handle, c_int(P), ptr(x[0]), ptr(x[1]), ptr(x[5]), ptr(x[2]), ptr(x[3]),
-                                    ptr(x[4]), *[ptr(cv[k][1]) for k in shapes], _stream()), "mhmr_smplx_forward")
+    call("mhmr_smplx_forward", m._handle, P, x[0], x[1], x[5], x[2], x[3], x[4], *[cv[k][1] for k in shapes], stream())
     torch.cuda.synchronize()
     _check_guards(cv, P)
     return {k: v[1] for k, v in cv.items()}

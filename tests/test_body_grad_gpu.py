@@ -251,26 +251,20 @@ def test_autograd_wrappers_match_entries(bodies, engine, cuda_device):
 
 
 def test_entries_reject_bad_arguments(bodies, engine, cuda_device):
-    from ctypes import c_int, c_void_p
-
-    from multihmr_b200._lib import MhmrError, check, ptr
+    from multihmr_b200._lib import MhmrError, call
 
     body = bodies["smpl"]
     x = body._inputs(*_raw_case("smpl", 2, 3)[:5])
     d = [torch.empty_like(t) for t in (x[0], x[1], x[2])]
-    call = lambda P, fp: body._lib.mhmr_body_backward(body._h, c_int(P), ptr(fp), ptr(x[1]), None, ptr(x[2]),
-                                                      ptr(x[3]), None, None, None, None, None, ptr(d[0]), ptr(d[1]),
-                                                      None, ptr(d[2]), c_void_p(0))
     for P, fp in ((49, x[0]), (-1, x[0]), (2, None)):
         with pytest.raises((AssertionError, MhmrError)):
-            check(call(P, fp), "mhmr_body_backward")
+            call("mhmr_body_backward", body._h, P, fp, x[1], None, x[2], x[3], None, None, None, None, None, d[0], d[1],
+                 None, d[2], None)
     m, _ = engine
     xs = m._smplx_inputs(*_placed_case(2, 3)[:6])
     with pytest.raises((AssertionError, MhmrError)):
-        check(m._lib.mhmr_smplx_backward(m._handle, c_int(33), *[ptr(t) for t in xs[:2]], ptr(xs[5]), ptr(xs[2]),
-                                         ptr(xs[3]), ptr(xs[4]), *([None] * 6), *[ptr(torch.empty_like(t)) for t in
-                                                                                  (xs[0], xs[1], xs[5], xs[2], xs[3])],
-                                         c_void_p(0)), "mhmr_smplx_backward")
+        call("mhmr_smplx_backward", m._handle, 33, *xs[:2], xs[5], xs[2], xs[3], xs[4], *([None] * 6),
+             *[torch.empty_like(t) for t in (xs[0], xs[1], xs[5], xs[2], xs[3])], None)
 
 
 def _fit(grad_fn, forward, params, target, steps=200):

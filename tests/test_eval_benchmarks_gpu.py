@@ -184,12 +184,9 @@ def test_new_entries_reject_bad_sizes(dev_assets, cuda_device):
 def test_body_create_from_host_arrays(assets, dev_assets, cuda_device):
     """mhmr_body_create takes host or device arrays: a handle built from host (CPU) tensors gives the same meshes as
     one built from device tensors."""
-    import ctypes
-
     from multihmr_b200 import _lib
-    from multihmr_b200._lib import c_int, c_void_p, check, ptr
+    from multihmr_b200._lib import call, stream
 
-    lib = _lib.load()
     bm = assets["smplx"]
     sd = torch.cat([bm["shapedirs"], bm["shapedirs_extra"]], -1)[..., :11].float().contiguous()
     f32 = lambda t: t.float().contiguous()
@@ -197,10 +194,9 @@ def test_body_create_from_host_arrays(assets, dev_assets, cuda_device):
     arrs = [f32(bm["v_template"]), sd, f32(bm["expr_dirs"]), f32(bm["posedirs"]), f32(bm["J_regressor"]),
             f32(bm["lbs_weights"]), i32(bm["parents"]), i32(bm["extra_joints_idxs"]),
             i32(bm["faces"].long()[bm["lmk_faces_idx"].long()]), f32(bm["lmk_bary_coords"])]
-    h = c_void_p()
-    check(lib.mhmr_body_create(c_int(1), c_int(bm["v_template"].shape[0]), c_int(11), c_int(8),
-                               *[ptr(a) for a in arrs], c_void_p(torch.cuda.current_stream().cuda_stream),
-                               ctypes.byref(h)), "mhmr_body_create (host arrays)")
+    h = torch.zeros(1, dtype=torch.int64)
+    call("mhmr_body_create", 1, bm["v_template"].shape[0], 11, 8, *arrs, stream(), h)
+    h = h.item()
     try:
         pose, betas, transl, K, expr = _body_case("smplx", 3, 5)
         ref = dev_assets["smplx"](pose, betas, transl, K, expression=expr)
@@ -208,13 +204,11 @@ def test_body_create_from_host_arrays(assets, dev_assets, cuda_device):
         # the inputs stay referenced for the call (a temporary's block could be handed to the next one)
         ins = [d(pose, 165), d(betas, 11), d(expr, 10), d(transl, 3), d(K, 9)]
         out = {k: torch.empty_like(v) for k, v in ref.items()}
-        check(lib.mhmr_body_forward(h, c_int(3), *[ptr(t) for t in ins], ptr(out["v3d"]), None, ptr(out["j3d"]),
-                                    ptr(out["j2d"]), ptr(out["transl_pelvis"]),
-                                    c_void_p(torch.cuda.current_stream().cuda_stream)), "mhmr_body_forward")
+        call("mhmr_body_forward", h, 3, *ins, out["v3d"], None, out["j3d"], out["j2d"], out["transl_pelvis"], stream())
         for k in ref:
             assert torch.equal(out[k], ref[k]), k
     finally:
-        lib.mhmr_body_destroy(h)
+        _lib.load().mhmr_body_destroy(h)
 
 
 def _stub(cases, dev):

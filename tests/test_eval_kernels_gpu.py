@@ -15,9 +15,6 @@ degenerate-geometry edges.
 Every output lands in a canvas with sentinel guard bands: slots from n_pairs up to max_pairs and anything past P or G
 must come back untouched.  n_pairs is written on the device right before each call.  Each planted mistake of the
 util falls outside its bound on at least one case here."""
-import ctypes
-from ctypes import c_float, c_int
-
 import numpy as np
 import pytest
 import torch
@@ -28,16 +25,6 @@ from fp64_util import SENTINEL, _report
 pytestmark = pytest.mark.gpu
 GUARD = 32
 ISENT = -777
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _lib():
-    from multihmr_b200 import _lib
-
-    return _lib.load()
 
 
 def _canvas(n, dev, dtype=torch.float32):
@@ -60,7 +47,7 @@ def _n_pairs(n, dev):
 
 # ------------------------------------------------------------------------------------------------------ matching
 def run_match(pred, gt, vmask, thr, dev):
-    from multihmr_b200._lib import check, ptr
+    from multihmr_b200._lib import call, stream
 
     P, G, J = len(pred), len(gt), gt.shape[1]
     pr = torch.from_numpy(pred).to(dev).contiguous() if P else None
@@ -70,8 +57,7 @@ def run_match(pred, gt, vmask, thr, dev):
     nb, nv = _canvas(1, dev, torch.int32)
     p2g, p2gv = _canvas(48, dev, torch.int32)
     g2p, g2pv = _canvas(48, dev, torch.int32)
-    check(_lib().mhmr_eval_match_2d(ptr(pr), ptr(g), ptr(vm), c_int(P), c_int(G), c_int(J), c_float(thr), ptr(pv),
-                                    ptr(nv), ptr(p2gv), ptr(g2pv), _stream()), "mhmr_eval_match_2d")
+    call("mhmr_eval_match_2d", pr, g, vm, P, G, J, thr, pv, nv, p2gv, g2pv, stream())
     torch.cuda.synchronize()
     n = int(nv.item())
     _untouched(nb, 1, "n_pairs")
@@ -126,7 +112,7 @@ def test_match_sensitivity(cuda_device):
 # ------------------------------------------------------------------------------------------------------ points
 def run_points(pred, pc, gt, gc, pairs, n, max_pairs, dev):
     """pred [P, npt, 3], gt [G, npt, 3], centres [*, 3] or None (numpy fp32); pairs [n, 2]."""
-    from multihmr_b200._lib import check, ptr
+    from multihmr_b200._lib import call, stream
 
     t = lambda a: None if a is None else torch.from_numpy(np.ascontiguousarray(a, np.float32)).to(dev)
     pr, pcd, g, gcd = t(pred), t(pc), t(gt), t(gc)
@@ -136,9 +122,7 @@ def run_points(pred, pc, gt, gc, pairs, n, max_pairs, dev):
     err, ev = _canvas(max_pairs, dev)
     pa, pav = _canvas(max_pairs, dev)
     nd = _n_pairs(n, dev)  # referenced until the kernel has run
-    check(_lib().mhmr_eval_points_error(ptr(pr), ptr(pcd), ptr(g), ptr(gcd), ptr(pd), ptr(nd),
-                                        c_int(max_pairs), c_int(pred.shape[1]), ptr(ev), ptr(pav), _stream()),
-          "mhmr_eval_points_error")
+    call("mhmr_eval_points_error", pr, pcd, g, gcd, pd, nd, max_pairs, pred.shape[1], ev, pav, stream())
     torch.cuda.synchronize()
     _untouched(err, n, "err_mm")
     _untouched(pa, n, "pa_err_mm")
@@ -207,7 +191,7 @@ def test_points_error_sensitivity(cuda_device):
 
 # ------------------------------------------------------------------------------------------------------ regression
 def run_regress(rowptr, col, val, R, N, rows, root, X, c, pairs, side, n, max_pairs, K, dev):
-    from multihmr_b200._lib import check, ptr
+    from multihmr_b200._lib import call, stream
 
     t = lambda a, dt=np.float32: None if a is None else torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)
     R_out = R if rows is None else len(rows)
@@ -221,9 +205,7 @@ def run_regress(rowptr, col, val, R, N, rows, root, X, c, pairs, side, n, max_pa
     # every input stays referenced until the kernel has run (a freed temporary's block goes to the next one)
     rw, cd, pd, nd = t(rows, np.int32), t(c), t(slots, np.int32), _n_pairs(n, dev)
     Kd = None if K is None else t(K.reshape(-1, 9))
-    check(_lib().mhmr_eval_regress(ptr(rp), ptr(cl), ptr(vl), c_int(R), c_int(N), ptr(rw), c_int(R_out),
-                                   c_int(root), ptr(Xd), ptr(cd), ptr(pd), c_int(side), ptr(nd), c_int(max_pairs),
-                                   ptr(Kd), ptr(ov), ptr(o2v), _stream()), "mhmr_eval_regress")
+    call("mhmr_eval_regress", rp, cl, vl, R, N, rw, R_out, root, Xd, cd, pd, side, nd, max_pairs, Kd, ov, o2v, stream())
     torch.cuda.synchronize()
     _untouched(out, n * R_out * 3, "out")
     y = ov[:n * R_out * 3].view(n, R_out, 3).double().cpu()

@@ -1,7 +1,5 @@
 """CPU: the C-ABI library builds, loads and exports every symbol include/mhmr.h declares; host logic that
 needs no GPU."""
-import ctypes
-
 import pytest
 import torch
 
@@ -18,18 +16,17 @@ def test_library_exports_every_declared_symbol():
 
 def test_create_validates_config_without_gpu():
     from multihmr_b200 import _lib
-    from multihmr_b200.model import _Config
 
     lib = _lib.load()
-    h = ctypes.c_void_p()
-    bad = _Config(2, 900, 1, 8, 2, 8, 10, 15, 10475)  # 900 % 14 != 0  (model.py:65 "Invalid img size")
-    assert lib.mhmr_create(ctypes.byref(bad), ctypes.byref(h)) == -2
+    h = torch.zeros(1, dtype=torch.int64)
+    cfg = dict(arch=2, img_size=896, max_batch=1, max_persons=8, xat_depth=2, xat_num_heads=8, num_betas=10,
+               person_center_idx=15, num_verts=10475)
+    create = lambda **change: lib.mhmr_create(_lib.struct("mhmr_config", **{**cfg, **change}), h)
+    assert create(img_size=900) == -2  # 900 % 14 != 0  (model.py:65 "Invalid img size")
     assert b"img size" in lib.mhmr_last_error()
-    bad = _Config(5, 896, 1, 8, 2, 8, 10, 15, 10475)
-    assert lib.mhmr_create(ctypes.byref(bad), ctypes.byref(h)) == -2
-    ok = _Config(2, 896, 1, 8, 2, 8, 10, 15, 10475)
-    assert lib.mhmr_create(ctypes.byref(ok), ctypes.byref(h)) == 0
-    assert lib.mhmr_destroy(h) == 0
+    assert create(arch=5) == -2
+    assert create() == 0
+    assert lib.mhmr_destroy(h.item()) == 0
 
 
 def test_model_requires_cuda_no_cpu_fallback():

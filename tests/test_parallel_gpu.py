@@ -22,10 +22,7 @@ def test_pack_kernel_matches_torch_statement(cuda_device, capacity):
     """mhmr_pack_records (one kernel, count read on the device) == parallel.pack_block_torch, bit for bit,
     both when the block has room (capacity 8 > 5 persons) and when it overflows (capacity 3: header reports 5
     detected / 3 packed)."""
-    import ctypes
-
     from multihmr_b200 import _lib, parallel
-    from multihmr_b200.model import _OUT_FIELDS, _Outputs
 
     case, sd, bm, x, K, idx = pu.build_inputs("s_224_S_forced")
     m = pu.build_engine(case, sd, bm, max_persons=16)
@@ -34,14 +31,11 @@ def test_pack_kernel_matches_torch_statement(cuda_device, capacity):
     lib = _lib.load()
     _, R = parallel.record_layout(m.num_betas, m.num_verts)
     block = torch.full((parallel.HEADER_WORDS + capacity * R,), 7.0, device=cuda_device)
-    o = _Outputs(*[ctypes.c_void_p(t[n].data_ptr()) if t.get(n) is not None else None for n in _OUT_FIELDS])
-    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    _lib.check(lib.mhmr_pack_records(ctypes.byref(o), 16, m.num_betas, m.num_verts, 24, capacity,
-                                     ctypes.c_void_p(block.data_ptr()), stream), "mhmr_pack_records")
+    _lib.call("mhmr_pack_records", _lib.struct("mhmr_outputs", **t), 16, m.num_betas, m.num_verts, 24, capacity, block,
+              _lib.stream())
     torch.cuda.synchronize()
     want = parallel.pack_block_torch(t, P, 24, capacity, m.num_betas, m.num_verts)
     assert torch.equal(block.view(torch.int32), want.view(torch.int32))
-    lib.mhmr_record_block_bytes.restype = ctypes.c_int64
     assert lib.mhmr_record_block_bytes(m.num_betas, m.num_verts, capacity) == block.numel() * 4
     assert lib.mhmr_record_floats(m.num_betas, m.num_verts) == R
 
