@@ -78,6 +78,21 @@ int mhmr_op_attention(const void* qkv, int64_t ld_qkv, void* out, int64_t ldo, i
  * host derives from that function the output is bit-identical, and the upload is 4x smaller.  W % 4 == 0. */
 int mhmr_op_normalize_u8(const void* img_u8, const float* lut, float* out, int B, int H, int W, void* stream);
 
+/* Letterbox of photos of any size into the S x S model input: `ImageOps.pad(ImageOps.contain(photo, (S, S)), (S, S))`
+ * of reference demo.py:27-51 (also app.py:114-122 and the dataset loaders), byte for byte.  Photo b is resized keeping
+ * its aspect ratio to (new_w, new_h), one side S and the other round(short / long * S) (half to even), with Pillow's
+ * 8-bit BICUBIC resampler (coefficients computed in double, 22-bit int32 weights, int32 sums), and pasted at (x0, y0) =
+ * round((S - new) / 2); every other byte of the output is `pad` (0 for the model input, 255 for demo.py:42's copy).
+ *   photos  HOST int64 [B, 4]: device address, H, W, row pitch in bytes (>= 3 W) of each uint8 RGB HWC photo; the
+ *           photos of one call may have different sizes
+ *   out     device uint8 [B, S, S, 3]
+ *   boxes   HOST int32 [B, 4] (nullable): x0, y0, new_w, new_h of each pasted photo
+ * Every argument is checked before any launch; a photo whose short side rounds to 0 pixels is MHMR_ERR_ARG (Pillow
+ * raises ValueError).  Two kernel launches for the whole batch.  The per-photo descriptors and coefficient tables go
+ * up in one cudaMemcpyAsync from pageable host memory, which the CUDA driver may stage synchronously with `stream`;
+ * the workspace is stream-ordered (cudaMallocAsync / cudaFreeAsync).  Nothing else waits for the device. */
+int mhmr_op_letterbox_u8(const int64_t* photos, int B, int S, int pad, uint8_t* out, int32_t* boxes, void* stream);
+
 /* Person-decoder kernels (the per-person path after the backbone), each the engine's own launcher behind a thin
  * validating entry.  All pointers are device pointers; `count` is a device int32 holding the person count
  * (<= max_persons), read on the device as in the engine: grids are sized for max_persons and exit early, and rows

@@ -3,7 +3,8 @@
 
     open_image, get_camera_parameters, load_model, forward_model
 
-Only the forward itself is H100-native; image decoding stays on the host (PIL), as in the reference.
+plus `open_images`, the batched form of `open_image`.  The letterbox (resize + pad) and the forward are H100-native;
+image decoding stays on the host (PIL), as in the reference.
 """
 from __future__ import annotations
 
@@ -15,7 +16,7 @@ import torch
 from .model import Model
 from .model_anny import ModelAnny
 
-from .preprocess import IMG_NORM_MEAN, IMG_NORM_STD, device_table, normalize_rgb, normalize_rgb_table  # noqa: F401
+from .preprocess import IMG_NORM_MEAN, IMG_NORM_STD, device_table, letterbox, normalize_rgb, normalize_rgb_table  # noqa: F401
 
 SMPLX_DIR = "models"                         # utils/constants.py:7
 CACHE_DIR_MULTIHMR = "models/multiHMR"       # utils/constants.py:9
@@ -29,23 +30,56 @@ def normalize_rgb_device(img_u8: torch.Tensor) -> torch.Tensor:
     return ops.normalize_u8(img_u8.contiguous(), device_table(img_u8.device))
 
 
+def _letterbox_photos(imgs_pil, img_size, device, fused):
+    """Decoded RGB photos -> (batch, full-resolution uint8 [H, W, 3] device photos, boxes): each photo is copied once
+    into pinned memory and uploaded once; the device letterbox (`preprocess.letterbox`) makes the uint8 [B, S, S, 3]
+    batch, normalised to fp32 [B, 3, S, S] unless `fused`."""
+    photos = []
+    for im in imgs_pil:
+        host = torch.empty((im.height, im.width, 3), dtype=torch.uint8, pin_memory=True)
+        host.numpy()[...] = np.asarray(im)
+        photos.append(host.to(device, non_blocking=True))
+    u8, boxes = letterbox(photos, img_size)
+    if fused:
+        return u8, photos, boxes
+    if img_size % 2:
+        raise ValueError("the device normalisation needs an even img_size")
+    B = u8.shape[0]   # viewed as rows of 4 pixels: the same pixels, channel planes of S*S values
+    x = normalize_rgb_device(u8.view(B, img_size * img_size // 4, 4, 3)).view(B, 3, img_size, img_size)
+    return x, photos, boxes
+
+
+def open_images(paths, img_size, device=torch.device("cuda"), fused=False):
+    """`open_image` for a batch of photo files of any sizes, on the device: decodes on the host (PIL), uploads each
+    full-resolution photo once and letterboxes the batch there, byte for byte as `ImageOps.contain` + `ImageOps.pad`.
+    Returns (normalised fp32 [B, 3, S, S], or with `fused=True` the uint8 [B, S, S, 3] batch that `Model.forward` /
+    `forward_model` take through the fused loader; the full-resolution uint8 [H, W, 3] device photos, the renderer's
+    backgrounds; int32 [B, 4] host tensor of (x0, y0, new_w, new_h), each photo's box in the square)."""
+    from PIL import Image
+
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise ValueError("open_images letterboxes on a CUDA device (open_image is the host path)")
+    with torch.cuda.device(device):
+        return _letterbox_photos([Image.open(p).convert("RGB") for p in paths], img_size, device, fused)
+
+
 def open_image(img_path, img_size, device=torch.device("cuda"), fused=False):
     """Open, resize keeping the aspect ratio, zero-pad to a square, normalise (demo.py:27-51).  On a CUDA
-    device the padded uint8 image is uploaded and normalised there (same values, a quarter of the bytes).
-    `fused=True` returns the uint8 [1,S,S,3] device tensor itself: `Model.forward` / `forward_model` then run the
-    fused loader (uint8 -> normalised fp16 patch rows, `mhmr_forward_u8`) and the fp32 image never exists."""
+    device the full-resolution photo is uploaded, letterboxed and normalised there (`open_images` of one photo: the
+    same bytes as the host path).  `fused=True` returns the uint8 [1,S,S,3] device tensor itself: `Model.forward` /
+    `forward_model` then run the fused loader (uint8 -> normalised fp16 patch rows, `mhmr_forward_u8`) and the fp32
+    image never exists."""
     from PIL import Image, ImageOps
 
     img_pil = Image.open(img_path).convert("RGB")
     img_pil_full = img_pil.copy()
-    img_pil = ImageOps.contain(img_pil, (img_size, img_size))
-    img_pil = ImageOps.pad(img_pil, size=(img_size, img_size))
     device = torch.device(device)
     if device.type == "cuda" and img_size % 4 == 0:
-        u8 = torch.from_numpy(np.ascontiguousarray(np.asarray(img_pil))).unsqueeze(0).to(device)
-        if fused:
-            return u8, img_pil_full
-        return normalize_rgb_device(u8), img_pil_full
+        with torch.cuda.device(device):
+            return _letterbox_photos([img_pil], img_size, device, fused)[0], img_pil_full
+    img_pil = ImageOps.contain(img_pil, (img_size, img_size))
+    img_pil = ImageOps.pad(img_pil, size=(img_size, img_size))
     x = torch.from_numpy(normalize_rgb(np.asarray(img_pil))).unsqueeze(0).to(device)
     return x, img_pil_full
 

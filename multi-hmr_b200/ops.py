@@ -58,6 +58,29 @@ def normalize_u8(img_u8, lut):
     return out
 
 
+def letterbox_u8(photos, S, pad=0):
+    """Photos (a list of uint8 [H, W, 3] CUDA tensors on one device, of any sizes; rows may be padded) -> (uint8
+    [B, S, S, 3] on their device, int32 [B, 4] host tensor of (x0, y0, new_w, new_h)): ImageOps.pad(ImageOps.contain(
+    photo, (S, S)), (S, S), color=pad) with Pillow's BICUBIC resampler, byte for byte (`mhmr_op_letterbox_u8`)."""
+    _cuda(*photos)
+    assert len(photos) >= 1, "letterbox needs at least one photo"
+    dev = photos[0].device
+    desc = torch.empty(len(photos), 4, dtype=torch.int64)
+    keep = []  # contiguous copies made here stay alive until the kernels are enqueued
+    for i, p in enumerate(photos):
+        assert p.dtype == torch.uint8 and p.dim() == 3 and p.shape[2] == 3 and p.device == dev, \
+            "uint8 [H, W, 3] photos on one device expected"
+        if not (p.stride(2) == 1 and p.stride(1) == 3 and (p.shape[0] == 1 or p.stride(0) >= 3 * p.shape[1])):
+            p = p.contiguous()
+        keep.append(p)
+        desc[i] = torch.tensor([p.data_ptr(), p.shape[0], p.shape[1], p.stride(0) if p.shape[0] > 1 else 3 * p.shape[1]])
+    out = torch.empty(len(photos), S, S, 3, dtype=torch.uint8, device=dev)
+    boxes = torch.empty(len(photos), 4, dtype=torch.int32)
+    with torch.cuda.device(dev):
+        call("mhmr_op_letterbox_u8", desc, len(photos), S, pad, out, boxes, stream())
+    return out, boxes
+
+
 def attention(qkv, B, T, D, out=None):
     """qkv [B*T, 3*D] fp16 -> out [B*T, D] fp16, heads of 64 dims, softmax(q k^T / 8) v per image."""
     _cuda(qkv)

@@ -1,5 +1,6 @@
 """Host statement of the reference's image normalisation (utils/image.py:8-24) and the [3][256] table that the
-device kernels (`mhmr_op_normalize_u8`, the fused loader of `mhmr_forward_u8`) use to reproduce it bit for bit."""
+device kernels (`mhmr_op_normalize_u8`, the fused loader of `mhmr_forward_u8`) use to reproduce it bit for bit, and
+the device letterbox of photos of any size (`ImageOps.contain` + `ImageOps.pad`, demo.py:27-51)."""
 from __future__ import annotations
 
 import numpy as np
@@ -21,6 +22,22 @@ def normalize_rgb_table() -> np.ndarray:
     """[3, 256] fp32: `normalize_rgb` of every uint8 value in every channel (the table of the device kernels)."""
     ramp = np.repeat(np.arange(256, dtype=np.uint8)[None, :, None], 3, axis=2)
     return np.ascontiguousarray(normalize_rgb(ramp)[:, 0, :])
+
+
+def letterbox(photos, img_size: int, color: int = 0):
+    """`ImageOps.pad(ImageOps.contain(photo, (S, S)), (S, S), color)` of every photo, on the device and byte for byte
+    (csrc/letterbox.cu; the arithmetic is restated in oracle/letterbox_ref.py).  `photos` is a list of uint8 [H, W, 3]
+    RGB tensors of any sizes: CUDA tensors are read where they are, host tensors are uploaded (pinned, non-blocking)
+    to the current CUDA device.  Returns (uint8 [B, S, S, 3] on the device, int32 [B, 4] host tensor of (x0, y0,
+    new_w, new_h), the box of each photo in the square).  The uint8 batch is what `Model.forward` / `forward_model`
+    take through the fused loader."""
+    import torch
+
+    from . import ops
+
+    dev = next((p.device for p in photos if p.is_cuda), torch.device("cuda"))
+    photos = [p if p.is_cuda else p.pin_memory().to(dev, non_blocking=True) for p in photos]
+    return ops.letterbox_u8(photos, img_size, color)
 
 
 _LUT_CACHE = {}
