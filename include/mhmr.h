@@ -285,6 +285,9 @@ typedef struct mhmr_outputs {
   float* j3d;          /* [max_persons, 127, 3]                                                           */
   float* j2d;          /* [max_persons, 127, 2]                                                           */
   float* z;            /* [B, N, D] backbone features (blocks/dinov2.py:25), nullable (stage parity)      */
+  /* Appended field. */
+  float* dec;          /* [max_persons, 318 + num_betas + 13] decoder rows pose6 | betas | cam | expression
+                          (model.py:571-575, the input of mhmr_op_person_post), nullable                   */
 } mhmr_outputs;
 
 /* Replaces `Model(**ckpt_args)` (reference demo.py:98-100, model.py:33-131). */
@@ -387,6 +390,29 @@ int mhmr_smplx_backward(mhmr_engine* h, int P, const float* rotvec, const float*
                         const float* g_j3d, const float* g_j2d, const float* g_transl, const float* g_transl_pelvis,
                         float* d_rotvec, float* d_shape, float* d_expression, float* d_loc, float* d_dist,
                         void* stream);
+/* ------------------------------------------------------------------------------------------------
+ * Training loss of the SMPL-X head (reference loss.py:47-115 on a forced-index forward, train.py:292-303) and its
+ * gradient with respect to the head's last Linears: the detection logits, the offset rows and the decoder rows.
+ * ---------------------------------------------------------------------------------------------- */
+/* Loss.forward(y_hat, y, epoch, img_size) for the first P persons of a forced-index mhmr_forward into y_hat (K [B,3,3]
+ * the forward's intrinsics; y_hat->v2d and y_hat->dec required), use_2d = (epoch >= start_2d_epoch).
+ *   targets  HOST int64 [11]: device addresses of the targets of Trainer.prepare_gt (train.py:116-182), fp32:
+ *            scores [B, res, res] (a cell is positive where scores >= 1), offset [P, 2], rotmat [P, 53, 3, 3] (root,
+ *            body 21, left hand 15, right hand 15, jaw), shape [P, shape_dim], dist_postprocessed [P], transl [P, 3],
+ *            transl_pelvis [P, 3], j3d [P, 127, 3], v3d [P, V, 3], j2d [P, 127, 2], v2d [P, V, 2]
+ *   weights  HOST float [10]: alpha_bce, _offset, _rotmat, _shape, _dist, _transl, _j3d, _v3d, _j2d, _v2d (loss.py:117-141)
+ * Writes loss [11] = total, bce, offset, rotmat, shape, dist, transl, j3d, v3d, j2d, v2d (each term after nan_to_num;
+ * the 2-D terms enter the total only with use_2d; the first min(shape_dim, num_betas) betas are compared) and the
+ * gradient of the total, written, not accumulated: d_logits [B * res * res] (through the clamped sigmoid: zero where
+ * scores_map sits on a clamp bound), d_offset [P, 2], d_dec [P, 318 + num_betas + 13].  A term replaced by
+ * nan_to_num contributes 0 and no gradient.  Chains through the SMPL-X layer's backward (mhmr_smplx_backward's
+ * kernels) and the Gram-Schmidt of the 6D rotations.  No float atomics; repeated calls are bitwise identical.  Every
+ * argument is checked before any launch; the scratch is stream-ordered (cudaMallocAsync / cudaFreeAsync).
+ * Asynchronous. */
+int mhmr_train_loss(mhmr_engine* h, int B, int P, const float* K, const mhmr_outputs* y_hat, const int64_t* targets,
+                    int shape_dim, const float* weights, int use_2d, float* loss, float* d_logits, float* d_offset,
+                    float* d_dec, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Sharded batches (one process per GPU, image shards per rank; SURVEY.md §8e).  The reference is single-GPU
  * (README.md:107); these entry points are what a multi-GPU caller of `forward_model` binds.

@@ -722,10 +722,11 @@ int head_forward(mhmr_engine* e, const ImgSrc& x, const float* K, int B, float d
   LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->query, Cq, count, Pm, e->C, e->Wte_q, Cq, e->te_const, kHphDim, nullptr, nullptr, 0.f,
                        0, nullptr, 0, e->xa, kHphDim, st));
   TRY(hph_decoder(e, det_b, count, st));
+  float* dec = o->dec != nullptr ? o->dec : e->dec;  // handed out when requested (training), same kernel and bits
   LAUNCH(MHMR_CAT_HEAD, skinny_linear(e->xa, kHphDim, count, Pm, kHphDim, e->Wdec, kHphDim, e->bdec, e->ndec, nullptr, nullptr, 0.f,
-                       0, nullptr, 0, e->dec, e->ndec, st));
+                       0, nullptr, 0, dec, e->ndec, st));
   const float focal_norm = static_cast<float>(e->cfg.img_size / (2.0 * tan(30.0 * 3.14159265358979323846 / 180.0)));
-  LAUNCH(MHMR_CAT_HEAD, person_post(e->dec, e->ndec, nb, o->offset, K, e->Kinv, det_b, det_y, det_x, count, Pm, focal_norm,
+  LAUNCH(MHMR_CAT_HEAD, person_post(dec, e->ndec, nb, o->offset, K, e->Kinv, det_b, det_y, det_x, count, Pm, focal_norm,
                      o->rotmat, o->rotvec, o->shape, o->expression, o->dist_pp, o->dist, o->loc, o->transl,
                      e->K_det, st));
   {
@@ -1046,6 +1047,34 @@ int mhmr_smplx_backward(mhmr_engine* h, int P, const float* rotvec, const float*
   g.v3d = g_v3d; g.v2d = g_v2d; g.j3d = g_j3d; g.j2d = g_j2d; g.tp = g_transl_pelvis;
   return smplx_backward(h->body.bm, h->body.gs, P, rotvec, shape, expression, loc, dist, K_det, g, g_transl, d_rotvec,
                         d_shape, d_expression, d_loc, d_dist, static_cast<cudaStream_t>(stream));
+}
+
+int mhmr_train_loss(mhmr_engine* h, int B, int P, const float* K, const mhmr_outputs* y_hat, const int64_t* targets,
+                    int shape_dim, const float* weights, int use_2d, float* loss, float* d_logits, float* d_offset,
+                    float* d_dec, void* stream) {
+  MHMR_REQUIRE(h != nullptr && K && y_hat && targets && weights && loss && d_logits, "null argument");
+  if (!h->finalized) { set_last_error("mhmr_train_loss before mhmr_finalize"); return MHMR_ERR_STATE; }
+  MHMR_REQUIRE(h->cfg.head == MHMR_HEAD_SMPLX, "mhmr_train_loss needs an SMPL-X engine");
+  MHMR_REQUIRE(B >= 1 && B <= h->cfg.max_batch, "batch exceeds max_batch");
+  MHMR_REQUIRE(P >= 0 && P <= h->cfg.max_persons, "P outside [0, max_persons]");
+  MHMR_REQUIRE(y_hat->scores_map && y_hat->det_idx && y_hat->offset && y_hat->dist_pp && y_hat->dist && y_hat->loc &&
+                   y_hat->rotmat && y_hat->rotvec && y_hat->shape && y_hat->expression && y_hat->transl &&
+                   y_hat->transl_pelvis && y_hat->v3d && y_hat->v2d && y_hat->j3d && y_hat->j2d && y_hat->dec,
+               "y_hat: every per-person output, v2d and dec are required");
+  for (int i = 0; i < 11; ++i) MHMR_REQUIRE(targets[i] != 0, "targets: every address is required");
+  MHMR_REQUIRE(shape_dim >= 1, "shape_dim must be positive");
+  MHMR_REQUIRE(P == 0 || (d_offset && d_dec), "d_offset and d_dec are required when P > 0");
+  TrainLossArgs a;
+  a.B = B; a.res = h->res; a.P = P; a.img_size = h->cfg.img_size; a.use_2d = use_2d != 0;
+  a.K = K; a.y_hat = y_hat;
+  const float** tp[11] = {&a.y.scores, &a.y.offset, &a.y.rotmat, &a.y.shape, &a.y.dist_pp, &a.y.transl,
+                          &a.y.transl_pelvis, &a.y.j3d, &a.y.v3d, &a.y.j2d, &a.y.v2d};
+  for (int i = 0; i < 11; ++i) *tp[i] = reinterpret_cast<const float*>(static_cast<intptr_t>(targets[i]));
+  a.y.shape_dim = shape_dim;
+  a.w = LossWeights{weights[0], weights[1], weights[2], weights[3], weights[4],
+                    weights[5], weights[6], weights[7], weights[8], weights[9]};
+  a.loss = loss; a.d_logits = d_logits; a.d_offset = d_offset; a.d_dec = d_dec;
+  return train_loss_smplx(h->body.bm, h->body.gs, a, static_cast<cudaStream_t>(stream));
 }
 
 int mhmr_last_launch_count(mhmr_engine* h) { return h != nullptr ? h->launches : 0; }

@@ -171,15 +171,36 @@ struct SmplxGradScratch {
 struct BodyGrads {
   const float *v3d = nullptr, *v2d = nullptr, *j3d = nullptr, *j2d = nullptr, *tp = nullptr;
 };
-// Placed layer: d_rotvec [P,53,3], d_shape [P,num_betas], d_expr [P,10] (nullable), d_loc [P,2], d_dist [P].
+// Placed layer: d_rotvec [P,53,3], d_shape [P,num_betas], d_expr [P,10] (nullable), d_loc [P,2], d_dist [P];
+// d_rotmat [P,53,9] (nullable): the gradient with respect to each joint's rotation matrix R = exp(rotvec).
 int smplx_backward(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* rotvec, const float* shape,
                    const float* expr, const float* loc, const float* dist, const float* K_det, const BodyGrads& g,
                    const float* g_transl, float* d_rotvec, float* d_shape, float* d_expr, float* d_loc, float* d_dist,
-                   cudaStream_t st);
+                   cudaStream_t st, float* d_rotmat = nullptr);
 // Raw body model: d_full_pose [P,NJ,3], d_betas [P,num_betas], d_expr [P,10] (nullable), d_transl [P,3].
 int body_backward_raw(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* full_pose,
                       const float* betas, const float* expr, const float* transl, const float* K, const BodyGrads& g,
                       float* d_full_pose, float* d_betas, float* d_expr, float* d_transl, cudaStream_t st);
+
+// ---- train_loss.cu: the SMPL-X head's training loss and its gradient (DESIGN.md §10) ------------------------
+// Targets and weights of mhmr_train_loss (include/mhmr.h), in that entry's order.
+struct TrainTargets {
+  const float *scores, *offset, *rotmat, *shape, *dist_pp, *transl, *transl_pelvis, *j3d, *v3d, *j2d, *v2d;
+  int shape_dim;
+};
+struct LossWeights {
+  float bce, offset, rotmat, shape, dist, transl, j3d, v3d, j2d, v2d;
+};
+struct TrainLossArgs {
+  int B = 0, res = 0, P = 0, img_size = 0, use_2d = 0;
+  const float* K = nullptr;  // [B, 3, 3]
+  const mhmr_outputs* y_hat = nullptr;
+  TrainTargets y;
+  LossWeights w;
+  float *loss = nullptr, *d_logits = nullptr, *d_offset = nullptr, *d_dec = nullptr;
+};
+// Arguments checked by the caller; enqueues everything on `st`.
+int train_loss_smplx(const SmplxDeviceModel& bm, SmplxGradScratch& gs, const TrainLossArgs& a, cudaStream_t st);
 
 // ---- body.cu: a body model on the device ----------------------------------------------------------
 // The folded tables, the forward and backward scratch and the person count of one SMPL / SMPL-X layer, in zero-filled

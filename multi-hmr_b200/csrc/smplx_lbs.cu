@@ -874,7 +874,8 @@ body_grad_stream_kernel(const float* __restrict__ PDX, int ldp, int KT, const fl
 }
 
 // 3. per person: tile sums, placement, A -> G, kinematic chain in reverse, pose features, Rodrigues, J(beta).
-// kRaw: d_rot = d_full_pose [P, NJ, 3], d_transl written; else d_rot = d_rotvec [P, 53, 3], d_loc / d_dist written.
+// kRaw: d_rot = d_full_pose [P, NJ, 3], d_transl written; else d_rot = d_rotvec [P, 53, 3], d_loc / d_dist written,
+// and d_R [P, 53, 9] (nullable) receives the gradient with respect to each rotation matrix, before Rodrigues.
 template <int NJ, int PF, bool kRaw>
 __global__ void __launch_bounds__(256)
 body_grad_person_kernel(const float* __restrict__ rotvec, const float* __restrict__ shape,
@@ -886,7 +887,7 @@ body_grad_person_kernel(const float* __restrict__ rotvec, const float* __restric
                         const float* __restrict__ dist, const float* __restrict__ K,
                         const float* __restrict__ g_transl, float* __restrict__ d_rot, float* __restrict__ d_shape,
                         float* __restrict__ d_expr, float* __restrict__ d_transl, float* __restrict__ d_loc,
-                        float* __restrict__ d_dist) {
+                        float* __restrict__ d_dist, float* __restrict__ d_R) {
   constexpr int kPSMax = NJ * 12 + kKTMax + 12;
   __shared__ float red[kPSMax];
   __shared__ float Rs[NJ][9], GR[NJ][9], Js[NJ][3];
@@ -958,6 +959,10 @@ body_grad_person_kernel(const float* __restrict__ rotvec, const float* __restric
           for (int n = 0; n < 3; ++n) gRr[m * 3 + n] += gJp[j * 3 + m] * (jp[j * 3 + n] - Jc[n]);
       const float* rv = rotvec + static_cast<int64_t>(p) * 53 * 3;
       rotvec_grad(rv[0], rv[1], rv[2], 0.f, true, gRr, d_rot + static_cast<int64_t>(p) * 53 * 3);
+      if (d_R != nullptr) {
+#pragma unroll
+        for (int q = 0; q < 9; ++q) d_R[static_cast<int64_t>(p) * 53 * 9 + q] = gRr[q];
+      }
 #pragma unroll
       for (int c = 0; c < 3; ++c) gcen[c] = -(X[c] * S[0] + X[3 + c] * S[1] + X[6 + c] * S[2]);
       // transl = K^-1 [loc, 1] dist (the inverse as loc_to_transl computes it)
@@ -1041,6 +1046,10 @@ body_grad_person_kernel(const float* __restrict__ rotvec, const float* __restric
     if (src >= 0) {
       float* o = d_rot + (static_cast<int64_t>(p) * (kRaw ? NJ : 53) + src) * 3;
       o[0] = gr[0]; o[1] = gr[1]; o[2] = gr[2];
+      if (!kRaw && d_R != nullptr) {
+#pragma unroll
+        for (int q = 0; q < 9; ++q) d_R[(static_cast<int64_t>(p) * 53 + src) * 9 + q] = gR[j][q];
+      }
     }
   }
   if (tid >= 64 && tid < 64 + L) {
@@ -1059,7 +1068,8 @@ template <int NJ, int PF, int NL, int PB, bool kRaw>
 int body_backward_impl(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* rotvec,
                        const float* shape, const float* expr, const float* transl, const float* K,
                        const BodyGrads& g, const float* loc, const float* dist, const float* g_transl, float* d_rot,
-                       float* d_shape, float* d_expr, float* d_transl, float* d_loc, float* d_dist, cudaStream_t st) {
+                       float* d_shape, float* d_expr, float* d_transl, float* d_loc, float* d_dist, float* d_R,
+                       cudaStream_t st) {
   const int KT = PF + bm.L, J = NJ + 21 + NL, V = bm.V;
   MHMR_REQUIRE(KT <= kKTMax, "smplx: too many blend-shape coefficients");
   MHMR_REQUIRE(bm.num_joints == NJ && bm.pose_feat == PF && bm.n_lmk == NL, "body model / kernel shape mismatch");
@@ -1092,7 +1102,7 @@ int body_backward_impl(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, 
   body_grad_person_kernel<NJ, PF, kRaw><<<P, 256, 0, st>>>(
       rotvec, shape, expr, bm.L - bm.num_betas, bm.Jt, bm.Jdirs, bm.parents, bm.num_betas, bm.center_idx, KT,
       gs.fw.Amat, gs.fw.jposed, gs.fw.xf, gs.gJ, J, gs.part, tiles, P, PS, loc, dist, K, g_transl, d_rot, d_shape,
-      d_expr, d_transl, d_loc, d_dist);
+      d_expr, d_transl, d_loc, d_dist, d_R);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }
@@ -1154,11 +1164,11 @@ int smplx_grad_init(DeviceBody* b, int max_persons, cudaStream_t st) {
 int smplx_backward(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* rotvec, const float* shape,
                    const float* expr, const float* loc, const float* dist, const float* K_det, const BodyGrads& g,
                    const float* g_transl, float* d_rotvec, float* d_shape, float* d_expr, float* d_loc, float* d_dist,
-                   cudaStream_t st) {
+                   cudaStream_t st, float* d_rotmat) {
   TRY(loc_to_transl(loc, dist, K_det, P, gs.transl, st));
   return body_backward_impl<kNJ, kPoseFeat, 51, 16, false>(bm, gs, P, rotvec, shape, expr, gs.transl, K_det, g, loc,
                                                            dist, g_transl, d_rotvec, d_shape, d_expr, nullptr, d_loc,
-                                                           d_dist, st);
+                                                           d_dist, d_rotmat, st);
 }
 
 int body_backward_raw(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, const float* full_pose,
@@ -1167,11 +1177,11 @@ int body_backward_raw(const SmplxDeviceModel& bm, SmplxGradScratch& gs, int P, c
   if (bm.num_joints == 24)
     return body_backward_impl<24, 207, 0, 8, true>(bm, gs, P, full_pose, betas, expr, transl, K, g, nullptr, nullptr,
                                                    nullptr, d_full_pose, d_betas, d_expr, d_transl, nullptr, nullptr,
-                                                   st);
+                                                   nullptr, st);
   if (bm.num_joints == kNJ)
     return body_backward_impl<kNJ, kPoseFeat, 51, 16, true>(bm, gs, P, full_pose, betas, expr, transl, K, g, nullptr,
                                                             nullptr, nullptr, d_full_pose, d_betas, d_expr, d_transl,
-                                                            nullptr, nullptr, st);
+                                                            nullptr, nullptr, nullptr, st);
   set_last_error("body model: only SMPL (24 joints) and SMPL-X (55 joints) are instantiated");
   return MHMR_ERR_UNSUPPORTED;
 }

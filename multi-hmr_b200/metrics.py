@@ -12,6 +12,8 @@ The three protocols of the reference README ("Evaluating BEDLAM-val / EHF-test /
           H36M joints of J_regressor_h36m"""
 from __future__ import annotations
 
+import math
+
 import torch
 
 from . import _lib
@@ -195,14 +197,16 @@ class BodyModel:
             ex = f(expression, 10) if expression is not None else torch.zeros(P, 10, device=dev)
         return fp, b, tr, Kd, ex
 
-    def _forward(self, fp, b, tr, Kd, ex):
+    def _forward(self, fp, b, tr, Kd, ex, want_v2d=False):
         dev, P = self.device, int(b.shape[0])
         V, J = self.num_verts, self.num_joints
         out = dict(v3d=torch.empty(P, V, 3, device=dev), j3d=torch.empty(P, J, 3, device=dev),
                    j2d=torch.empty(P, J, 2, device=dev), transl_pelvis=torch.empty(P, 3, device=dev))
+        if want_v2d:
+            out["v2d"] = torch.empty(P, V, 2, device=dev)
         with torch.cuda.device(dev):
-            call("mhmr_body_forward", self._h, P, fp, b, ex, tr, Kd, out["v3d"], None, out["j3d"], out["j2d"],
-                 out["transl_pelvis"], stream(dev))
+            call("mhmr_body_forward", self._h, P, fp, b, ex, tr, Kd, out["v3d"], out.get("v2d"), out["j3d"],
+                 out["j2d"], out["transl_pelvis"], stream(dev))
         return out
 
     def _backward(self, fp, b, tr, Kd, ex, g_v3d=None, g_v2d=None, g_j3d=None, g_j2d=None, g_transl_pelvis=None):
@@ -254,19 +258,18 @@ def _center_index(person_center) -> int:
     return person_center if isinstance(person_center, int) else KINEMATIC_JOINTS.index(person_center)
 
 
-def prepare_gt(y: dict, body_models, person_center="head", *, img_size: int, patch_size: int = 14):
-    """What Trainer.evaluate reads from Trainer.prepare_gt (train.py:58-182): {'K', 'j2d', 'v3d', 'transl_pelvis', 'j3d'}
-    for a batch `y` in the reference's collate_fn format, on the device.  body_models maps 'smpl_male', 'smpl_female'
-    and 'smplx' to `BodyModel`s (an `EvalAssets` works).  Input kinds:
-      smplx_vertices  EHF: the vertices themselves, joints = smplx J_regressor @ vertices (:70-73)
-      smpl_*          3DPW: SMPL male, replaced by SMPL female for persons with smpl_gender_id == 2 (:74-94)
-      smplx_*         BEDLAM: SMPL-X neutral, 11 betas, eyes and jaw included, expression zero (:95-110)
-    Persons whose `person_center` joint falls on a patch already taken by an earlier person are dropped (:137-180).
-    Returns None when `y` holds none of the three (an image without annotated persons)."""
+def _gt_bodies(y: dict, body_models, want_v2d: bool = False):
+    """The ground-truth body forward of Trainer.prepare_gt (train.py:61-112) on the valid persons of `y`:
+    (idx_h, outputs {'v3d', 'j3d', 'j2d', 'transl_pelvis'} (+ 'v2d' with want_v2d)), or None when `y` holds no persons'
+    annotation."""
     valid_h = y["valid_humans"]
     idx_h = torch.where(valid_h)
     nhv = int(valid_h.sum())
     K = y["K"][idx_h[0]]
+
+    def run(bm, *args):
+        return bm._forward(*bm._inputs(*args, None), want_v2d=True) if want_v2d else bm(*args)
+
     if "smplx_vertices" in y:
         verts = y["smplx_vertices"].reshape(1, -1, 3).to(torch.float32).contiguous()
         bm = body_models["smplx"]
@@ -274,13 +277,15 @@ def prepare_gt(y: dict, body_models, person_center="head", *, img_size: int, pat
         n = torch.ones(1, dtype=torch.int32, device=verts.device)
         jts, j2d = regress(bm.j_regressor, verts, one, n, side=1, K=K[:1])
         out = dict(v3d=verts, j3d=jts, j2d=j2d, transl_pelvis=jts[:, 0].contiguous())
+        if want_v2d:
+            out["v2d"] = _project(verts, K[:1])
     elif "smpl_root_pose" in y:
         sel = lambda k, n: y[k][idx_h[0], idx_h[1]].reshape(nhv, n)
         full_pose = torch.cat([sel("smpl_root_pose", 3), sel("smpl_body_pose", 23 * 3)], dim=1)
         args = (full_pose, sel("smpl_shape", 10), sel("smpl_transl", 3), K)
-        out = body_models["smpl_male"](*args)
+        out = run(body_models["smpl_male"], *args)
         if int(y["smpl_gender_id"].max()) == 2:
-            fem = body_models["smpl_female"](*args)
+            fem = run(body_models["smpl_female"], *args)
             idx = torch.where(y["smpl_gender_id"] == 2)[1]
             for k in out:
                 out[k][idx] = fem[k][idx]
@@ -290,12 +295,16 @@ def prepare_gt(y: dict, body_models, person_center="head", *, img_size: int, pat
         full_pose = torch.cat([sel("smplx_root_pose", 3), sel("smplx_body_pose", 21 * 3), sel("smplx_jaw_pose", 3),
                                sel("smplx_leye_pose", 3), sel("smplx_reye_pose", 3),
                                sel("smplx_left_hand_pose", 15 * 3), sel("smplx_right_hand_pose", 15 * 3)], dim=1)
-        out = body_models["smplx"](full_pose, sel("smplx_shape", 11), sel("smplx_transl", 3), K)
+        out = run(body_models["smplx"], full_pose, sel("smplx_shape", 11), sel("smplx_transl", 3), K)
     else:
         return None
-    # one person per patch of the primary keypoint (train.py:137-157); the patch indices come to the host once
+    return idx_h, out
+
+
+def _one_per_patch(idx_h, pk_loc, img_size: int, patch_size: int):
+    """One person per patch of the primary keypoint (train.py:137-157): (kept persons in order, their patch
+    (x, y) indices [n, 2] as a host list); the patch indices come to the host once."""
     n_patch = img_size // patch_size
-    pk_loc = out["j2d"][:, _center_index(person_center)]
     pk_idx = torch.clamp((pk_loc // patch_size).int(), 0, n_patch - 1).cpu().tolist()
     taken, keep = set(), []
     for k in range(len(pk_idx)):
@@ -303,11 +312,96 @@ def prepare_gt(y: dict, body_models, person_center="head", *, img_size: int, pat
         if cell not in taken:
             taken.add(cell)
             keep.append(k)
+    return keep, pk_idx
+
+
+def _project(x, K):
+    """utils/camera.py:14-27 perspective_projection: x [P, N, 3], K [P, 3, 3] -> [P, N, 2]."""
+    y = x / x[:, :, -1:]
+    return torch.einsum("bij,bkj->bki", K, y)[:, :, :2]
+
+
+def _rotvec_to_rotmat(rv):
+    """roma.rotvec_to_rotmat (first order below 1e-6 rad): [..., 3] -> [..., 3, 3]."""
+    shape = rv.shape[:-1]
+    rv = rv.reshape(-1, 3)
+    theta = rv.norm(dim=-1)
+    axis = rv / theta.clamp_min(1e-6)[:, None]
+    kx, ky, kz = axis.unbind(-1)
+    s, omc = torch.sin(theta), 1 - torch.cos(theta)
+    R = torch.stack([1 - (ky * ky + kz * kz) * omc, kx * ky * omc - kz * s, kx * kz * omc + ky * s,
+                     kx * ky * omc + kz * s, 1 - (kx * kx + kz * kz) * omc, ky * kz * omc - kx * s,
+                     kx * kz * omc - ky * s, ky * kz * omc + kx * s, 1 - (kx * kx + ky * ky) * omc], -1)
+    x, y_, z = rv.unbind(-1)
+    o = torch.ones_like(x)
+    first = torch.stack([o, -z, y_, z, o, -x, -y_, x, o], -1)
+    R = torch.where((theta < 1e-6)[:, None], first, R)
+    return R.reshape(*shape, 3, 3)
+
+
+def prepare_gt(y: dict, body_models, person_center="head", *, img_size: int, patch_size: int = 14):
+    """What Trainer.evaluate reads from Trainer.prepare_gt (train.py:58-182): {'K', 'j2d', 'v3d', 'transl_pelvis', 'j3d'}
+    for a batch `y` in the reference's collate_fn format, on the device.  body_models maps 'smpl_male', 'smpl_female'
+    and 'smplx' to `BodyModel`s (an `EvalAssets` works).  Input kinds:
+      smplx_vertices  EHF: the vertices themselves, joints = smplx J_regressor @ vertices (:70-73)
+      smpl_*          3DPW: SMPL male, replaced by SMPL female for persons with smpl_gender_id == 2 (:74-94)
+      smplx_*         BEDLAM: SMPL-X neutral, 11 betas, eyes and jaw included, expression zero (:95-110)
+    Persons whose `person_center` joint falls on a patch already taken by an earlier person are dropped (:137-180).
+    Returns None when `y` holds none of the three (an image without annotated persons)."""
+    r = _gt_bodies(y, body_models)
+    if r is None:
+        return None
+    idx_h, out = r
+    keep, _ = _one_per_patch(idx_h, out["j2d"][:, _center_index(person_center)], img_size, patch_size)
     dev = out["v3d"].device
     keep = torch.tensor(keep, dtype=torch.long, device=dev)
     gt = {k: v[keep].contiguous() for k, v in out.items()}
     gt["K"] = y["K"]
     return gt
+
+
+def prepare_train_targets(y: dict, body_models, person_center="head", *, img_size: int, patch_size: int = 14):
+    """The training targets of Trainer.prepare_gt (train.py:58-182, its `_target` dict) on the device: 'idx'
+    (batch, patch y, patch x, 0) of the kept persons, 'scores' [B, res, res] (1 at their patches), 'K', and per kept
+    person 'transl' (the person_center joint), 'transl_pelvis', 'dist', 'dist_postprocessed' (log depth normalised
+    by the focal length, fovn 60 at img_size), 'v3d', 'j3d', 'j2d', 'v2d', 'loc' (projected centre joint), 'offset'
+    (from the patch centre, in patches), and for SMPL-X parameters (BEDLAM) 'rotvec' / 'rotmat' [P, 53, ...] in the
+    model's order root, body 21, left hand 15, right hand 15, jaw, and 'shape'.  Input kinds and the one-person-per-
+    patch rule as in `prepare_gt`; None when `y` holds no annotation."""
+    r = _gt_bodies(y, body_models, want_v2d=True)
+    if r is None:
+        return None
+    idx_h, out = r
+    B = y["valid_humans"].shape[0]
+    jts = out["j3d"]
+    dev = jts.device
+    c = _center_index(person_center)
+    K = y["K"][idx_h[0]].to(dev, torch.float32)
+    tgt = dict(transl=jts[:, c], transl_pelvis=jts[:, 0], dist=jts[:, 0, 2])
+    fn = img_size / (2 * math.tan(math.radians(60) / 2))        # utils/camera.py:50-61, fovn 60
+    tgt["dist_postprocessed"] = torch.log(tgt["dist"] + 1e-10) * (fn / K[:, 0, 0])
+    tgt.update(v3d=out["v3d"], j3d=jts, j2d=out["j2d"], v2d=out["v2d"])
+    pk_loc = out["j2d"][:, c]
+    keep, pk_idx = _one_per_patch(idx_h, pk_loc, img_size, patch_size)
+    pk = torch.tensor(pk_idx, dtype=torch.float32, device=dev).reshape(-1, 2)
+    tgt["loc"] = pk_loc
+    tgt["offset"] = (pk_loc - (pk + 0.5) * patch_size) / patch_size
+    if "smplx_root_pose" in y:
+        sel = lambda k: y[k][idx_h[0], idx_h[1]].reshape(len(idx_h[0]), -1, 3).to(dev, torch.float32)
+        tgt["rotvec"] = torch.cat([sel("smplx_root_pose"), sel("smplx_body_pose"), sel("smplx_left_hand_pose"),
+                                   sel("smplx_right_hand_pose"), sel("smplx_jaw_pose")], 1)
+        tgt["rotmat"] = _rotvec_to_rotmat(tgt["rotvec"])
+        tgt["shape"] = y["smplx_shape"][idx_h[0], idx_h[1]].to(dev, torch.float32)
+    keep_t = torch.tensor(keep, dtype=torch.long, device=dev)
+    n_patch = img_size // patch_size
+    scores = torch.zeros(B, n_patch, n_patch, device=dev)
+    cells = pk.long()[keep_t] if keep else torch.zeros(0, 2, dtype=torch.long, device=dev)
+    b = idx_h[0].to(dev)[keep_t]
+    scores[b, cells[:, 1], cells[:, 0]] = 1.0
+    targets = {"idx": (b, cells[:, 1], cells[:, 0], torch.zeros_like(b)), "scores": scores, "K": y["K"]}
+    for k, v in tgt.items():
+        targets[k] = v[keep_t].contiguous()
+    return targets
 
 
 class Evaluator:

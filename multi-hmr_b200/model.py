@@ -246,6 +246,15 @@ class _EngineModel:
         return {c: (float(ms[i]), int(cnt[i])) for i, c in enumerate(self.PROFILE_CATEGORIES)}
 
 
+class TrainingOutputs(dict):
+    """The flat dict of `Model.forward(..., is_training=True)`; `raw` = (model, raw outputs, P, K) lets
+    `loss.Loss` score it on the device."""
+
+    def __init__(self, raw, d):
+        super().__init__(d)
+        self.raw = raw
+
+
 class Model(_EngineModel):
     """H100-native drop-in for reference `model.Model` (inference path)."""
 
@@ -314,7 +323,7 @@ class Model(_EngineModel):
             (self._set_table if k in BODY_TABLES else self._set_weight)("smplx." + k, v)
 
     # ------------------------------------------------------------------ forward
-    def _alloc_outputs(self, B, want_v2d, want_z):
+    def _alloc_outputs(self, B, want_v2d, want_z, want_dec=False):
         Pm, V, nb, dev = self.max_persons, self.num_verts, self.num_betas, self.device
         f = lambda *s: torch.empty(*s, device=dev, dtype=torch.float32)
         t = {
@@ -325,20 +334,24 @@ class Model(_EngineModel):
             "v3d": f(Pm, V, 3), "v2d": f(Pm, V, 2) if want_v2d else None, "j3d": f(Pm, 127, 3), "j2d": f(Pm, 127, 2),
             "z": f(B, self.res * self.res, self.embed_dim) if want_z else None,
         }
+        if want_dec:
+            t["dec"] = f(Pm, 318 + nb + 13)
         return t
 
-    def forward_raw(self, x, K, idx=None, det_thresh=0.3, nms_kernel_size=3, want_v2d=False, want_z=False):
-        """Enqueues one forward and returns (outputs dict of max_persons-sized device tensors, P)."""
+    def forward_raw(self, x, K, idx=None, det_thresh=0.3, nms_kernel_size=3, want_v2d=False, want_z=False,
+                    want_dec=False):
+        """Enqueues one forward and returns (outputs dict of max_persons-sized device tensors, P).  want_dec adds
+        'dec' [max_persons, 318 + num_betas + 13], the decoder rows pose6 | betas | cam | expression."""
         self.finalize()
         with torch.cuda.device(self.device):
-            return self._forward_raw(x, K, idx, det_thresh, nms_kernel_size, want_v2d, want_z)
+            return self._forward_raw(x, K, idx, det_thresh, nms_kernel_size, want_v2d, want_z, want_dec)
 
-    def _forward_raw(self, x, K, idx, det_thresh, nms_kernel_size, want_v2d, want_z):
+    def _forward_raw(self, x, K, idx, det_thresh, nms_kernel_size, want_v2d, want_z, want_dec=False):
         x, fused = self._prepare_image(x)
         K = K.to(self.device, dtype=torch.float32, non_blocking=True).contiguous()
         B = x.shape[0]
         assert K.shape == (B, 3, 3), "K must be [B,3,3]"
-        t = self._alloc_outputs(B, want_v2d, want_z)
+        t = self._alloc_outputs(B, want_v2d, want_z, want_dec)
         fidx, unsort = None, None
         if idx is not None:
             fidx = self._forced_idx(idx[:4] if len(idx) >= 4 else idx[:3], B)
@@ -350,9 +363,9 @@ class Model(_EngineModel):
         P = self._run(x, fused, K, det_thresh, nms_kernel_size, fidx, t)
         if unsort is not None and P > 0:
             per_person = ("det_score", "offset", "loc", "dist_pp", "dist", "rotmat", "rotvec", "shape", "expression",
-                          "transl", "transl_pelvis", "v3d", "v2d", "j3d", "j2d")
+                          "transl", "transl_pelvis", "v3d", "v2d", "j3d", "j2d", "dec")
             for k in per_person:
-                if t[k] is not None:
+                if t.get(k) is not None:
                     t[k][:P] = t[k][:P].index_select(0, unsort)
             t["det_idx"][:, :P] = t["det_idx"][:, :P].index_select(1, unsort)
         return t, P
@@ -363,17 +376,17 @@ class Model(_EngineModel):
         if is_training:
             assert idx is not None                                                   # model.py:151
         t, P = self.forward_raw(x, K, idx=idx if is_training else None, det_thresh=det_thresh,
-                                nms_kernel_size=nms_kernel_size, want_v2d=is_training)
+                                nms_kernel_size=nms_kernel_size, want_v2d=is_training, want_dec=is_training)
         if P == 0 and not is_training:
             return []                                                                # model.py:241-243
         if is_training:
-            return {
+            return TrainingOutputs((self, t, P, K), {
                 "dist_postprocessed": t["dist_pp"][:P, None], "scores": t["scores_map"][..., None],
                 "offset": t["offset"][:P], "dist": t["dist"][:P, None], "expression": t["expression"][:P],
                 "rotmat": t["rotmat"][:P], "shape": t["shape"][:P], "rotvec": t["rotvec"][:P], "loc": t["loc"][:P],
                 "v3d": t["v3d"][:P], "j3d": t["j3d"][:P], "j2d": t["j2d"][:P], "v2d": t["v2d"][:P],
                 "transl": t["transl"][:P], "transl_pelvis": t["transl_pelvis"][:P, None],
-            }
+            })
         persons = []
         for i in range(P):                                                           # model.py:329-347
             persons.append({
@@ -385,6 +398,19 @@ class Model(_EngineModel):
         return persons
 
     __call__ = forward
+
+    def training_loss(self, x, targets, epoch, loss_args):
+        """One training step's loss without the parameter update (train.py:292-303): the forced-index forward at
+        targets['idx'] / targets['K'] (`metrics.prepare_train_targets`), then `Loss.forward(pred, targets, epoch,
+        img_size)` and its backward on the device (`mhmr_train_loss`).  loss_args carries loss.py's alpha_* and
+        start_2d_epoch (`loss.Loss.add_specific_args`).  Returns (total, dict_loss, grads): 0-d device tensors,
+        and the gradients of total with respect to the head's last Linears, grads = {'scores_logits' [B, res, res],
+        'offset' [P, 2], 'dec' [P, 318 + num_betas + 13]}."""
+        from .loss import run_train_loss
+
+        K = targets["K"]
+        t, P = self.forward_raw(x, K, idx=targets["idx"], want_v2d=True, want_dec=True)
+        return run_train_loss(self, t, P, K, targets, epoch, loss_args)
 
     # ------------------------------------------------------------------ stage-level entries (parity / ncu)
     def backbone(self, x):
