@@ -147,6 +147,11 @@ def projection_bound(o, K, do):
 
 
 def forward_bound(bm, full_pose, comps, nb, transl, K, placed=None, center=15):
+    """forward_pieces(...)["out"]."""
+    return forward_pieces(bm, full_pose, comps, nb, transl, K, placed, center)["out"]
+
+
+def forward_pieces(bm, full_pose, comps, nb, transl, K, placed=None, center=15):
     """Per-element bound of the fp32 forward (body_prep_kernel, smplx_vertex_kernel, smplx_joints_kernel) against
     the fp64 one, from the accumulation lengths of the kernels.  Inputs fp64 on one device: full_pose [P,NJ,3] in
     smplx order, comps = [betas | expression], transl [P,3] (placed: the fp64 transl of loc / dist), K [P,3,3].
@@ -168,7 +173,9 @@ def forward_bound(bm, full_pose, comps, nb, transl, K, placed=None, center=15):
       * Placement: raw, + transl (1 rounding); placed, R (q - pelvis) - R (J_c - pelvis) + transl.
       * Vertex-picked joints copy the vertex; landmarks add 3 barycentric products (3 u).
       * Projection: projection_bound.
-    Returns a dict of fp64 bounds shaped like the outputs (v3d, v2d, j3d, j2d, transl_pelvis[, transl])."""
+    Returns the fp64 forward quantities with their bounds (rot / eR, J / dJ, Gt / dGt, A / eG, dAt, T / dTR, dTt, the
+    output points v / dv and joints j / dj, placed: R) and, under "out", a dict of fp64 bounds shaped like the outputs
+    (v3d, v2d, j3d, j2d, transl_pelvis[, transl])."""
     dt, dev = comps.dtype, comps.device
     d = lambda k: torch.as_tensor(bm[k]).to(dev, dt)
     P = comps.shape[0]
@@ -246,7 +253,8 @@ def forward_bound(bm, full_pose, comps, nb, transl, K, placed=None, center=15):
                transl_pelvis=dj[:, :1].expand(P, 3))
     if placed is not None:
         out["transl"] = placed["dtr"][:, None].expand(P, 3)
-    return out
+    return dict(rot=rot, pf=pf, eR=eR, J=J, dJ=dJ, Gt=Gt, dGt=dGt, A=A, eG=eG, dAt=dAt, T=T, dTR=dTR, dTt=dTt,
+                v=v, dv=dv, j=j, dj=dj, R=None if placed is None else placed["R"], out=out)
 
 
 def transl_bound(loc, dist, K):
