@@ -563,7 +563,8 @@ typedef struct mhmr_render_extra {
 } mhmr_render_extra;
 /* mhmr_render_forward plus props, per-view alpha and backgrounds.  Mesh m of the key is person m for m <
  * max_persons and prop m - max_persons after; max_persons + num_props must fit the key next to the face index.  The
- * person map (args->person) holds that mesh index. */
+ * person map (args->person) holds that mesh index.  Persons and props go through the same four launches;
+ * mhmr_render_forward is this call with e = NULL. */
 int mhmr_render_forward_extra(mhmr_render* h, const mhmr_render_args* a, const mhmr_render_extra* e, void* stream);
 
 /* Camera poses of the demo's views, on the device (demo.py:160-241 create_rotating_video, utils/render.py:407

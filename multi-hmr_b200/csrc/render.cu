@@ -3,12 +3,14 @@
 // runs through pyrender / OpenGL.  Here it is a z-buffer rasterizer over the meshes the engine leaves on the device.
 //
 // One call renders B views.  A view has its own intrinsics, an optional world->camera [R|t] (OpenCV convention) and a
-// background image; person p is drawn into every view whose image is person_image[p].  Four launches, no host sync:
+// background image.  The call draws meshes: mesh m < P is person m (the handle's body topology), drawn into every view
+// whose image is person_image[m]; mesh P + j is prop j (one of the handle's extra topologies), drawn into the views its
+// visibility flags allow.  Every stage runs once over all meshes.  Four launches, no host sync:
 //   1. prep     clears the 64-bit key buffer and the big-triangle queue; with smooth shading, one thread per
-//               (person, vertex) sums the angle-weighted face normals of its faces through a CSR built at create
+//               (mesh, vertex) sums the angle-weighted face normals of its faces through a CSR built at create
 //               (fixed order: no float atomics).
-//   2. raster   one thread per (view, person, face): transform, back-face cull, near-plane clip for the bounding box,
-//               coverage of the pixel centres, atomicMin of key = (z bits) << 32 | person << fbits | face.  A
+//   2. raster   one thread per (view, mesh, face): transform, back-face cull, near-plane clip for the bounding box,
+//               coverage of the pixel centres, atomicMin of key = (z bits) << 32 | mesh << fbits | face.  A
 //               triangle whose box exceeds kBigArea pixels goes to a queue instead.
 //   3. big      one CTA per queued triangle (persistent grid), its threads striding over the box.
 //   4. shade    one thread per output pixel: decode the key, perspective-correct barycentrics, pyrender's
@@ -159,32 +161,94 @@ __device__ __forceinline__ void write_key(unsigned long long* keys, float z, uns
   if (key < *reinterpret_cast<volatile unsigned long long*>(keys)) atomicMin(keys, key);
 }
 
+// Where a topology sits in the handle's concatenated arrays: faces [face_off, face_off + F) of `faces` (vertex indices
+// local to the topology), vertex -> (face, corner) entries [3 face_off, 3 (face_off + F)) of `csr_ent`, and V + 1
+// row pointers from ptr_off in `csr_ptr` (local to the topology's entries).  The body mesh, topology 0, starts them.
+struct Topo {
+  int face_off, F, ptr_off, V;
+};
+
 struct Params {
-  int views, H, W, P, F, V, fbits, smooth;
+  int views, H, W, P, F, V, fbits, smooth;  // F, V: the body mesh's
+  int nprops, prop_vmax;                    // props, largest prop vertex count (stride of the normal pass)
+  int person_blocks, prop_blocks;           // raster CTAs per person / per prop (128 faces each)
+  Topo prop_topo[MHMR_RENDER_MAX_PROPS];
+  int prop_vert_off[MHMR_RENDER_MAX_PROPS];  // first vertex of prop j in prop_verts
   const int* faces;
   const int* csr_ptr;
   const int* csr_ent;
   const float* verts;
+  const float* colors;
   const int* person_image;
   const int* view_image;
   const int* count;
+  const float* prop_verts;
+  const float* prop_colors;
+  const unsigned char* prop_visible;
   const float* K;
   const float* pose;
-  float* normals;
+  float* normals;  // persons' vertices [P, V], then the props' back to back
   unsigned long long* keys;
-  int2* queue;
+  int2* queue;     // (view, key low word) of the queued triangles
   int* queue_count;
 };
 
 __device__ __forceinline__ int person_count(const Params& a) { return min(max(*a.count, 0), a.P); }
 
+struct Mesh {
+  const float* verts;  // [V, 3]
+  const int* faces;    // [F, 3]
+  const int* csr_ptr;  // [V + 1]
+  const int* csr_ent;
+  float* normals;      // [V, 3]
+  const float* color;
+  int F, V;
+};
+
+// Mesh m of the call: person m for m < P, prop m - P after.
+__device__ __forceinline__ Mesh mesh_of(const Params& a, int m) {
+  Mesh M{a.verts + static_cast<size_t>(m) * a.V * 3, a.faces, a.csr_ptr, a.csr_ent,
+         a.normals + static_cast<size_t>(m) * a.V * 3, a.colors + 3 * m, a.F, a.V};
+  if (m >= a.P) {
+    const int j = m - a.P;
+    const Topo& t = a.prop_topo[j];
+    M.verts = a.prop_verts + static_cast<size_t>(a.prop_vert_off[j]) * 3;
+    M.faces = a.faces + 3ll * t.face_off;
+    M.csr_ptr = a.csr_ptr + t.ptr_off;
+    M.csr_ent = a.csr_ent + 3ll * t.face_off;
+    M.normals = a.normals + (static_cast<size_t>(a.P) * a.V + a.prop_vert_off[j]) * 3;
+    M.color = a.prop_colors + 3 * j;
+    M.F = t.F;
+    M.V = t.V;
+  }
+  return M;
+}
+
+// Whether mesh m is drawn into view b.  Every mesh tests the count first (props fail it: count <= P), so its load
+// does not wait for m; person_image is read for counted persons only.
+__device__ __forceinline__ bool drawn(const Params& a, int m, int b) {
+  if (m < person_count(a)) return a.person_image[m] == a.view_image[b];
+  return m >= a.P && (!a.prop_visible || a.prop_visible[static_cast<size_t>(b) * a.nprops + (m - a.P)]);
+}
+
+// A flat work index over n persons of `per_person` items each, then the props of `per_prop` items each:
+// (mesh, item within the mesh).
+template <typename I>  // unsigned int or unsigned long long
+__device__ __forceinline__ int2 mesh_item(const Params& a, I i, int n, int per_person, int per_prop) {
+  const I np = static_cast<I>(n) * static_cast<I>(per_person);
+  const bool person = i < np;
+  const I k = person ? i : i - np, per = static_cast<I>(person ? per_person : per_prop);
+  return make_int2((person ? 0 : a.P) + static_cast<int>(k / per), static_cast<int>(k % per));
+}
+
 // ---- 1. clear + vertex normals ----------------------------------------------------------------------------------
 // trimesh's vertex normals [3P-memory]: unit face normals weighted by the face's corner angle at the vertex, summed,
-// then normalised; a zero sum stays zero.
+// then normalised; a zero sum stays zero.  Persons past the count are not drawn and get none.
 __global__ void render_prep_kernel(Params a) {
   const long long npix = static_cast<long long>(a.views) * a.H * a.W;
   const int np = a.smooth ? person_count(a) : 0;
-  const long long total = npix + static_cast<long long>(np) * a.V;
+  const long long total =
+      npix + (a.smooth ? static_cast<long long>(np) * a.V + static_cast<long long>(a.nprops) * a.prop_vmax : 0);
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   if (blockIdx.x == 0 && threadIdx.x == 0) *a.queue_count = 0;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += stride) {
@@ -192,15 +256,16 @@ __global__ void render_prep_kernel(Params a) {
       a.keys[i] = kEmpty;
       continue;
     }
-    const long long j = i - npix;
-    const int p = static_cast<int>(j / a.V), v = static_cast<int>(j % a.V);
-    const float* vp = a.verts + static_cast<size_t>(p) * a.V * 3;
+    const int2 mv = mesh_item(a, static_cast<unsigned long long>(i - npix), np, a.V, a.prop_vmax);
+    const Mesh M = mesh_of(a, mv.x);
+    const int v = mv.y;
+    if (v >= M.V) continue;
     float3 acc = make_float3(0.f, 0.f, 0.f);
-    for (int q = a.csr_ptr[v]; q < a.csr_ptr[v + 1]; ++q) {
-      const int ent = a.csr_ent[q], f = ent / 3, corner = ent % 3;
-      const int* fc = a.faces + 3 * f;
-      const float3 p0 = load3(vp + 3 * fc[corner]), p1 = load3(vp + 3 * fc[(corner + 1) % 3]),
-                   p2 = load3(vp + 3 * fc[(corner + 2) % 3]);
+    for (int q = M.csr_ptr[v]; q < M.csr_ptr[v + 1]; ++q) {
+      const int ent = M.csr_ent[q], f = ent / 3, corner = ent % 3;
+      const int* fc = M.faces + 3 * f;
+      const float3 p0 = load3(M.verts + 3 * fc[corner]), p1 = load3(M.verts + 3 * fc[(corner + 1) % 3]),
+                   p2 = load3(M.verts + 3 * fc[(corner + 2) % 3]);
       const float3 fn = cross3(sub3(p1, p0), sub3(p2, p0));  // same orientation for every corner
       const float3 u = sub3(p1, p0), w = sub3(p2, p0);
       const float ang = atan2f(sqrtf(dot3(fn, fn)), dot3(u, w));
@@ -208,7 +273,7 @@ __global__ void render_prep_kernel(Params a) {
       acc.x = fmaf(ang, un.x, acc.x); acc.y = fmaf(ang, un.y, acc.y); acc.z = fmaf(ang, un.z, acc.z);
     }
     const float3 n = normalize3(acc);
-    float* out = a.normals + (static_cast<size_t>(p) * a.V + v) * 3;
+    float* out = M.normals + static_cast<size_t>(v) * 3;
     out[0] = n.x; out[1] = n.y; out[2] = n.z;
   }
 }
@@ -225,23 +290,28 @@ __device__ __forceinline__ void raster_box(const Params& a, const Tri& T, const 
   }
 }
 
+// grid (person_blocks per person, then prop_blocks per prop; views): the meshes of other views leave at once.
 __global__ void __launch_bounds__(128) render_raster_kernel(Params a) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  const int b = blockIdx.y / a.P, p = blockIdx.y % a.P;
-  if (p >= person_count(a) || a.person_image[p] != a.view_image[b] || f >= a.F) return;
+  const int b = blockIdx.y;
+  const int2 mb = mesh_item(a, blockIdx.x, a.P, a.person_blocks, a.prop_blocks);
+  const int m = mb.x, f = mb.y * blockDim.x + threadIdx.x;
+  if (!drawn(a, m, b)) return;
+  const Mesh M = mesh_of(a, m);
+  if (f >= M.F) return;
   const Cam c = load_cam(a.K, a.pose, b);
   if (!(c.fx > 0.f) || !(c.fy > 0.f)) return;
   Tri T;
-  if (!tri_setup(a.verts + static_cast<size_t>(p) * a.V * 3, a.faces + 3 * f, c, a.W, a.H, T)) return;
+  if (!tri_setup(M.verts, M.faces + 3 * f, c, a.W, a.H, T)) return;
+  const unsigned int low = (static_cast<unsigned int>(m) << a.fbits) | f;
   const int area = (T.x1 - T.x0 + 1) * (T.y1 - T.y0 + 1);
   if (area > kBigArea) {
     const int slot = atomicAdd(a.queue_count, 1);
     if (slot < kQueueCap) {
-      a.queue[slot] = make_int2(blockIdx.y, f);
+      a.queue[slot] = make_int2(b, static_cast<int>(low));
       return;
     }
   }
-  raster_box(a, T, c, b, (static_cast<unsigned int>(p) << a.fbits) | f, 0, 1);
+  raster_box(a, T, c, b, low, 0, 1);
 }
 
 // ---- 3. queued large triangles: one CTA each --------------------------------------------------------------------
@@ -249,91 +319,26 @@ __global__ void __launch_bounds__(256) render_raster_big_kernel(Params a) {
   const int nq = min(*a.queue_count, kQueueCap);
   for (int q = blockIdx.x; q < nq; q += gridDim.x) {
     const int2 ent = a.queue[q];
-    const int b = ent.x / a.P, p = ent.x % a.P, f = ent.y;
+    const int b = ent.x;
+    const unsigned int low = static_cast<unsigned int>(ent.y);
+    const Mesh M = mesh_of(a, static_cast<int>(low >> a.fbits));
+    const int f = static_cast<int>(low & ((1u << a.fbits) - 1u));
     const Cam c = load_cam(a.K, a.pose, b);
     Tri T;
-    if (!tri_setup(a.verts + static_cast<size_t>(p) * a.V * 3, a.faces + 3 * f, c, a.W, a.H, T)) continue;
-    raster_box(a, T, c, b, (static_cast<unsigned int>(p) << a.fbits) | f, threadIdx.x, blockDim.x);
+    if (!tri_setup(M.verts, M.faces + 3 * f, c, a.W, a.H, T)) continue;
+    raster_box(a, T, c, b, low, threadIdx.x, blockDim.x);
   }
-}
-
-// ---- props: extra meshes of other topologies in the same z-buffer ------------------------------------------------
-// Prop j is mesh P + j of the key.  Its topology's faces and CSR sit in the handle's concatenated topology arrays;
-// the per-prop offsets travel by value.
-struct Props {
-  int n, total_faces, total_verts;
-  int face_off[MHMR_RENDER_MAX_PROPS], nf[MHMR_RENDER_MAX_PROPS];   // into faces (in faces), of the topology
-  int ptr_off[MHMR_RENDER_MAX_PROPS], nv[MHMR_RENDER_MAX_PROPS];    // into csr_ptr, vertices of the topology
-  int vert_off[MHMR_RENDER_MAX_PROPS], fsum[MHMR_RENDER_MAX_PROPS]; // into verts / normals; faces of props < j
-  const int* faces;
-  const int* csr_ptr;
-  const int* csr_ent;
-  const float* verts;
-  const float* colors;
-  const unsigned char* visible;
-  float* normals;
-};
-
-__device__ __forceinline__ int prop_of_vertex(const Props& q, int i) {
-  int j = 0;
-  while (j + 1 < q.n && q.vert_off[j + 1] <= i) ++j;
-  return j;
-}
-
-__device__ __forceinline__ int prop_of_face(const Props& q, int i) {
-  int j = 0;
-  while (j + 1 < q.n && q.fsum[j + 1] <= i) ++j;
-  return j;
-}
-
-// Vertex normals of the props, as render_prep_kernel computes the persons'.
-__global__ void render_prop_normals_kernel(Props q) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= q.total_verts) return;
-  const int j = prop_of_vertex(q, i), v = i - q.vert_off[j];
-  const float* vp = q.verts + static_cast<size_t>(q.vert_off[j]) * 3;
-  const int* faces = q.faces + 3ll * q.face_off[j];
-  const int* ptr = q.csr_ptr + q.ptr_off[j];
-  float3 acc = make_float3(0.f, 0.f, 0.f);
-  for (int e = ptr[v]; e < ptr[v + 1]; ++e) {
-    const int ent = q.csr_ent[e], f = ent / 3, corner = ent % 3;
-    const int* fc = faces + 3 * f;
-    const float3 p0 = load3(vp + 3 * fc[corner]), p1 = load3(vp + 3 * fc[(corner + 1) % 3]),
-                 p2 = load3(vp + 3 * fc[(corner + 2) % 3]);
-    const float3 fn = cross3(sub3(p1, p0), sub3(p2, p0));
-    const float3 u = sub3(p1, p0), w = sub3(p2, p0);
-    const float ang = atan2f(sqrtf(dot3(fn, fn)), dot3(u, w));
-    const float3 un = normalize3(fn);
-    acc.x = fmaf(ang, un.x, acc.x); acc.y = fmaf(ang, un.y, acc.y); acc.z = fmaf(ang, un.z, acc.z);
-  }
-  const float3 n = normalize3(acc);
-  float* out = q.normals + static_cast<size_t>(i) * 3;
-  out[0] = n.x; out[1] = n.y; out[2] = n.z;
-}
-
-// One CTA per (prop face, view): props are few faces, often large on screen (a glyph next to the camera).
-__global__ void __launch_bounds__(128) render_prop_raster_kernel(Params a, Props q) {
-  const int b = blockIdx.y, j = prop_of_face(q, blockIdx.x), f = blockIdx.x - q.fsum[j];
-  if (q.visible && !q.visible[static_cast<size_t>(b) * q.n + j]) return;
-  const Cam c = load_cam(a.K, a.pose, b);
-  if (!(c.fx > 0.f) || !(c.fy > 0.f)) return;
-  Tri T;
-  if (!tri_setup(q.verts + static_cast<size_t>(q.vert_off[j]) * 3, q.faces + 3ll * (q.face_off[j] + f), c, a.W, a.H,
-                 T))
-    return;
-  raster_box(a, T, c, b, (static_cast<unsigned int>(a.P + j) << a.fbits) | f, threadIdx.x, blockDim.x);
 }
 
 // ---- 4. shading + composite -------------------------------------------------------------------------------------
 struct Shade {
   const unsigned char* images;
-  const float* colors;
   float alpha, intensity, metallic, roughness;
   unsigned char* overlay;
   float* depth;
   int* person;
-  const float* view_alpha;      // kExtra only: per-view alpha, or null
-  const int* view_background;   // kExtra only: per-view background image, or null
+  const float* view_alpha;  // per-view alpha, or null: alpha
+  const int* background;    // [views] background image of each view
 };
 
 // pyrender's metallic-roughness fragment shader (the glTF reference BRDF) for one white directional light along the
@@ -369,18 +374,14 @@ __device__ __forceinline__ float3 shade_pbr(float3 n, float3 v, float3 base, flo
   return make_float3(out[0], out[1], out[2]);
 }
 
-// kExtra: props, per-view alpha and backgrounds (mhmr_render_forward_extra); without, the one-topology path.
-template <bool kExtra>
-__global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s, Props q) {
+__global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s) {
   const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   const long long hw = static_cast<long long>(a.H) * a.W;
   if (i >= a.views * hw) return;
   const int b = static_cast<int>(i / hw), pix = static_cast<int>(i % hw), y = pix / a.W, x = pix % a.W;
   const unsigned long long* keys = a.keys + b * hw;
   const unsigned long long key = keys[pix];
-  const int bg_image = kExtra && s.view_background ? s.view_background[b] : a.view_image[b];
-  const float alpha = kExtra && s.view_alpha ? s.view_alpha[b] : s.alpha;
-  const unsigned char* bg = s.images + (static_cast<size_t>(bg_image) * hw + pix) * 3;
+  const unsigned char* bg = s.images + (static_cast<size_t>(s.background[b]) * hw + pix) * 3;
   unsigned char* out = s.overlay + i * 3;
   if (key == kEmpty) {  // fg = 0: the blend returns the photo exactly
     out[0] = bg[0]; out[1] = bg[1]; out[2] = bg[2];
@@ -401,19 +402,10 @@ __global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s, Pr
   const int p = static_cast<int>(low >> a.fbits), f = static_cast<int>(low & ((1u << a.fbits) - 1u));
   const float z = __uint_as_float(static_cast<unsigned int>(key >> 32));
   const Cam c = load_cam(a.K, a.pose, b);
-  const float* vp = a.verts + static_cast<size_t>(p) * a.V * 3;
-  const int* fc = a.faces + 3 * f;
-  const float* vn_base = a.normals + static_cast<size_t>(p) * a.V * 3;
-  const float* col = s.colors + 3 * p;
-  if (kExtra && p >= a.P) {
-    const int j = p - a.P;
-    vp = q.verts + static_cast<size_t>(q.vert_off[j]) * 3;
-    fc = q.faces + 3ll * (q.face_off[j] + f);
-    vn_base = q.normals + static_cast<size_t>(q.vert_off[j]) * 3;
-    col = q.colors + 3 * j;
-  }
+  const Mesh M = mesh_of(a, p);
+  const int* fc = M.faces + 3 * f;
   Tri T;
-  tri_setup(vp, fc, c, a.W, a.H, T);
+  tri_setup(M.verts, fc, c, a.W, a.H, T);
   const float rx = ray_x(c, x), ry = ray_y(c, y);
   float e[3];
 #pragma unroll
@@ -424,7 +416,7 @@ __global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s, Pr
     float3 acc = make_float3(0.f, 0.f, 0.f);
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-      const float3 vn = load3(vn_base + static_cast<size_t>(fc[k]) * 3);
+      const float3 vn = load3(M.normals + static_cast<size_t>(fc[k]) * 3);
       const float w = e[k] * inv;
       acc.x = fmaf(w, vn.x, acc.x); acc.y = fmaf(w, vn.y, acc.y); acc.z = fmaf(w, vn.z, acc.z);
     }
@@ -433,8 +425,10 @@ __global__ void __launch_bounds__(256) render_shade_kernel(Params a, Shade s, Pr
     n = normalize3(cross3(sub3(T.p[1], T.p[0]), sub3(T.p[2], T.p[0])));
   }
   const float3 v = normalize3(make_float3(-rx * z, -ry * z, -z));
-  const float3 rgb = shade_pbr(n, v, make_float3(col[0], col[1], col[2]), s.intensity, s.metallic, s.roughness);
+  const float3 rgb = shade_pbr(n, v, make_float3(M.color[0], M.color[1], M.color[2]), s.intensity, s.metallic,
+                               s.roughness);
   const float rgbv[3] = {rgb.x, rgb.y, rgb.z};
+  const float alpha = s.view_alpha ? s.view_alpha[b] : s.alpha;
 #pragma unroll
   for (int ch = 0; ch < 3; ++ch) {
     const float r8 = rintf(rgbv[ch] * 255.f);
@@ -586,7 +580,8 @@ __global__ void __launch_bounds__(kPoseThreads) render_pose_kernel(PoseArgs a) {
 }  // namespace
 
 struct mhmr_render {
-  int F = 0, V = 0, fbits = 0, nnz = 0;
+  int fbits = 0;
+  std::vector<Topo> topo;  // topology 0: the body mesh; then the extra topologies
   int* faces = nullptr;
   int* csr_ptr = nullptr;
   int* csr_ent = nullptr;
@@ -596,18 +591,10 @@ struct mhmr_render {
   size_t key_cap = 0;
   float* normals = nullptr;
   size_t normal_cap = 0;
-  // extra topologies: faces (local indices) and CSR back to back; per topology, host offsets
-  int* topo_faces = nullptr;
-  int* topo_ptr = nullptr;
-  int* topo_ent = nullptr;
-  float* prop_normals = nullptr;
-  size_t prop_normal_cap = 0;
-  std::vector<int> topo_face_off, topo_nf, topo_ptr_off, topo_nv;
   ~mhmr_render() {
     for (void* p : {static_cast<void*>(faces), static_cast<void*>(csr_ptr), static_cast<void*>(csr_ent),
                     static_cast<void*>(queue), static_cast<void*>(queue_count), static_cast<void*>(keys),
-                    static_cast<void*>(normals), static_cast<void*>(topo_faces), static_cast<void*>(topo_ptr),
-                    static_cast<void*>(topo_ent), static_cast<void*>(prop_normals)})
+                    static_cast<void*>(normals)})
       if (p) cudaFree(p);
   }
 };
@@ -625,8 +612,8 @@ int grow(T** buf, size_t* cap, size_t n) {
   return MHMR_OK;
 }
 
-// vertex -> incident (face, corner) entries, faces in increasing order; ptr values offset by `base`
-void build_csr(const int32_t* hf, int F, int V, int base, std::vector<int32_t>& ptr, std::vector<int32_t>& ent) {
+// vertex -> incident (face, corner) entries, faces in increasing order, appended to ptr / ent
+void build_csr(const int32_t* hf, int F, int V, std::vector<int32_t>& ptr, std::vector<int32_t>& ent) {
   const size_t p0 = ptr.size(), e0 = ent.size();
   ptr.resize(p0 + V + 1, 0);
   ent.resize(e0 + 3ll * F);
@@ -634,44 +621,32 @@ void build_csr(const int32_t* hf, int F, int V, int base, std::vector<int32_t>& 
   for (int v = 0; v < V; ++v) ptr[p0 + v + 1] += ptr[p0 + v];
   std::vector<int32_t> fill(ptr.begin() + p0, ptr.begin() + p0 + V);
   for (int i = 0; i < 3 * F; ++i) ent[e0 + fill[hf[i]]++] = i;
-  for (size_t i = p0; i < ptr.size(); ++i) ptr[i] += base;
 }
 
-int render_build_topologies(mhmr_render* h, const int32_t* topo_faces, int total_faces, cudaStream_t st) {
-  std::vector<int32_t> hf(3ll * total_faces), ptr, ent;
-  MHMR_CUDA_CHECK(cudaMemcpy(hf.data(), topo_faces, 12ll * total_faces, cudaMemcpyDefault));
-  for (size_t t = 0; t < h->topo_nf.size(); ++t) {
-    const int32_t* f = hf.data() + 3ll * h->topo_face_off[t];
-    for (int i = 0; i < 3 * h->topo_nf[t]; ++i)
-      MHMR_REQUIRE(f[i] >= 0 && f[i] < h->topo_nv[t], "topology face vertex index outside [0, its num_verts)");
-    h->topo_ptr_off.push_back(static_cast<int>(ptr.size()));
-    build_csr(f, h->topo_nf[t], h->topo_nv[t], static_cast<int>(ent.size()), ptr, ent);
+// Faces and CSR of every topology in h->topo, back to back: the body's from `faces`, the others' from `topo_faces`.
+int render_build(mhmr_render* h, const int32_t* faces, const int32_t* topo_faces, cudaStream_t st) {
+  const long long nbody = h->topo[0].F, total = h->topo.back().face_off + h->topo.back().F;
+  std::vector<int32_t> hf(3 * total), ptr, ent;
+  MHMR_CUDA_CHECK(cudaMemcpy(hf.data(), faces, 12 * nbody, cudaMemcpyDefault));
+  if (total > nbody)
+    MHMR_CUDA_CHECK(cudaMemcpy(hf.data() + 3 * nbody, topo_faces, 12 * (total - nbody), cudaMemcpyDefault));
+  for (size_t t = 0; t < h->topo.size(); ++t) {
+    Topo& tp = h->topo[t];
+    const int32_t* f = hf.data() + 3ll * tp.face_off;
+    for (int i = 0; i < 3 * tp.F; ++i)
+      MHMR_REQUIRE(f[i] >= 0 && f[i] < tp.V, (t == 0 ? "face vertex index outside [0, num_verts)"
+                                                     : "topology face vertex index outside [0, its num_verts)"));
+    tp.ptr_off = static_cast<int>(ptr.size());
+    build_csr(f, tp.F, tp.V, ptr, ent);
   }
-  MHMR_CUDA_CHECK(cudaMalloc(&h->topo_faces, 12ll * total_faces));
-  MHMR_CUDA_CHECK(cudaMalloc(&h->topo_ptr, 4ll * ptr.size()));
-  MHMR_CUDA_CHECK(cudaMalloc(&h->topo_ent, 4ll * ent.size()));
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->topo_faces, hf.data(), 12ll * total_faces, cudaMemcpyHostToDevice, st));
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->topo_ptr, ptr.data(), 4ll * ptr.size(), cudaMemcpyHostToDevice, st));
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->topo_ent, ent.data(), 4ll * ent.size(), cudaMemcpyHostToDevice, st));
-  MHMR_CUDA_CHECK(cudaStreamSynchronize(st));
-  return MHMR_OK;
-}
-
-int render_build(mhmr_render* h, const int32_t* faces, cudaStream_t st) {
-  const int F = h->F, V = h->V;
-  std::vector<int32_t> hf(3ll * F);
-  MHMR_CUDA_CHECK(cudaMemcpy(hf.data(), faces, 12ll * F, cudaMemcpyDefault));
-  for (int32_t v : hf) MHMR_REQUIRE(v >= 0 && v < V, "face vertex index outside [0, num_verts)");
-  std::vector<int32_t> ptr, ent;
-  build_csr(hf.data(), F, V, 0, ptr, ent);
-  MHMR_CUDA_CHECK(cudaMalloc(&h->faces, 12ll * F));
-  MHMR_CUDA_CHECK(cudaMalloc(&h->csr_ptr, 4ll * (V + 1)));
-  MHMR_CUDA_CHECK(cudaMalloc(&h->csr_ent, 12ll * F));
+  MHMR_CUDA_CHECK(cudaMalloc(&h->faces, 12 * total));
+  MHMR_CUDA_CHECK(cudaMalloc(&h->csr_ptr, 4 * ptr.size()));
+  MHMR_CUDA_CHECK(cudaMalloc(&h->csr_ent, 12 * total));
   MHMR_CUDA_CHECK(cudaMalloc(&h->queue, sizeof(int2) * kQueueCap));
   MHMR_CUDA_CHECK(cudaMalloc(&h->queue_count, sizeof(int)));
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->faces, hf.data(), 12ll * F, cudaMemcpyHostToDevice, st));
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->csr_ptr, ptr.data(), 4ll * (V + 1), cudaMemcpyHostToDevice, st));
-  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->csr_ent, ent.data(), 12ll * F, cudaMemcpyHostToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->faces, hf.data(), 12 * total, cudaMemcpyHostToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->csr_ptr, ptr.data(), 4 * ptr.size(), cudaMemcpyHostToDevice, st));
+  MHMR_CUDA_CHECK(cudaMemcpyAsync(h->csr_ent, ent.data(), 12 * total, cudaMemcpyHostToDevice, st));
   MHMR_CUDA_CHECK(cudaStreamSynchronize(st));  // the host vectors go out of scope
   return MHMR_OK;
 }
@@ -701,15 +676,11 @@ int mhmr_render_create_topologies(const int32_t* faces, int num_faces, int num_v
   while ((1ll << fbits) < max_faces) ++fbits;
   MHMR_REQUIRE(fbits <= 24, "at most 2^24 faces (the depth key keeps 32 bits for mesh and face)");
   auto* h = new mhmr_render();
-  h->F = num_faces; h->V = num_verts; h->fbits = fbits; h->nnz = 3 * num_faces;
-  for (int t = 0, off = 0; t < num_topologies; off += topo_num_faces[t++]) {
-    h->topo_face_off.push_back(off);
-    h->topo_nf.push_back(topo_num_faces[t]);
-    h->topo_nv.push_back(topo_num_verts[t]);
-  }
-  int rc = render_build(h, faces, static_cast<cudaStream_t>(stream));
-  if (rc == MHMR_OK && num_topologies > 0)
-    rc = render_build_topologies(h, topo_faces, static_cast<int>(total), static_cast<cudaStream_t>(stream));
+  h->fbits = fbits;
+  h->topo.push_back({0, num_faces, 0, num_verts});
+  for (int t = 0, off = num_faces; t < num_topologies; off += topo_num_faces[t++])
+    h->topo.push_back({off, topo_num_faces[t], 0, topo_num_verts[t]});
+  const int rc = render_build(h, faces, topo_faces, static_cast<cudaStream_t>(stream));
   if (rc != MHMR_OK) {
     delete h;
     return rc;
@@ -729,8 +700,8 @@ int mhmr_render_destroy(mhmr_render* h) {
 
 int mhmr_render_info(const mhmr_render* h, int* num_faces, int* num_verts, int* face_bits) {
   MHMR_REQUIRE(h != nullptr, "null renderer");
-  if (num_faces) *num_faces = h->F;
-  if (num_verts) *num_verts = h->V;
+  if (num_faces) *num_faces = h->topo[0].F;
+  if (num_verts) *num_verts = h->topo[0].V;
   if (face_bits) *face_bits = h->fbits;
   return MHMR_OK;
 }
@@ -744,21 +715,26 @@ int mhmr_render_forward_extra(mhmr_render* h, const mhmr_render_args* a, const m
   MHMR_REQUIRE(nprops >= 0 && nprops <= MHMR_RENDER_MAX_PROPS, "at most MHMR_RENDER_MAX_PROPS props");
   MHMR_REQUIRE(static_cast<long long>(a->max_persons) + nprops <= (1ll << (32 - h->fbits)),
                "max_persons does not fit the depth key next to the face index");
-  Props q{};
+  Params p{};
+  p.views = a->views; p.H = a->H; p.W = a->W; p.P = a->max_persons; p.F = h->topo[0].F; p.V = h->topo[0].V;
+  p.fbits = h->fbits; p.smooth = a->smooth ? 1 : 0;
+  p.person_blocks = (p.F + 127) / 128;
+  p.nprops = nprops;
+  int prop_verts = 0, prop_faces_max = 0;
   if (nprops > 0) {
     MHMR_REQUIRE(e->prop_topology && e->prop_verts && e->prop_colors, "null prop argument");
-    q.n = nprops;
     for (int j = 0; j < nprops; ++j) {
       const int t = e->prop_topology[j];
-      MHMR_REQUIRE(t >= 0 && t < static_cast<int>(h->topo_nf.size()), "prop topology outside the handle's");
-      q.face_off[j] = h->topo_face_off[t]; q.nf[j] = h->topo_nf[t];
-      q.ptr_off[j] = h->topo_ptr_off[t]; q.nv[j] = h->topo_nv[t];
-      q.vert_off[j] = q.total_verts; q.fsum[j] = q.total_faces;
-      q.total_verts += q.nv[j]; q.total_faces += q.nf[j];
+      MHMR_REQUIRE(t >= 0 && t < static_cast<int>(h->topo.size()) - 1, "prop topology outside the handle's");
+      p.prop_topo[j] = h->topo[1 + t];
+      p.prop_vert_off[j] = prop_verts;
+      prop_verts += p.prop_topo[j].V;
+      p.prop_vmax = std::max(p.prop_vmax, p.prop_topo[j].V);
+      prop_faces_max = std::max(prop_faces_max, p.prop_topo[j].F);
     }
-    q.faces = h->topo_faces; q.csr_ptr = h->topo_ptr; q.csr_ent = h->topo_ent;
-    q.verts = e->prop_verts; q.colors = e->prop_colors; q.visible = e->prop_visible;
+    p.prop_verts = e->prop_verts; p.prop_colors = e->prop_colors; p.prop_visible = e->prop_visible;
   }
+  p.prop_blocks = (prop_faces_max + 127) / 128;
   MHMR_REQUIRE(static_cast<long long>(a->views) * a->max_persons <= 65535, "views x max_persons exceeds 65535");
   MHMR_REQUIRE(a->images && a->view_image && a->K && a->verts && a->person_image && a->count && a->colors &&
                    a->overlay,
@@ -766,48 +742,33 @@ int mhmr_render_forward_extra(mhmr_render* h, const mhmr_render_args* a, const m
   MHMR_REQUIRE(a->alpha >= 0.f && a->alpha <= 1.f, "alpha must lie in [0, 1]");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t npix = static_cast<size_t>(a->views) * a->H * a->W;
+  const size_t mesh_verts = static_cast<size_t>(a->max_persons) * p.V + prop_verts;
   if (grow(&h->keys, &h->key_cap, npix) != MHMR_OK) return MHMR_ERR_CUDA;
-  if (a->smooth && grow(&h->normals, &h->normal_cap, static_cast<size_t>(a->max_persons) * h->V * 3) != MHMR_OK)
-    return MHMR_ERR_CUDA;
-  if (nprops > 0 && a->smooth &&
-      grow(&h->prop_normals, &h->prop_normal_cap, static_cast<size_t>(q.total_verts) * 3) != MHMR_OK)
-    return MHMR_ERR_CUDA;
-  q.normals = h->prop_normals;
-  Params p;
-  p.views = a->views; p.H = a->H; p.W = a->W; p.P = a->max_persons; p.F = h->F; p.V = h->V; p.fbits = h->fbits;
-  p.smooth = a->smooth ? 1 : 0;
+  if (a->smooth && grow(&h->normals, &h->normal_cap, mesh_verts * 3) != MHMR_OK) return MHMR_ERR_CUDA;
   p.faces = h->faces; p.csr_ptr = h->csr_ptr; p.csr_ent = h->csr_ent;
-  p.verts = a->verts; p.person_image = a->person_image; p.view_image = a->view_image; p.count = a->count;
-  p.K = a->K; p.pose = a->pose; p.normals = h->normals; p.keys = h->keys; p.queue = h->queue;
+  p.verts = a->verts; p.colors = a->colors; p.person_image = a->person_image; p.view_image = a->view_image;
+  p.count = a->count; p.K = a->K; p.pose = a->pose; p.normals = h->normals; p.keys = h->keys; p.queue = h->queue;
   p.queue_count = h->queue_count;
   Shade s;
-  s.images = a->images; s.colors = a->colors; s.alpha = a->alpha; s.intensity = a->intensity;
+  s.images = a->images; s.alpha = a->alpha; s.intensity = a->intensity;
   s.metallic = a->metallic; s.roughness = a->roughness; s.overlay = a->overlay; s.depth = a->depth;
   s.person = a->person;
   s.view_alpha = e ? e->view_alpha : nullptr;
-  s.view_background = e ? e->view_background : nullptr;
+  s.background = e && e->view_background ? e->view_background : a->view_image;
   const int sms = device_sm_count();
-  const size_t prep_work = npix + (a->smooth ? static_cast<size_t>(a->max_persons) * h->V : 0);
+  const size_t prep_work =
+      npix + (a->smooth ? static_cast<size_t>(a->max_persons) * p.V + static_cast<size_t>(nprops) * p.prop_vmax
+                        : 0);
   const int prep_blocks = static_cast<int>(std::min<size_t>((prep_work + 255) / 256, static_cast<size_t>(sms) * 16));
   render_prep_kernel<<<prep_blocks, 256, 0, st>>>(p);
   MHMR_CUDA_CHECK(cudaGetLastError());
-  render_raster_kernel<<<dim3((h->F + 127) / 128, a->views * a->max_persons), 128, 0, st>>>(p);
+  // (mesh, face block) on x, views on y: views <= 65535 follows from views x max_persons <= 65535
+  const unsigned raster_x = static_cast<unsigned>(p.P * p.person_blocks + nprops * p.prop_blocks);
+  render_raster_kernel<<<dim3(raster_x, a->views), 128, 0, st>>>(p);
   MHMR_CUDA_CHECK(cudaGetLastError());
-  if (nprops > 0) {
-    if (a->smooth) {
-      render_prop_normals_kernel<<<(q.total_verts + 255) / 256, 256, 0, st>>>(q);
-      MHMR_CUDA_CHECK(cudaGetLastError());
-    }
-    render_prop_raster_kernel<<<dim3(q.total_faces, a->views), 128, 0, st>>>(p, q);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-  }
   render_raster_big_kernel<<<sms * 8, 256, 0, st>>>(p);
   MHMR_CUDA_CHECK(cudaGetLastError());
-  const unsigned shade_blocks = static_cast<unsigned>((npix + 255) / 256);
-  if (e)
-    render_shade_kernel<true><<<shade_blocks, 256, 0, st>>>(p, s, q);
-  else
-    render_shade_kernel<false><<<shade_blocks, 256, 0, st>>>(p, s, q);
+  render_shade_kernel<<<static_cast<unsigned>((npix + 255) / 256), 256, 0, st>>>(p, s);
   MHMR_CUDA_CHECK(cudaGetLastError());
   return MHMR_OK;
 }

@@ -148,15 +148,11 @@ class Renderer:
         self.topology_verts = [int(t.max()) + 1 for t in topo]
         self._lib = _lib.load()
         h = torch.zeros(1, dtype=torch.int64)
+        tf = torch.cat(topo).contiguous() if topo else None
+        nf = torch.tensor([t.shape[0] for t in topo], dtype=torch.int32)
+        nv = torch.tensor(self.topology_verts, dtype=torch.int32)
         with torch.cuda.device(dev):
-            if topo:
-                tf = torch.cat(topo).contiguous()
-                nf = torch.tensor([t.shape[0] for t in topo], dtype=torch.int32)
-                nv = torch.tensor(self.topology_verts, dtype=torch.int32)
-                call("mhmr_render_create_topologies", self.faces, self.num_faces, V, len(topo), tf, nf, nv,
-                     stream(dev), h)
-            else:
-                call("mhmr_render_create", self.faces, self.num_faces, V, stream(dev), h)
+            call("mhmr_render_create_topologies", self.faces, self.num_faces, V, len(topo), tf, nf, nv, stream(dev), h)
         self._h = h.item()
         self._glyph = self._palette = None
         fb = torch.zeros(1, dtype=torch.int32)
@@ -241,10 +237,7 @@ class Renderer:
                            roughness=float(roughness), smooth=int(bool(smooth)), overlay=out["overlay"],
                            depth=out["depth"], person=out["index"])
         with torch.cuda.device(dev):
-            if extra is None:
-                call("mhmr_render_forward", self._h, args, stream(dev))
-            else:
-                call("mhmr_render_forward_extra", self._h, args, extra[0], stream(dev))
+            call("mhmr_render_forward_extra", self._h, args, None if extra is None else extra[0], stream(dev))
         return {k: v for k, v in out.items() if v is not None}
 
     def _extra(self, B, N, props, prop_visible, view_alpha, view_background):

@@ -7,7 +7,8 @@ Workloads: an 896 x 896 image with 4 persons; a 1920 x 1080 photo with 20 person
 a 20-frame rotating view of one image with 3 persons in one call (demo.py:160-195).  Meshes are seeded blob people
 (`synth.make_blob_people`) of 18 432 faces each, close to SMPL-X's 20 908, between 3 and 8 m from the camera.
 Then two `Renderer.render_views` workloads (see `view_workloads`; `--skip-views` leaves them out).  `--dump x.npz`
-saves the one-topology outputs, to compare builds bit for bit.
+saves every workload's outputs (overlay, depth and index; for the views also orbit and side), to compare builds bit
+for bit.
 """
 import argparse
 import json
@@ -33,6 +34,22 @@ def _people(n, W, H, f, seed):
     return synth.make_blob_people(np.stack([x, y, z], 1), seed=seed, n_lat=32, n_lon=48)
 
 
+def _kernel_ms(fn, n=20):
+    """Device time per call of each renderer kernel over n calls of fn, from torch.profiler."""
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(n):
+            fn()
+        torch.cuda.synchronize()
+    kern = {}
+    for ev in prof.key_averages():
+        if "render_" in ev.key:
+            short = ev.key.split("render_")[1].split("_kernel")[0]
+            kern[short] = round(ev.device_time_total / n / 1000.0, 4)
+    return kern
+
+
 def workloads():
     out = {}
     for name, (W, H, n, views) in {"896x896_4p": (896, 896, 4, 1), "1920x1080_20p": (1920, 1080, 20, 1),
@@ -51,7 +68,7 @@ def workloads():
     return out
 
 
-def view_workloads(res, args, dev):
+def view_workloads(res, args, dev, dumps):
     """Renderer.render_views: the demo orbit of one 1920 x 1080 photo with 3 persons (n_frames 20, angle_range 60:
     61 distinct views), and a batch of 8 images at 896 x 896 with 4 persons each taking the overlay, a 20-frame orbit
     and the three side views (with the camera glyph) in one call."""
@@ -67,9 +84,14 @@ def view_workloads(res, args, dev):
              "det_idx": torch.arange(P, dtype=torch.int32, device=dev).div(n, rounding_mode="floor").expand(3, P)
              .contiguous(), "count": torch.full((1,), P, dtype=torch.int32, device=dev),
              "transl_pelvis": torch.from_numpy(verts.mean(1)).to(dev)}
-        photos = torch.randint(0, 256, (B, H, W, 3), dtype=torch.uint8, device=dev)
+        photos = torch.randint(0, 256, (B, H, W, 3), dtype=torch.uint8, device=dev,
+                               generator=torch.Generator(dev).manual_seed(len(name)))
         K = torch.tensor([[f, 0, W / 2], [0, f, H / 2], [0, 0, 1]], dtype=torch.float32).expand(B, 3, 3).to(dev)
         kw = dict(orbit=(20, 60), side=side, alpha=0.8)
+        if args.dump:
+            o = r.render_views(t, photos, K, depth=True, index=True, **kw)
+            dumps.update({f"{name}_{k}": o[k].cpu().numpy() for k in ("overlay", "orbit", "side", "depth", "index")
+                          if k in o})
         for _ in range(args.warmup):
             r.render_views(t, photos, K, **kw)
         torch.cuda.synchronize()
@@ -81,10 +103,12 @@ def view_workloads(res, args, dev):
         e1.record()
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / calls
+        kern = _kernel_ms(lambda: r.render_views(t, photos, K, **kw), 10)
         views = B * (1 + 60 + (3 if side else 0))
         res["workloads"][name] = {"ms_per_call": round(ms, 4), "ms_per_view": round(ms / views, 4), "views": views,
-                                  "persons": P, "faces_per_person": int(faces.shape[0]), "calls": calls}
-        print(f"{name}: {ms:.3f} ms per call, {ms / views:.4f} ms per view ({views} views)")
+                                  "persons": P, "faces_per_person": int(faces.shape[0]), "calls": calls,
+                                  "kernel_ms_per_call": kern}
+        print(f"{name}: {ms:.3f} ms per call, {ms / views:.4f} ms per view ({views} views); kernels {kern}")
 
 
 def main():
@@ -93,7 +117,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--out", default=None)
     ap.add_argument("--skip-views", action="store_true", help="only the three one-topology workloads")
-    ap.add_argument("--dump", default=None, help="write the one-topology outputs of each workload to this .npz")
+    ap.add_argument("--dump", default=None, help="write the outputs of each workload to this .npz")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_render needs a CUDA device")
@@ -128,25 +152,15 @@ def main():
         e1.record()
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / args.calls
-        from torch.profiler import ProfilerActivity, profile
-
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(20):
-                r.render(verts, K, imgs, **kw)
-            torch.cuda.synchronize()
-        kern = {}
-        for ev in prof.key_averages():
-            if "render_" in ev.key:
-                short = ev.key.split("render_")[1].split("_kernel")[0]
-                kern[short] = round(ev.device_time_total / 20 / 1000.0, 4)
+        kern = _kernel_ms(lambda: r.render(verts, K, imgs, **kw))
         res["workloads"][name] = {"ms_per_call": round(ms, 4), "ms_per_view": round(ms / w["views"], 4),
                                   "views": w["views"], "persons": P, "faces_per_person": int(w["faces"].shape[0]),
                                   "kernel_ms_per_call": kern}
         print(f"{name}: {ms:.3f} ms per call, {ms / w['views']:.3f} ms per view; kernels {kern}")
+    if not args.skip_views:
+        view_workloads(res, args, dev, dumps)
     if args.dump:
         np.savez_compressed(args.dump, **dumps)
-    if not args.skip_views:
-        view_workloads(res, args, dev)
     line = json.dumps(res)
     print(line)
     if args.out:
