@@ -93,6 +93,39 @@ int mhmr_op_normalize_u8(const void* img_u8, const float* lut, float* out, int B
  * the workspace is stream-ordered (cudaMallocAsync / cudaFreeAsync).  Nothing else waits for the device. */
 int mhmr_op_letterbox_u8(const int64_t* photos, int B, int S, int pad, uint8_t* out, int32_t* boxes, void* stream);
 
+/* JPEG photos decoded on the device, byte for byte as Pillow's `Image.open(f).convert("RGB")` (libjpeg-turbo's
+ * default path: islow IDCT, fancy upsampling, fixed-point YCbCr -> RGB).  The device takes baseline / extended
+ * sequential Huffman files (SOF0, SOF1 at 8 bits) with 8-bit quantisation tables and one scan holding every component:
+ * grayscale, or YCbCr (JFIF, Adobe transform 1, or neither marker and component ids other than 'R', 'G', 'B') at
+ * 4:4:4, 4:2:2 or 4:2:0, any restart interval, the scan followed by EOI.  Every other file, and any malformed header,
+ * is for the host.
+ *
+ * Host only: reads the header of `data` (nbytes) and fills info[6] = width, height, components, luma h and v sampling
+ * (1, 1 for gray), eligible (0 / 1; the sizes are 0 when ineligible). */
+int mhmr_jpeg_info(const uint8_t* data, int64_t nbytes, int* info);
+
+/* Decodes B eligible JPEG files.
+ *   photos  HOST int64 [B, 7]: host address of the file's bytes, their count, device address of the same bytes (one
+ *           concatenated upload for the batch is the intended use), output device address of uint8 [H, W, 3] RGB,
+ *           its row pitch in bytes (>= 3 W), H, W (both as mhmr_jpeg_info reports them)
+ *   status  device int32 [B]: 0, or bits of what made the device decode unusable (1 a code with no table entry, 2 a
+ *           DC category above 11 or AC size above 10, 4 a run past coefficient 63, 8 the data ending before the
+ *           header's block count, 16 RSTn markers missing, extra or out of order, 32 an IDCT block outside the range
+ *           where libjpeg-turbo's SIMD and C IDCTs agree); such a photo's output is unspecified and the caller decodes
+ *           it on the host.
+ * Every argument, and every header, is checked before any launch; an ineligible file is MHMR_ERR_ARG.  The tables and
+ * layout of the batch go up in one cudaMemcpyAsync from pageable memory; the workspace is stream-ordered; nothing
+ * waits for the device. */
+int mhmr_op_jpeg_decode(const int64_t* photos, int B, int32_t* status, void* stream);
+
+/* Stage-level entry of the same decode up to the entropy stage, with the parallel Huffman decoder's subsequence
+ * length `subseq_bits` (>= 1) as a parameter: coefs (device int16) receives each photo's component planes back to
+ * back, [blocks high][blocks wide][64] natural-order coefficients (the padded MCU grid; one block per MCU and
+ * ceil(W/8) x ceil(H/8) blocks for gray); passes (device int32, nullable) the number of synchronisation passes the
+ * batch needed.  `photos` as for mhmr_op_jpeg_decode, output address and pitch unused. */
+int mhmr_op_jpeg_coefficients(const int64_t* photos, int B, int subseq_bits, int16_t* coefs, int32_t* status,
+                              int32_t* passes, void* stream);
+
 /* Person-decoder kernels (the per-person path after the backbone), each the engine's own launcher behind a thin
  * validating entry.  All pointers are device pointers; `count` is a device int32 holding the person count
  * (<= max_persons), read on the device as in the engine: grids are sized for max_persons and exit early, and rows

@@ -3,8 +3,9 @@
 
     open_image, get_camera_parameters, load_model, forward_model
 
-plus `open_images`, the batched form of `open_image`.  The letterbox (resize + pad) and the forward are H100-native;
-image decoding stays on the host (PIL), as in the reference.
+plus `open_images`, the batched form of `open_image`.  JPEG decoding (of the baseline files the device takes), the
+letterbox (resize + pad) and the forward are H100-native; other files are decoded on the host (PIL), as in the
+reference.
 """
 from __future__ import annotations
 
@@ -30,15 +31,22 @@ def normalize_rgb_device(img_u8: torch.Tensor) -> torch.Tensor:
     return ops.normalize_u8(img_u8.contiguous(), device_table(img_u8.device))
 
 
+def _upload_pil(im, device):
+    """A decoded RGB photo copied once into pinned memory and uploaded once."""
+    host = torch.empty((im.height, im.width, 3), dtype=torch.uint8, pin_memory=True)
+    host.numpy()[...] = np.asarray(im)
+    return host.to(device, non_blocking=True)
+
+
 def _letterbox_photos(imgs_pil, img_size, device, fused):
-    """Decoded RGB photos -> (batch, full-resolution uint8 [H, W, 3] device photos, boxes): each photo is copied once
-    into pinned memory and uploaded once; the device letterbox (`preprocess.letterbox`) makes the uint8 [B, S, S, 3]
-    batch, normalised to fp32 [B, 3, S, S] unless `fused`."""
-    photos = []
-    for im in imgs_pil:
-        host = torch.empty((im.height, im.width, 3), dtype=torch.uint8, pin_memory=True)
-        host.numpy()[...] = np.asarray(im)
-        photos.append(host.to(device, non_blocking=True))
+    """Decoded RGB photos -> (batch, full-resolution uint8 [H, W, 3] device photos, boxes): each photo is uploaded once
+    (`_upload_pil`) and letterboxed on the device (`_letterbox_device`)."""
+    return _letterbox_device([_upload_pil(im, device) for im in imgs_pil], img_size, fused)
+
+
+def _letterbox_device(photos, img_size, fused):
+    """Full-resolution uint8 [H, W, 3] device photos -> (batch, the photos, boxes): the device letterbox
+    (`preprocess.letterbox`) makes the uint8 [B, S, S, 3] batch, normalised to fp32 [B, 3, S, S] unless `fused`."""
     u8, boxes = letterbox(photos, img_size)
     if fused:
         return u8, photos, boxes
@@ -50,18 +58,52 @@ def _letterbox_photos(imgs_pil, img_size, device, fused):
 
 
 def open_images(paths, img_size, device=torch.device("cuda"), fused=False):
-    """`open_image` for a batch of photo files of any sizes, on the device: decodes on the host (PIL), uploads each
-    full-resolution photo once and letterboxes the batch there, byte for byte as `ImageOps.contain` + `ImageOps.pad`.
-    Returns (normalised fp32 [B, 3, S, S], or with `fused=True` the uint8 [B, S, S, 3] batch that `Model.forward` /
+    """`open_image` for a batch of photo files of any sizes, on the device.  Pillow first opens every file's header
+    in order (`Image.open`, which decodes nothing), so a file it refuses (not an image, a decompression bomb, ...)
+    raises exactly as before and no device memory is spent on it.  The bytes of the files Pillow opened as RGB or
+    gray go up in one pinned upload, and the baseline JPEGs among them are decoded there in one call
+    (`preprocess.decode_jpeg`), byte for byte as `Image.open(p).convert("RGB")`; their statuses come back in one host
+    synchronisation per batch.  Any other file (progressive or arithmetic-coded JPEG, CMYK, 4:1:1, PNG, ...) and any
+    JPEG whose entropy data the device flagged is decoded on the host with Pillow, in file order, and uploaded once.
+    The batch is then letterboxed on the device, byte for byte as `ImageOps.contain` + `ImageOps.pad`.  Returns
+    (normalised fp32 [B, 3, S, S], or with `fused=True` the uint8 [B, S, S, 3] batch that `Model.forward` /
     `forward_model` take through the fused loader; the full-resolution uint8 [H, W, 3] device photos, the renderer's
     backgrounds; int32 [B, 4] host tensor of (x0, y0, new_w, new_h), each photo's box in the square)."""
     from PIL import Image
 
+    from .preprocess import decode_jpeg
+
     device = torch.device(device)
     if device.type != "cuda":
         raise ValueError("open_images letterboxes on a CUDA device (open_image is the host path)")
-    with torch.cuda.device(device):
-        return _letterbox_photos([Image.open(p).convert("RGB") for p in paths], img_size, device, fused)
+    # Headers in file order; Pillow's decode of file i used to run before file i + 1 was opened, so an open error is
+    # raised only after the files before it have been decoded (and have raised, if they fail to decode).
+    ims, open_error = [], None
+    for p in paths:
+        try:
+            ims.append(Image.open(p))
+        except Exception as err:   # noqa: BLE001  (re-raised below, unchanged)
+            open_error = err
+            break
+    try:
+        blobs = []
+        for p, im in zip(paths, ims):
+            if im.mode in ("RGB", "L"):
+                with open(p, "rb") as fh:
+                    blobs.append(fh.read())
+            else:
+                blobs.append(b"")
+        with torch.cuda.device(device):
+            photos, ok = decode_jpeg(blobs, device)
+            for i, im in enumerate(ims):
+                if not (ok[i] and im.size == (photos[i].shape[1], photos[i].shape[0])):
+                    photos[i] = _upload_pil(im.convert("RGB"), device)
+            if open_error is not None:
+                raise open_error
+            return _letterbox_device(photos, img_size, fused)
+    finally:
+        for im in ims:
+            im.close()
 
 
 def open_image(img_path, img_size, device=torch.device("cuda"), fused=False):

@@ -81,6 +81,75 @@ def letterbox_u8(photos, S, pad=0):
     return out, boxes
 
 
+def jpeg_info(data):
+    """(width, height, components, luma h, luma v, eligible) of a JPEG file's bytes (host only, `mhmr_jpeg_info`):
+    eligible files are the ones `jpeg_decode` takes; the sizes are 0 for the others."""
+    data = bytes(data)
+    info = torch.zeros(6, dtype=torch.int32)
+    call("mhmr_jpeg_info", data if data else b"\0", len(data), info)
+    return tuple(info.tolist())
+
+
+def _jpeg_desc(host, dev, spans, sizes, outs):
+    assert host.dtype == torch.uint8 and not host.is_cuda and host.is_contiguous()
+    assert dev.dtype == torch.uint8 and dev.is_cuda and dev.is_contiguous() and dev.numel() == host.numel()
+    desc = torch.zeros(len(spans), 7, dtype=torch.int64)
+    for i, ((off, n), (h, w)) in enumerate(zip(spans, sizes)):
+        assert 0 <= off and off + n <= host.numel(), "span outside the uploaded bytes"
+        o = outs[i] if outs is not None else None
+        desc[i] = torch.tensor([host.data_ptr() + off, n, dev.data_ptr() + off, 0 if o is None else o.data_ptr(),
+                                0 if o is None else o.stride(0), h, w])
+    return desc
+
+
+def jpeg_decode(host, dev, spans, outs):
+    """Decodes JPEG files on the device (`mhmr_op_jpeg_decode`): `host` is the uint8 CPU tensor of the files' bytes
+    back to back, `dev` its copy on the device, `spans` each file's (offset, length), `outs` uint8 [H, W, 3] CUDA
+    tensors (channels contiguous, rows may be padded).  Returns the device int32 [B] status (0: the photo equals
+    Pillow's `convert("RGB")`); nothing waits for the device."""
+    _cuda(dev, *outs)
+    for o in outs:
+        assert o.dtype == torch.uint8 and o.dim() == 3 and o.shape[2] == 3 and o.stride(2) == 1 and o.stride(1) == 3 \
+            and o.device == dev.device, "uint8 [H, W, 3] outputs with contiguous pixels on the bytes' device expected"
+    desc = _jpeg_desc(host, dev, spans, [tuple(o.shape[:2]) for o in outs], outs)
+    status = torch.empty(len(spans), dtype=torch.int32, device=dev.device)
+    with torch.cuda.device(dev.device):
+        call("mhmr_op_jpeg_decode", desc, len(spans), status, stream())
+    return status
+
+
+def jpeg_plane_blocks(w, h, ncomp, hs, vs):
+    """[(blocks wide, blocks high)] of each component's coefficient plane (the padded MCU grid)."""
+    if ncomp == 1:
+        return [(-(-w // 8), -(-h // 8))]
+    mx, my = -(-w // (8 * hs)), -(-h // (8 * vs))
+    return [(mx * hs, my * vs), (mx, my), (mx, my)]
+
+
+def jpeg_coefficients(host, dev, spans, subseq_bits):
+    """The entropy stage alone at a given subsequence length (`mhmr_op_jpeg_coefficients`): (per photo, per
+    component int16 [blocks high, blocks wide, 64] natural-order coefficients on the device, device int32 [B] status,
+    device int32 [1] synchronisation passes)."""
+    _cuda(dev)
+    infos = [jpeg_info(host[o:o + n].numpy().tobytes()) for o, n in spans]
+    assert all(i[5] for i in infos), "every file must be eligible"
+    planes = [jpeg_plane_blocks(*i[:5]) for i in infos]
+    total = sum(bw * bh * 64 for p in planes for bw, bh in p)
+    coefs = torch.empty(total, dtype=torch.int16, device=dev.device)
+    status = torch.empty(len(spans), dtype=torch.int32, device=dev.device)
+    passes = torch.zeros(1, dtype=torch.int32, device=dev.device)
+    desc = _jpeg_desc(host, dev, spans, [(i[1], i[0]) for i in infos], None)
+    with torch.cuda.device(dev.device):
+        call("mhmr_op_jpeg_coefficients", desc, len(spans), subseq_bits, coefs, status, passes, stream())
+    out, pos = [], 0
+    for p in planes:
+        out.append([])
+        for bw, bh in p:
+            out[-1].append(coefs[pos:pos + bw * bh * 64].view(bh, bw, 64))
+            pos += bw * bh * 64
+    return out, status, passes
+
+
 def attention(qkv, B, T, D, out=None):
     """qkv [B*T, 3*D] fp16 -> out [B*T, D] fp16, heads of 64 dims, softmax(q k^T / 8) v per image."""
     _cuda(qkv)

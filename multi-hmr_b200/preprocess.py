@@ -1,6 +1,7 @@
 """Host statement of the reference's image normalisation (utils/image.py:8-24) and the [3][256] table that the
-device kernels (`mhmr_op_normalize_u8`, the fused loader of `mhmr_forward_u8`) use to reproduce it bit for bit, and
-the device letterbox of photos of any size (`ImageOps.contain` + `ImageOps.pad`, demo.py:27-51)."""
+device kernels (`mhmr_op_normalize_u8`, the fused loader of `mhmr_forward_u8`) use to reproduce it bit for bit, the
+device letterbox of photos of any size (`ImageOps.contain` + `ImageOps.pad`, demo.py:27-51), and the device decode of
+JPEG files (`Image.open(f).convert("RGB")`, byte for byte, for the baseline files it takes)."""
 from __future__ import annotations
 
 import numpy as np
@@ -38,6 +39,51 @@ def letterbox(photos, img_size: int, color: int = 0):
     dev = next((p.device for p in photos if p.is_cuda), torch.device("cuda"))
     photos = [p if p.is_cuda else p.pin_memory().to(dev, non_blocking=True) for p in photos]
     return ops.letterbox_u8(photos, img_size, color)
+
+
+def upload_bytes(blobs, device):
+    """The byte strings back to back in one pinned host tensor and one non-blocking upload: (host, device copy,
+    [(offset, length)])."""
+    import torch
+
+    spans, off = [], 0
+    for b in blobs:
+        spans.append((off, len(b)))
+        off += len(b)
+    host = torch.empty(max(off, 1), dtype=torch.uint8, pin_memory=True)
+    view = host.numpy()
+    for (o, n), b in zip(spans, blobs):
+        view[o:o + n] = np.frombuffer(b, dtype=np.uint8)
+    return host, host.to(device, non_blocking=True), spans
+
+
+def decode_jpeg(blobs, device):
+    """JPEG files' bytes -> (uint8 [H, W, 3] RGB device photos, ok flags), byte for byte `Image.open(f).convert("RGB")`
+    (csrc/jpeg.cu; the arithmetic is restated in oracle/jpeg_ref.py).  Eligible files (`ops.jpeg_info`) are decoded in
+    one call; a photo is None and its flag False when the file is not eligible, has more pixels than Pillow's
+    `Image.MAX_IMAGE_PIXELS` (Pillow warns about such files or refuses them as decompression bombs; nothing is
+    allocated for them here), or its entropy data was flagged (the caller decodes those with Pillow).  The bytes go up
+    in one pinned upload; the statuses come back in one host sync."""
+    import torch
+    from PIL import Image
+
+    from . import ops
+
+    device = torch.device(device)
+    limit = Image.MAX_IMAGE_PIXELS
+    infos = [ops.jpeg_info(b) for b in blobs]
+    idx = [i for i, info in enumerate(infos) if info[5] and (limit is None or info[0] * info[1] <= limit)]
+    photos, ok = [None] * len(blobs), [False] * len(blobs)
+    if not idx:
+        return photos, ok
+    with torch.cuda.device(device):
+        host, dev, spans = upload_bytes([blobs[i] for i in idx], device)
+        outs = [torch.empty((infos[i][1], infos[i][0], 3), dtype=torch.uint8, device=device) for i in idx]
+        status = ops.jpeg_decode(host, dev, spans, outs).cpu().tolist()
+    for i, o, s in zip(idx, outs, status):
+        if s == 0:
+            photos[i], ok[i] = o, True
+    return photos, ok
 
 
 _LUT_CACHE = {}
