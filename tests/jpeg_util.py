@@ -81,6 +81,86 @@ def saturating_quantisers() -> bytes:
     return bytes(edited)
 
 
+def bit_readers(data: bytes):
+    """The bit readers of the restatement's sequential decode, one per restart interval it decoded, as they stopped:
+    `pos` is where the interval's last block ended (its 1-padding follows) or where an anomaly stopped the decode,
+    `n` the interval's destuffed bits."""
+    from oracle import jpeg_ref as jr
+
+    made = []
+
+    class Recorder(jr._Bits):
+        def __init__(self, buf):
+            super().__init__(buf)
+            made.append(self)
+
+    keep, jr._Bits = jr._Bits, Recorder
+    try:
+        jr.decode_coefficients(data, jr.parse(data))
+    finally:
+        jr._Bits = keep
+    return made
+
+
+def _kept_offsets(data: bytes):
+    """Per restart interval, the file offset of each destuffed byte (the 0xFF of a stuffed pair stands for it)."""
+    s, e = ecs_span(data)
+    out, cur, i = [], [], s
+    while i < e:
+        if data[i] == 0xFF:
+            if data[i + 1] == 0:
+                cur.append(i)
+            else:
+                out.append(cur)
+                cur = []
+            i += 2
+            continue
+        cur.append(i)
+        i += 1
+    out.append(cur)
+    return out
+
+
+def corruptions(rng, data):
+    """Seeded corruptions of a clean file's entropy-coded segment: (kind, bytes).  Bit flips, truncation (EOI kept),
+    and with restart markers: one dropped or swapped, non-0xFF garbage before one (libjpeg skips it), an empty interval
+    (two adjacent RSTn), a truncation exactly at an interval boundary, bit flips confined to an interval's 1-padding
+    (nothing reads those bits: the file must stay exact), and a duplicated RSTn once the index has wrapped past 7."""
+    s, e = ecs_span(data)
+    out = []
+    for _ in range(12):
+        b = bytearray(data)
+        for _ in range(int(rng.integers(1, 4))):
+            i = int(rng.integers(s, e))
+            b[i] ^= 1 << int(rng.integers(0, 8))
+        out.append(("flip", bytes(b)))
+    for _ in range(4):
+        cut = int(rng.integers(s, e))
+        out.append(("truncate", data[:cut] + b"\xff\xd9"))
+    ends, kept = [b.pos for b in bit_readers(data)], _kept_offsets(data)
+    padded = [i for i, (end, k) in enumerate(zip(ends, kept)) if end < 8 * len(k)]
+    for _ in range(2 if padded else 0):
+        iv = padded[int(rng.integers(0, len(padded)))]
+        p = int(rng.integers(ends[iv], 8 * len(kept[iv])))
+        out.append(("padding flip", edit(data, kept[iv][p >> 3], [data[kept[iv][p >> 3]] ^ (0x80 >> (p & 7))])))
+    rst = [i for i in range(s, e - 1) if data[i] == 0xFF and 0xD0 <= data[i + 1] <= 0xD7]
+    if len(rst) >= 2:
+        i = rst[int(rng.integers(0, len(rst)))]
+        out.append(("drop rst", data[:i] + data[i + 2:]))
+        i, j = rst[0], rst[1]
+        out.append(("swap rst", edit(edit(data, i + 1, [data[j + 1]]), j + 1, [data[i + 1]])))
+        i = rst[int(rng.integers(0, len(rst)))]
+        garbage = bytes(int(v) for v in rng.integers(0, 255, int(rng.integers(1, 6))))
+        out.append(("garbage before rst", data[:i] + garbage + data[i:]))
+        k = int(rng.integers(0, len(rst) - 1))
+        out.append(("empty interval", data[:rst[k] + 2] + data[rst[k + 1]:]))
+        out.append(("truncate at rst", data[:rst[int(rng.integers(0, len(rst)))]] + b"\xff\xd9"))
+    if len(rst) >= 9:
+        i = rst[int(rng.integers(8, len(rst)))]
+        out.append(("duplicate wrapped rst", data[:i + 2] + data[i:]))
+    return out
+
+
 def bomb_header() -> bytes:
     """A small 4:4:4 JPEG whose SOF claims 65535 x 65535 pixels: eligible by its header, a decompression bomb to
     Pillow."""
