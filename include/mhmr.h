@@ -126,6 +126,38 @@ int mhmr_op_jpeg_decode(const int64_t* photos, int B, int32_t* status, void* str
 int mhmr_op_jpeg_coefficients(const int64_t* photos, int B, int subseq_bits, int16_t* coefs, int32_t* status,
                               int32_t* passes, void* stream);
 
+/* PNG photos decoded on the device, byte for byte as Pillow's `Image.open(f).convert("RGB")`.  The device takes
+ * non-interlaced files of bit depth 8 in colour types 0 (gray), 2 (RGB), 3 (palette), 4 (gray + alpha) and 6 (RGBA)
+ * whose chunks are laid out as IHDR first, a PLTE before the IDATs for type 3, one run of IDAT chunks, then IEND, with
+ * the CRCs Pillow checks intact and only the ancillary chunks Pillow reads without raising or warning.
+ *
+ * Host only: reads the chunks of `data` (nbytes) and fills info[4] = width, height, colour type, eligible (0 / 1;
+ * the others are 0 when ineligible). */
+int mhmr_png_info(const uint8_t* data, int64_t nbytes, int* info);
+
+/* Decodes B eligible PNG files.
+ *   photos  HOST int64 [B, 8]: host address of the file's bytes, their count, device address of the file's zlib
+ *           stream (its IDAT payloads back to back; one concatenated upload for the batch is the intended use), the
+ *           stream's bytes, output device address of uint8 [H, W, 3] RGB, its row pitch in bytes (>= 3 W), H, W
+ *   status  device int32 [B]: 0, or bits of what made the device decode unusable (1 an invalid block type, stored
+ *           length, code-length code, code lengths, Huffman code or symbol, 2 a distance reaching before the
+ *           stream's first byte, 4 a block reading past the stream or more blocks than the chain holds, 8 an inflated
+ *           length other than H (1 + row bytes), 16 a filter byte above 4, 32 the Adler-32 missing or different,
+ *           64 a bad zlib header or a preset dictionary); such a photo's output is unspecified and the caller decodes
+ *           it on the host.
+ * Every argument, and every file, is checked before any launch; an ineligible file is MHMR_ERR_ARG.  The
+ * descriptors and palettes go up in one cudaMemcpyAsync; the workspace is stream-ordered; nothing waits for the
+ * device. */
+int mhmr_op_png_decode(const int64_t* photos, int B, int32_t* status, void* stream);
+
+/* Stage-level entry of the same inflate: B raw zlib streams to their inflated bytes.
+ *   streams HOST int64 [B, 4]: device address of the stream, its bytes, device address of the output, its expected
+ *           inflated length (a stream inflating to any other length has status bit 8)
+ *   status  device int32 [B] as for mhmr_op_png_decode (bits 1-8, 32, 64)
+ *   counts  device int32 [B, 4] (nullable): chain blocks, header candidates found, chain blocks that were not
+ *           candidates (decoded on the slow path), inflated bytes. */
+int mhmr_op_png_inflate(const int64_t* streams, int B, int32_t* status, int32_t* counts, void* stream);
+
 /* Person-decoder kernels (the per-person path after the backbone), each the engine's own launcher behind a thin
  * validating entry.  All pointers are device pointers; `count` is a device int32 holding the person count
  * (<= max_persons), read on the device as in the engine: grids are sized for max_persons and exit early, and rows

@@ -3,7 +3,7 @@
 
     open_image, get_camera_parameters, load_model, forward_model
 
-plus `open_images`, the batched form of `open_image`.  JPEG decoding (of the baseline files the device takes), the
+plus `open_images`, the batched form of `open_image`.  JPEG and PNG decoding (of the files the device takes), the
 letterbox (resize + pad) and the forward are H100-native; other files are decoded on the host (PIL), as in the
 reference.
 """
@@ -60,18 +60,20 @@ def _letterbox_device(photos, img_size, fused):
 def open_images(paths, img_size, device=torch.device("cuda"), fused=False):
     """`open_image` for a batch of photo files of any sizes, on the device.  Pillow first opens every file's header
     in order (`Image.open`, which decodes nothing), so a file it refuses (not an image, a decompression bomb, ...)
-    raises exactly as before and no device memory is spent on it.  The bytes of the files Pillow opened as RGB or
-    gray go up in one pinned upload, and the baseline JPEGs among them are decoded there in one call
-    (`preprocess.decode_jpeg`), byte for byte as `Image.open(p).convert("RGB")`; their statuses come back in one host
-    synchronisation per batch.  Any other file (progressive or arithmetic-coded JPEG, CMYK, 4:1:1, PNG, ...) and any
-    JPEG whose entropy data the device flagged is decoded on the host with Pillow, in file order, and uploaded once.
+    raises exactly as before and no device memory is spent on it.  The bytes of the files Pillow opened as RGB or gray
+    go up in one pinned upload, and the baseline ones among them are decoded there in one call
+    (`preprocess.decode_jpeg`); the PNGs it opened as RGB, gray, palette, RGBA or gray + alpha go up in another, and
+    the eligible ones (8-bit, not interlaced) are decoded there in one call (`preprocess.decode_png`).  Both are byte
+    for byte `Image.open(p).convert("RGB")`; each call's statuses come back in one host synchronisation.  Any other
+    file (progressive or arithmetic-coded JPEG, CMYK, 4:1:1, interlaced or 16-bit PNG, ...) and any file the device
+    flagged is decoded on the host with Pillow, in file order, and uploaded once.
     The batch is then letterboxed on the device, byte for byte as `ImageOps.contain` + `ImageOps.pad`.  Returns
     (normalised fp32 [B, 3, S, S], or with `fused=True` the uint8 [B, S, S, 3] batch that `Model.forward` /
     `forward_model` take through the fused loader; the full-resolution uint8 [H, W, 3] device photos, the renderer's
     backgrounds; int32 [B, 4] host tensor of (x0, y0, new_w, new_h), each photo's box in the square)."""
     from PIL import Image
 
-    from .preprocess import decode_jpeg
+    from .preprocess import decode_jpeg, decode_png
 
     device = torch.device(device)
     if device.type != "cuda":
@@ -86,15 +88,23 @@ def open_images(paths, img_size, device=torch.device("cuda"), fused=False):
             open_error = err
             break
     try:
-        blobs = []
+        jpegs, pngs = [], []
         for p, im in zip(paths, ims):
-            if im.mode in ("RGB", "L"):
+            jpeg = im.mode in ("RGB", "L")
+            png = im.format == "PNG" and im.mode in ("RGB", "L", "P", "RGBA", "LA")
+            blob = b""
+            if jpeg or png:
                 with open(p, "rb") as fh:
-                    blobs.append(fh.read())
-            else:
-                blobs.append(b"")
+                    blob = fh.read()
+            jpegs.append(blob if jpeg else b"")
+            pngs.append(blob if png else b"")
         with torch.cuda.device(device):
-            photos, ok = decode_jpeg(blobs, device)
+            photos, ok = decode_jpeg(jpegs, device)
+            if any(pngs):
+                png_photos, png_ok = decode_png(pngs, device)
+                for i, good in enumerate(png_ok):
+                    if good:
+                        photos[i], ok[i] = png_photos[i], True
             for i, im in enumerate(ims):
                 if not (ok[i] and im.size == (photos[i].shape[1], photos[i].shape[0])):
                     photos[i] = _upload_pil(im.convert("RGB"), device)

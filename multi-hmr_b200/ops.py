@@ -150,6 +150,73 @@ def jpeg_coefficients(host, dev, spans, subseq_bits):
     return out, status, passes
 
 
+def png_info(data):
+    """(width, height, colour type, eligible) of a PNG file's bytes (host only, `mhmr_png_info`): eligible files are
+    the ones `png_decode` takes; the sizes are 0 for the others."""
+    data = bytes(data)
+    info = torch.zeros(4, dtype=torch.int32)
+    call("mhmr_png_info", data if data else b"\0", len(data), info)
+    return tuple(info.tolist())
+
+
+def png_idat(data):
+    """The zlib stream of an eligible PNG file: its IDAT payloads back to back."""
+    data = memoryview(bytes(data))
+    out, pos = [], 8
+    while pos + 8 <= len(data):
+        n = int.from_bytes(data[pos:pos + 4], "big")
+        kind = bytes(data[pos + 4:pos + 8])
+        if kind == b"IDAT":
+            out.append(data[pos + 8:pos + 8 + n])
+        elif out:
+            break
+        pos += 12 + n
+    return b"".join(out)
+
+
+def png_decode(files, host, dev, spans, outs):
+    """Decodes PNG files on the device (`mhmr_op_png_decode`): `files` the files' bytes, `host` the uint8 CPU tensor of
+    their zlib streams (`png_idat`) back to back, `dev` its copy on the device, `spans` each stream's (offset, length),
+    `outs` uint8 [H, W, 3] CUDA tensors (channels contiguous, rows may be padded).  Returns the device int32 [B] status
+    (0: the photo equals Pillow's `convert("RGB")`); nothing waits for the device."""
+    _cuda(dev, *outs)
+    assert host.dtype == torch.uint8 and not host.is_cuda and host.is_contiguous()
+    assert dev.dtype == torch.uint8 and dev.is_cuda and dev.is_contiguous() and dev.numel() == host.numel()
+    desc = torch.zeros(len(spans), 8, dtype=torch.int64)
+    keep = [bytes(f) for f in files]   # alive until the call returns: the entry reads each file's chunks
+    for i, (f, (off, n), o) in enumerate(zip(keep, spans, outs)):
+        assert o.dtype == torch.uint8 and o.dim() == 3 and o.shape[2] == 3 and o.stride(2) == 1 and o.stride(1) == 3 \
+            and o.device == dev.device, "uint8 [H, W, 3] outputs with contiguous pixels on the bytes' device expected"
+        assert 0 <= off and off + n <= host.numel(), "span outside the uploaded bytes"
+        fb = torch.frombuffer(bytearray(f), dtype=torch.uint8) if f else torch.zeros(1, dtype=torch.uint8)
+        keep.append(fb)
+        desc[i] = torch.tensor([fb.data_ptr(), len(f), dev.data_ptr() + off, n, o.data_ptr(),
+                                o.stride(0) if o.shape[0] > 1 else 3 * o.shape[1], o.shape[0], o.shape[1]])
+    status = torch.empty(len(spans), dtype=torch.int32, device=dev.device)
+    with torch.cuda.device(dev.device):
+        call("mhmr_op_png_decode", desc, len(spans), status, stream())
+    return status
+
+
+def png_inflate(dev, spans, lengths):
+    """Raw zlib streams -> their inflated bytes on the device (`mhmr_op_png_inflate`): `dev` the uint8 CUDA tensor of
+    the streams back to back, `spans` each stream's (offset, length), `lengths` each one's expected inflated length.
+    Returns (per stream a uint8 CUDA tensor of that length, device int32 [B] status, device int32 [B, 4] counts: chain
+    blocks, header candidates, slow-path blocks, inflated bytes)."""
+    _cuda(dev)
+    assert dev.dtype == torch.uint8 and dev.is_contiguous()
+    outs = [torch.empty(max(int(n), 1), dtype=torch.uint8, device=dev.device) for n in lengths]
+    desc = torch.zeros(len(spans), 4, dtype=torch.int64)
+    for i, ((off, n), o, want) in enumerate(zip(spans, outs, lengths)):
+        assert 0 <= off and off + n <= dev.numel() and want >= 1, "span outside the bytes, or an empty output"
+        desc[i] = torch.tensor([dev.data_ptr() + off, n, o.data_ptr(), want])
+    status = torch.empty(len(spans), dtype=torch.int32, device=dev.device)
+    counts = torch.empty(len(spans), 4, dtype=torch.int32, device=dev.device)
+    with torch.cuda.device(dev.device):
+        call("mhmr_op_png_inflate", desc, len(spans), status, counts, stream())
+    return outs, status, counts
+
+
 def attention(qkv, B, T, D, out=None):
     """qkv [B*T, 3*D] fp16 -> out [B*T, D] fp16, heads of 64 dims, softmax(q k^T / 8) v per image."""
     _cuda(qkv)

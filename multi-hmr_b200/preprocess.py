@@ -1,7 +1,7 @@
 """Host statement of the reference's image normalisation (utils/image.py:8-24) and the [3][256] table that the
 device kernels (`mhmr_op_normalize_u8`, the fused loader of `mhmr_forward_u8`) use to reproduce it bit for bit, the
 device letterbox of photos of any size (`ImageOps.contain` + `ImageOps.pad`, demo.py:27-51), and the device decode of
-JPEG files (`Image.open(f).convert("RGB")`, byte for byte, for the baseline files it takes)."""
+JPEG and PNG files (`Image.open(f).convert("RGB")`, byte for byte, for the files it takes)."""
 from __future__ import annotations
 
 import numpy as np
@@ -80,6 +80,35 @@ def decode_jpeg(blobs, device):
         host, dev, spans = upload_bytes([blobs[i] for i in idx], device)
         outs = [torch.empty((infos[i][1], infos[i][0], 3), dtype=torch.uint8, device=device) for i in idx]
         status = ops.jpeg_decode(host, dev, spans, outs).cpu().tolist()
+    for i, o, s in zip(idx, outs, status):
+        if s == 0:
+            photos[i], ok[i] = o, True
+    return photos, ok
+
+
+def decode_png(blobs, device):
+    """PNG files' bytes -> (uint8 [H, W, 3] RGB device photos, ok flags), byte for byte `Image.open(f).convert("RGB")`
+    (csrc/png.cu; the arithmetic is restated in oracle/png_ref.py).  The contract of `decode_jpeg`: eligible files
+    (`ops.png_info`) are decoded in one call; a photo is None and its flag False when the file is not eligible, has
+    more pixels than Pillow's `Image.MAX_IMAGE_PIXELS`, or was flagged on the device (the caller decodes those with
+    Pillow).  Each file's zlib stream (its IDAT payloads) goes up in one pinned upload; the statuses come back in one
+    host sync."""
+    import torch
+    from PIL import Image
+
+    from . import ops
+
+    device = torch.device(device)
+    limit = Image.MAX_IMAGE_PIXELS
+    infos = [ops.png_info(b) for b in blobs]
+    idx = [i for i, info in enumerate(infos) if info[3] and (limit is None or info[0] * info[1] <= limit)]
+    photos, ok = [None] * len(blobs), [False] * len(blobs)
+    if not idx:
+        return photos, ok
+    with torch.cuda.device(device):
+        host, dev, spans = upload_bytes([ops.png_idat(blobs[i]) for i in idx], device)
+        outs = [torch.empty((infos[i][1], infos[i][0], 3), dtype=torch.uint8, device=device) for i in idx]
+        status = ops.png_decode([blobs[i] for i in idx], host, dev, spans, outs).cpu().tolist()
     for i, o, s in zip(idx, outs, status):
         if s == 0:
             photos[i], ok[i] = o, True
