@@ -60,7 +60,7 @@ int mhmr_op_gemm_f16(const void* A, int64_t lda, const void* W, int64_t ldw, int
  * second GEMM runs on the hi plane with the row-centred W * diag(ln_g) and applies 1/sigma in its epilogue.  A, Wp fp16
  * (K contiguous); X fp32 [M, D] in place (split on entry, merged on exit); W fp32 [N, D] (folded and rounded inside);
  * D multiple of 128 (<= 1024), N multiple of 32.
- * Unit-test entry: allocates its temporaries and synchronises the stream. */
+ * Unit-test entry: its temporaries are stream-ordered on `stream`; nothing waits for the device. */
 int mhmr_op_resid_ln_linear_f16(const void* A, int64_t lda, const void* Wp, int64_t ldwp, const float* bp,
                                 const float* ls, float* X, int M, int D, int Ka, const float* ln_g,
                                 const float* ln_b, const float* W, const float* b, int N, int gelu, void* out16,
@@ -196,7 +196,8 @@ int mhmr_op_detect(const float* scores, int B, int res, int nms_k, float thresh,
 /* SMPL-X per-person outputs (utils/humans.py:12-22, model.py:189-203, :272-275, :291, blocks/smpl_layer.py:123):
  * dec [P, ld_dec] = pose6 (318) | betas (num_betas) | cam (3) | expression (10); K [B, 3, 3] (inverted inside);
  * focal_norm = img_size / (2 tan 30 deg).  Writes rotmat [P, 53, 3, 3], rotvec [P, 53, 3], shape, expr, dist_pp,
- * dist, loc [P, 2], transl [P, 3], K_det [P, 3, 3].  Allocates a temporary and synchronises the stream. */
+ * dist, loc [P, 2], transl [P, 3], K_det [P, 3, 3].  Its temporary is stream-ordered on `stream`; nothing waits for
+ * the device. */
 int mhmr_op_person_post(const float* dec, int ld_dec, int num_betas, const float* offset, const float* K, int B,
                         const int* det_b, const int* det_y, const int* det_x, const int* count, int max_persons,
                         float focal_norm, float* rotmat, float* rotvec, float* shape, float* expr, float* dist_pp,
@@ -206,7 +207,7 @@ int mhmr_op_person_post(const float* dec, int ld_dec, int num_betas, const float
  * mlp_fov_unique) fov [B], K_regressed and K_use [B, 3, 3] (K if given, else K_regressed); then per person the 6D
  * rows rot6d [P, ld6] (J joints) -> rotmat [P, J, 3, 3] blended with the identity by useful [J], rotmat_homo
  * [P, J, 4, 4], rotvec, dist = K_use[0,0] / max(exp(dist_pp), 1e-5), loc, transl, K_det, and shape [P, num_betas]
- * replaced by its sigmoid in place.  Allocates a temporary and synchronises the stream. */
+ * replaced by its sigmoid in place.  Its temporary is stream-ordered on `stream`; nothing waits for the device. */
 int mhmr_op_anny_person_post(const float* hid, int D, const float* w2, const float* b2, const float* fov_max,
                              const float* K, int B, int img_size, float* fov, float* K_regressed, float* K_use,
                              const float* rot6d, int ld6, int J, const float* useful, float* shape, int num_betas,
@@ -218,7 +219,8 @@ int mhmr_op_anny_person_post(const float* hid, int D, const float* w2, const flo
  * blocks: x += ls1 * (Wproj . O16[l][rowidx[p]] + bproj);  x += ls2 * (Wfc2 . gelu(Wfc1 . LN2(x) + bfc1) + bfc2)
  * (LayerNorm eps 1e-6).  Weights stacked per layer: Wproj [depth, D, D], Wfc1 [depth, 4D, D], Wfc2 [depth, D, 4D],
  * vectors [depth, D] (bfc1 [depth, 4D]); O16 fp16 [depth, rows_o16, D].  D % 4 == 0.  Bit-reproducible.
- * Allocates its temporaries and synchronises the stream. */
+ * Its temporaries are stream-ordered on `stream`; the layer table goes up in one cudaMemcpyAsync from pageable
+ * memory; nothing else waits for the device. */
 int mhmr_op_refine_chain(int depth, int D, const int* count, int max_persons, const float* Wproj, const float* bproj,
                          const float* ls1, const float* ln2_g, const float* ln2_b, const float* Wfc1, const float* bfc1,
                          const float* Wfc2, const float* bfc2, const float* ls2, const void* O16, int64_t rows_o16,

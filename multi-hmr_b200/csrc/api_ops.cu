@@ -3,8 +3,6 @@
 #include "gemm_tc.cuh"
 #include "kernels.cuh"
 
-#include <vector>
-
 using namespace mhmr;
 
 namespace {
@@ -45,45 +43,31 @@ int mhmr_op_resid_ln_linear_f16(const void* A, int64_t lda, const void* Wp, int6
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int bn_d = (D % 256 == 0) ? 512 : 128, bn_n = (N % 256 == 0) ? 512 : 128;
   const int slots = gemm_stat_slots(D, bn_d);
-  __half *x16 = nullptr, *xlo = nullptr, *W16 = nullptr;
-  float2* stats = nullptr;
-  float* bias2 = nullptr;
-  auto release = [&]() {
-    cudaStreamSynchronize(st);
-    cudaFree(x16); cudaFree(xlo); cudaFree(W16); cudaFree(stats); cudaFree(bias2);
-  };
-  int rc = MHMR_OK;
-  auto run = [&]() -> int {
-    MHMR_CUDA_CHECK(cudaMalloc(&x16, static_cast<size_t>(M) * D * 2));
-    MHMR_CUDA_CHECK(cudaMalloc(&xlo, static_cast<size_t>(M) * D * 2));
-    MHMR_CUDA_CHECK(cudaMalloc(&W16, static_cast<size_t>(N) * D * 2));
-    MHMR_CUDA_CHECK(cudaMalloc(&stats, static_cast<size_t>(M) * slots * sizeof(float2)));
-    MHMR_CUDA_CHECK(cudaMalloc(&bias2, static_cast<size_t>(N) * 4));
-    int r = fold_ln_linear(W, b, ln_g, ln_b, W16, bias2, N, D, st);
-    if (r != MHMR_OK) return r;
-    r = split_rowstats(X, x16, xlo, D, stats, slots, M, D, st);  // the stream enters as (hi, lo)
-    if (r != MHMR_OK) return r;
-    GemmEpi p;
-    p.bias = bp; p.gamma = ls;
-    p.x16 = x16; p.xlo = xlo; p.ldx16 = D; p.stats = stats; p.stat_slots = slots;
-    GemmPlan pp;
-    r = gemm_plan_init(&pp, static_cast<const __half*>(A), lda, static_cast<const __half*>(Wp), ldwp, M, D, Ka,
-                       EPI_LS_RESID_SPLIT, p, bn_d);
-    if (r != MHMR_OK) return r;
-    r = gemm_plan_run(&pp, st);
-    if (r != MHMR_OK) return r;
-    GemmEpi c;
-    c.bias = bias2; c.stats = stats; c.stat_slots = slots; c.out = out16; c.ldo = ldo;
-    GemmPlan cp;
-    r = gemm_plan_init(&cp, x16, D, W16, D, M, N, D, gelu ? EPI_LN_GELU_F16 : EPI_LN_BIAS_F16, c, bn_n);
-    if (r != MHMR_OK) return r;
-    r = gemm_plan_run(&cp, st);
-    if (r != MHMR_OK) return r;
-    return merge_split(x16, xlo, X, static_cast<int64_t>(M) * D, st);
-  };
-  rc = run();
-  release();
-  return rc;
+  CallScratch ws(st);
+  const size_t r_x16 = ws.region(static_cast<size_t>(M) * D * 2), r_xlo = ws.region(static_cast<size_t>(M) * D * 2),
+               r_W16 = ws.region(static_cast<size_t>(N) * D * 2),
+               r_stats = ws.region(static_cast<size_t>(M) * slots * sizeof(float2)),
+               r_bias2 = ws.region(static_cast<size_t>(N) * 4);
+  TRY(ws.allocate());
+  __half *x16 = ws.dev<__half>(r_x16), *xlo = ws.dev<__half>(r_xlo), *W16 = ws.dev<__half>(r_W16);
+  float2* stats = ws.dev<float2>(r_stats);
+  float* bias2 = ws.dev<float>(r_bias2);
+  TRY(fold_ln_linear(W, b, ln_g, ln_b, W16, bias2, N, D, st));
+  TRY(split_rowstats(X, x16, xlo, D, stats, slots, M, D, st));  // the stream enters as (hi, lo)
+  GemmEpi p;
+  p.bias = bp; p.gamma = ls;
+  p.x16 = x16; p.xlo = xlo; p.ldx16 = D; p.stats = stats; p.stat_slots = slots;
+  GemmPlan pp;
+  TRY(gemm_plan_init(&pp, static_cast<const __half*>(A), lda, static_cast<const __half*>(Wp), ldwp, M, D, Ka,
+                     EPI_LS_RESID_SPLIT, p, bn_d));
+  TRY(gemm_plan_run(&pp, st));
+  GemmEpi c;
+  c.bias = bias2; c.stats = stats; c.stat_slots = slots; c.out = out16; c.ldo = ldo;
+  GemmPlan cp;
+  TRY(gemm_plan_init(&cp, x16, D, W16, D, M, N, D, gelu ? EPI_LN_GELU_F16 : EPI_LN_BIAS_F16, c, bn_n));
+  TRY(gemm_plan_run(&cp, st));
+  TRY(merge_split(x16, xlo, X, static_cast<int64_t>(M) * D, st));
+  return ws.release();
 }
 
 int mhmr_op_attention(const void* qkv, int64_t ld_qkv, void* out, int64_t ldo, int B, int T, int D,
@@ -156,18 +140,14 @@ int mhmr_op_person_post(const float* dec, int ld_dec, int num_betas, const float
                "person_post: bad sizes (num_betas in [1, 32], decoder row = 318 + num_betas + 3 + 10)");
   if (max_persons == 0) return MHMR_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  float* Kinv = nullptr;
-  auto run = [&]() -> int {
-    MHMR_CUDA_CHECK(cudaMalloc(&Kinv, static_cast<size_t>(B) * 9 * sizeof(float)));
-    int r = invert_K(K, Kinv, B, st);
-    if (r != MHMR_OK) return r;
-    return person_post(dec, ld_dec, num_betas, offset, K, Kinv, det_b, det_y, det_x, count, max_persons, focal_norm,
-                       rotmat, rotvec, shape, expr, dist_pp, dist, loc, transl, K_det, st);
-  };
-  const int rc = run();
-  cudaStreamSynchronize(st);
-  cudaFree(Kinv);
-  return rc;
+  CallScratch ws(st);
+  const size_t r_Kinv = ws.region(static_cast<size_t>(B) * 9 * sizeof(float));
+  TRY(ws.allocate());
+  float* Kinv = ws.dev<float>(r_Kinv);
+  TRY(invert_K(K, Kinv, B, st));
+  TRY(person_post(dec, ld_dec, num_betas, offset, K, Kinv, det_b, det_y, det_x, count, max_persons, focal_norm, rotmat,
+                  rotvec, shape, expr, dist_pp, dist, loc, transl, K_det, st));
+  return ws.release();
 }
 
 int mhmr_op_anny_person_post(const float* hid, int D, const float* w2, const float* b2, const float* fov_max,
@@ -182,18 +162,15 @@ int mhmr_op_anny_person_post(const float* hid, int D, const float* w2, const flo
   MHMR_REQUIRE(B >= 1 && D >= 1 && img_size >= 1 && J >= 1 && ld6 >= 6 * J && num_betas >= 0 && max_persons >= 0,
                "anny_person_post: bad sizes");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  float* Kinv = nullptr;
-  auto run = [&]() -> int {
-    MHMR_CUDA_CHECK(cudaMalloc(&Kinv, static_cast<size_t>(B) * 9 * sizeof(float)));
-    int r = anny_camera(hid, D, w2, b2, fov_max, K, B, img_size, fov, K_regressed, K_use, Kinv, st);
-    if (r != MHMR_OK || max_persons == 0) return r;
-    return anny_person_post(rot6d, ld6, J, useful, shape, num_betas, offset, dist_pp, K_use, Kinv, det_b, det_y, det_x,
-                            count, max_persons, rotmat, rotmat_homo, rotvec, dist, loc, transl, K_det, st);
-  };
-  const int rc = run();
-  cudaStreamSynchronize(st);
-  cudaFree(Kinv);
-  return rc;
+  CallScratch ws(st);
+  const size_t r_Kinv = ws.region(static_cast<size_t>(B) * 9 * sizeof(float));
+  TRY(ws.allocate());
+  float* Kinv = ws.dev<float>(r_Kinv);
+  TRY(anny_camera(hid, D, w2, b2, fov_max, K, B, img_size, fov, K_regressed, K_use, Kinv, st));
+  if (max_persons > 0)
+    TRY(anny_person_post(rot6d, ld6, J, useful, shape, num_betas, offset, dist_pp, K_use, Kinv, det_b, det_y, det_x,
+                         count, max_persons, rotmat, rotmat_homo, rotvec, dist, loc, transl, K_det, st));
+  return ws.release();
 }
 
 int mhmr_op_refine_chain(int depth, int D, const int* count, int max_persons, const float* Wproj, const float* bproj,
@@ -210,28 +187,23 @@ int mhmr_op_refine_chain(int depth, int D, const int* count, int max_persons, co
   if (max_persons == 0) return MHMR_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t DD = static_cast<int64_t>(D) * D;
-  std::vector<RefineLayer> rl(depth);
+  CallScratch ws(st);
+  const size_t r_layers = ws.region(depth * sizeof(RefineLayer), true),
+               r_term = ws.region(static_cast<size_t>(depth) * max_persons * D * sizeof(float)),
+               r_h = ws.region(static_cast<size_t>(max_persons) * 4 * D * sizeof(float)),
+               r_barrier = ws.region(sizeof(unsigned int));
+  RefineLayer* rl = ws.host<RefineLayer>(r_layers);
   for (int l = 0; l < depth; ++l)
     rl[l] = RefineLayer{static_cast<const __half*>(O16) + l * rows_o16 * D, Wproj + l * DD, bproj + l * D, ls1 + l * D,
                         ln2_g + l * D, ln2_b + l * D, Wfc1 + l * 4 * DD, bfc1 + l * 4 * D, Wfc2 + l * 4 * DD,
                         bfc2 + l * D, ls2 + l * D};
-  RefineLayer* layers = nullptr;
-  float *term = nullptr, *h = nullptr;
-  unsigned int* barrier = nullptr;
-  auto run = [&]() -> int {
-    MHMR_CUDA_CHECK(cudaMalloc(&layers, rl.size() * sizeof(RefineLayer)));
-    MHMR_CUDA_CHECK(cudaMalloc(&term, static_cast<size_t>(depth) * max_persons * D * sizeof(float)));
-    MHMR_CUDA_CHECK(cudaMalloc(&h, static_cast<size_t>(max_persons) * 4 * D * sizeof(float)));
-    MHMR_CUDA_CHECK(cudaMalloc(&barrier, sizeof(unsigned int)));
-    MHMR_CUDA_CHECK(cudaMemcpyAsync(layers, rl.data(), rl.size() * sizeof(RefineLayer), cudaMemcpyHostToDevice, st));
-    int r = refine_proj_terms(layers, depth, rowidx, count, D, max_persons, term, st);
-    if (r != MHMR_OK) return r;
-    return refine_mlp_chain(layers, depth, count, D, max_persons, term, x, h, barrier, st);
-  };
-  const int rc = run();
-  cudaStreamSynchronize(st);
-  cudaFree(layers); cudaFree(term); cudaFree(h); cudaFree(barrier);
-  return rc;
+  TRY(ws.allocate());
+  TRY(ws.upload());
+  const RefineLayer* layers = ws.dev<const RefineLayer>(r_layers);
+  float *term = ws.dev<float>(r_term), *h = ws.dev<float>(r_h);
+  TRY(refine_proj_terms(layers, depth, rowidx, count, D, max_persons, term, st));
+  TRY(refine_mlp_chain(layers, depth, count, D, max_persons, term, x, h, ws.dev<unsigned int>(r_barrier), st));
+  return ws.release();
 }
 
 // ---- backbone entry, folded LayerNorm and the gathers of the heads (vit_misc.cu, gemm_tc.cu, head.cu) --------------

@@ -93,27 +93,6 @@ int body_build(DeviceBody* b, int joints, int V, int nb, int ne, int center_idx,
 
 }  // namespace mhmr
 
-namespace {
-
-// Device copies of the caller's float arrays, which may be host or device memory: every folding kernel reads these,
-// never the caller's pointers.  Freed when loading is done.
-struct Staging {
-  std::vector<void*> bufs;
-  ~Staging() {
-    for (void* p : bufs) cudaFree(p);
-  }
-  int copy(const float* src, size_t n, const float** out, cudaStream_t st) {
-    void* p = nullptr;
-    MHMR_CUDA_CHECK(cudaMalloc(&p, n * sizeof(float)));
-    bufs.push_back(p);
-    MHMR_CUDA_CHECK(cudaMemcpyAsync(p, src, n * sizeof(float), cudaMemcpyDefault, st));
-    *out = static_cast<const float*>(p);
-    return MHMR_OK;
-  }
-};
-
-}  // namespace
-
 extern "C" {
 
 int mhmr_body_create(int kind, int num_verts, int num_betas, int max_persons, const float* v_template,
@@ -132,19 +111,26 @@ int mhmr_body_create(int kind, int num_verts, int num_betas, int max_persons, co
   const int V = num_verts, nb = num_betas, ne = x ? 10 : 0, NJ = x ? 55 : 24, PF = 9 * (NJ - 1);
   TRY(body_limits(NJ, nb + ne));  // before staging reads num_betas columns of shapedirs
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Staging stage;
-  const float *vt, *sd, *ed = nullptr, *pd, *jr, *lw, *bary = nullptr;
-  TRY(stage.copy(v_template, 3ll * V, &vt, st));
-  TRY(stage.copy(shapedirs, 3ll * V * nb, &sd, st));
-  if (x) TRY(stage.copy(expr_dirs, 3ll * V * ne, &ed, st));
-  TRY(stage.copy(posedirs, static_cast<size_t>(PF) * 3 * V, &pd, st));
-  TRY(stage.copy(J_regressor, static_cast<size_t>(NJ) * V, &jr, st));
-  TRY(stage.copy(lbs_weights, static_cast<size_t>(V) * NJ, &lw, st));
-  if (x) TRY(stage.copy(lmk_bary, 51 * 3, &bary, st));
+  // Device copies of the caller's float arrays, which may be host or device memory: every folding kernel reads these,
+  // never the caller's pointers.  Freed when loading is done.
+  const float* src[7] = {v_template, shapedirs, x ? expr_dirs : nullptr, posedirs, J_regressor, lbs_weights,
+                         x ? lmk_bary : nullptr};
+  const size_t n[7] = {3ull * V, 3ull * V * nb, 3ull * V * ne, static_cast<size_t>(PF) * 3 * V,
+                       static_cast<size_t>(NJ) * V, static_cast<size_t>(V) * NJ, x ? 51ull * 3 : 0ull};
+  CallScratch ws(st);
+  size_t r[7];
+  for (int i = 0; i < 7; ++i) r[i] = ws.region(n[i] * sizeof(float));
+  TRY(ws.allocate());
+  const float* d[7];
+  for (int i = 0; i < 7; ++i) {
+    d[i] = src[i] ? ws.dev<const float>(r[i]) : nullptr;
+    if (src[i]) MHMR_CUDA_CHECK(cudaMemcpyAsync(ws.dev<float>(r[i]), src[i], n[i] * sizeof(float), cudaMemcpyDefault, st));
+  }
   auto h = std::make_unique<mhmr_body>();
   h->kind = kind;
-  TRY(body_build(&h->body, NJ, V, nb, ne, 0, max_persons, vt, sd, ed, pd, jr, lw, parents, extra_joints_idxs, lmk_tri,
-                 bary, st));
+  TRY(body_build(&h->body, NJ, V, nb, ne, 0, max_persons, d[0], d[1], d[2], d[3], d[4], d[5], parents,
+                 extra_joints_idxs, lmk_tri, d[6], st));
+  TRY(ws.release());
   *out = h.release();
   return MHMR_OK;
 }

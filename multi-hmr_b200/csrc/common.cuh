@@ -11,6 +11,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
+#include <vector>
 
 #include "../../include/mhmr.h"
 
@@ -77,6 +78,47 @@ struct PerDeviceOnce {
 };
 // Programmatic dependent launch for the back-to-back kernels of the ViT loop (MHMR_PDL=0 disables).
 bool pdl_enabled();
+
+inline size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
+
+// Device memory of one C-ABI call: regions laid out on the host at 256-byte alignment, the staged ones before every
+// device-only one, in one stream-ordered allocation on the call's stream.  The staged regions' host bytes, filled by
+// the caller (after allocate() when they hold device addresses inside the scratch), go up in one cudaMemcpyAsync from
+// pageable memory, which returns once the driver has read them.  The scratch is freed stream-ordered on the same
+// stream on every return path: by release() on success, by the destructor on an error return.
+class CallScratch {
+ public:
+  explicit CallScratch(cudaStream_t st) : st_(st) {}
+  ~CallScratch();
+  CallScratch(const CallScratch&) = delete;
+  CallScratch& operator=(const CallScratch&) = delete;
+  // Handle of a new region of `bytes` (0 allowed); a staged region is uploaded by upload().
+  size_t region(size_t bytes, bool staged = false);
+  int allocate();  // the whole layout (at least 256 bytes)
+  // Device address of a region, valid after allocate().
+  template <class T>
+  T* dev(size_t r) const {
+    return reinterpret_cast<T*>(base_ + regions_[r].off + (regions_[r].staged ? 0 : staged_bytes_));
+  }
+  // Host bytes of a staged region (zero-filled); a later staged region() call may move them.
+  template <class T>
+  T* host(size_t r) {
+    return reinterpret_cast<T*>(blob_.data() + regions_[r].off);
+  }
+  int upload();
+  int release();  // frees now, returning the status of the free
+
+ private:
+  struct Region {
+    size_t off;
+    bool staged;
+  };
+  cudaStream_t st_;
+  uint8_t* base_ = nullptr;
+  std::vector<Region> regions_;
+  std::vector<uint8_t> blob_;  // the staged regions' host bytes
+  size_t staged_bytes_ = 0, device_bytes_ = 0;
+};
 
 #ifdef __CUDACC__
 // ----------------------------------------------------------------------------------

@@ -2,6 +2,7 @@
 #include <cstdlib>
 #include "common.cuh"
 
+#include <algorithm>
 #include <mutex>
 
 namespace mhmr {
@@ -112,6 +113,36 @@ int device_sm_count() {
       sms[dev] = 132;
   }
   return sms[dev];
+}
+
+CallScratch::~CallScratch() {
+  if (base_ != nullptr) cudaFreeAsync(base_, st_);
+}
+
+size_t CallScratch::region(size_t bytes, bool staged) {
+  size_t& end = staged ? staged_bytes_ : device_bytes_;
+  regions_.push_back({end, staged});
+  end += align256(bytes);
+  if (staged) blob_.resize(staged_bytes_);
+  return regions_.size() - 1;
+}
+
+int CallScratch::allocate() {
+  const size_t bytes = std::max<size_t>(staged_bytes_ + device_bytes_, 256);
+  MHMR_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&base_), bytes, st_));
+  return MHMR_OK;
+}
+
+int CallScratch::upload() {
+  if (staged_bytes_ > 0) MHMR_CUDA_CHECK(cudaMemcpyAsync(base_, blob_.data(), staged_bytes_, cudaMemcpyHostToDevice, st_));
+  return MHMR_OK;
+}
+
+int CallScratch::release() {
+  uint8_t* p = base_;
+  base_ = nullptr;
+  if (p != nullptr) MHMR_CUDA_CHECK(cudaFreeAsync(p, st_));
+  return MHMR_OK;
 }
 
 bool pdl_enabled() {

@@ -863,8 +863,6 @@ Layout layout(const Header& h) {
   return L;
 }
 
-size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
-
 // The shared body of both entries: coefficients only (coef_out != nullptr: the caller's buffer, photos' planes
 // back to back) or the whole decode into the photos' outputs.
 int run(const int64_t* photos, int B, int subseq_bits, int16_t* coef_out, int32_t* status, int32_t* passes,
@@ -939,121 +937,110 @@ int run(const int64_t* photos, int B, int subseq_bits, int16_t* coef_out, int32_
   const int NC = static_cast<int>(chunks.size()), NI = static_cast<int>(ivs.size()), NS = static_cast<int>(max_sub);
 
   // workspace: [photos | tables | chunks | intervals | planes] (uploaded) then device-only arrays
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
-  const size_t o_ph = take(sizeof(JPhoto) * B), o_tab = take(sizeof(JTables) * B), o_ch = take(sizeof(Chunk) * NC),
-               o_iv = take(sizeof(JIv) * NI), o_pl = take(sizeof(PlaneRef) * planes.size());
-  const size_t up_bytes = off;
-  const size_t o_kept = take(4ll * NC), o_marks = take(4ll * NC), o_nsub = take(4), o_subiv = take(4ll * NS),
-               o_start = take(8ll * NS), o_end = take(16ll * NS), o_cnt = take(4ll * NS), o_dcs = take(12ll * NS),
-               o_cntx = take(4ll * NS), o_dcx = take(12ll * NS), o_part = take(16ll * ((NS + 1023) / 1024)),
-               o_done = take(4ll * NI), o_flags = take(16),
-               o_dst = take(dst_bytes), o_coef = take(coef_out ? 0 : 2 * coef_elems),
-               o_plane = take(coef_out ? 0 : plane_bytes);
-  uint8_t* ws = nullptr;
-  MHMR_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&ws), off, st));
+  CallScratch ws(st);
+  const size_t r_ph = ws.region(sizeof(JPhoto) * B, true), r_tab = ws.region(sizeof(JTables) * B, true),
+               r_ch = ws.region(sizeof(Chunk) * NC, true), r_iv = ws.region(sizeof(JIv) * NI, true),
+               r_pl = ws.region(sizeof(PlaneRef) * planes.size(), true);
+  const size_t r_kept = ws.region(4ll * NC), r_marks = ws.region(4ll * NC), r_nsub = ws.region(4),
+               r_subiv = ws.region(4ll * NS), r_start = ws.region(8ll * NS), r_end = ws.region(16ll * NS),
+               r_cnt = ws.region(4ll * NS), r_dcs = ws.region(12ll * NS), r_cntx = ws.region(4ll * NS),
+               r_dcx = ws.region(12ll * NS), r_part = ws.region(16ll * ((NS + 1023) / 1024)), r_done = ws.region(4ll * NI),
+               r_flags = ws.region(16), r_dst = ws.region(dst_bytes), r_coef = ws.region(coef_out ? 0 : 2 * coef_elems),
+               r_plane = ws.region(coef_out ? 0 : plane_bytes);
+  TRY(ws.allocate());
   // device addresses of each photo's destuffed stream, coefficients and planes
   size_t dpos = 0;
   int64_t cpos = 0;
   for (int b = 0; b < B; ++b) {
     JPhoto& p = ph[b];
-    p.dst = ws + o_dst + dpos;
+    p.dst = ws.dev<uint8_t>(r_dst) + dpos;
     dpos += align256(p.ecs_len + kSlack);
     for (int c = 0; c < p.ncomp; ++c) {
       const int64_t n = static_cast<int64_t>(p.bw[c]) * p.bh[c] * 64;
-      p.coef[c] = (coef_out ? coef_out : reinterpret_cast<int16_t*>(ws + o_coef)) + cpos;
-      if (!coef_out) p.plane[c] = ws + o_plane + cpos;
+      p.coef[c] = (coef_out ? coef_out : ws.dev<int16_t>(r_coef)) + cpos;
+      if (!coef_out) p.plane[c] = ws.dev<uint8_t>(r_plane) + cpos;
       cpos += n;
     }
   }
-  std::vector<uint8_t> blob(up_bytes);
-  std::memcpy(blob.data() + o_ph, ph.data(), sizeof(JPhoto) * B);
-  for (int b = 0; b < B; ++b) std::memcpy(blob.data() + o_tab + sizeof(JTables) * b, &hdr[b].tab, sizeof(JTables));
-  std::memcpy(blob.data() + o_ch, chunks.data(), sizeof(Chunk) * NC);
-  std::memcpy(blob.data() + o_iv, ivs.data(), sizeof(JIv) * NI);
-  std::memcpy(blob.data() + o_pl, planes.data(), sizeof(PlaneRef) * planes.size());
+  std::memcpy(ws.host<JPhoto>(r_ph), ph.data(), sizeof(JPhoto) * B);
+  for (int b = 0; b < B; ++b) ws.host<JTables>(r_tab)[b] = hdr[b].tab;
+  std::memcpy(ws.host<Chunk>(r_ch), chunks.data(), sizeof(Chunk) * NC);
+  std::memcpy(ws.host<JIv>(r_iv), ivs.data(), sizeof(JIv) * NI);
+  std::memcpy(ws.host<PlaneRef>(r_pl), planes.data(), sizeof(PlaneRef) * planes.size());
 
   Ctx ctx{};
-  ctx.ph = reinterpret_cast<const JPhoto*>(ws + o_ph);
-  ctx.tab = reinterpret_cast<const JTables*>(ws + o_tab);
-  ctx.iv = reinterpret_cast<JIv*>(ws + o_iv);
+  ctx.ph = ws.dev<const JPhoto>(r_ph);
+  ctx.tab = ws.dev<const JTables>(r_tab);
+  ctx.iv = ws.dev<JIv>(r_iv);
   ctx.niv = NI;
   ctx.subseq_bits = subseq_bits;
   ctx.max_sub = NS;
-  ctx.nsub = reinterpret_cast<int*>(ws + o_nsub);
-  ctx.sub_iv = reinterpret_cast<int*>(ws + o_subiv);
-  ctx.start = reinterpret_cast<int2*>(ws + o_start);
-  ctx.endst = reinterpret_cast<int2*>(ws + o_end);
-  ctx.cnt = reinterpret_cast<int*>(ws + o_cnt);
-  ctx.dcs = reinterpret_cast<uint32_t*>(ws + o_dcs);
-  ctx.cntx = reinterpret_cast<int*>(ws + o_cntx);
-  ctx.dcx = reinterpret_cast<uint32_t*>(ws + o_dcx);
-  ctx.part = reinterpret_cast<uint32_t*>(ws + o_part);
+  ctx.nsub = ws.dev<int>(r_nsub);
+  ctx.sub_iv = ws.dev<int>(r_subiv);
+  ctx.start = ws.dev<int2>(r_start);
+  ctx.endst = ws.dev<int2>(r_end);
+  ctx.cnt = ws.dev<int>(r_cnt);
+  ctx.dcs = ws.dev<uint32_t>(r_dcs);
+  ctx.cntx = ws.dev<int>(r_cntx);
+  ctx.dcx = ws.dev<uint32_t>(r_dcx);
+  ctx.part = ws.dev<uint32_t>(r_part);
   ctx.nparts = (NS + 1023) / 1024;
-  ctx.done = reinterpret_cast<int*>(ws + o_done);
-  ctx.flags = reinterpret_cast<int*>(ws + o_flags);
+  ctx.done = ws.dev<int>(r_done);
+  ctx.flags = ws.dev<int>(r_flags);
   ctx.passes = passes;
   ctx.status = status;
-  int* kept = reinterpret_cast<int*>(ws + o_kept);
-  int* marks = reinterpret_cast<int*>(ws + o_marks);
+  const Chunk* dch = ws.dev<const Chunk>(r_ch);
+  int* kept = ws.dev<int>(r_kept);
+  int* marks = ws.dev<int>(r_marks);
 
   static PerDeviceOnce once;
   static int coop_blocks[64];
   int dev = 0;
-  auto run_all = [&]() -> int {
-    MHMR_CUDA_CHECK(cudaGetDevice(&dev));
-    if (once.first()) {
-      MHMR_CUDA_CHECK(cudaMemcpyToSymbol(c_zigzag, kZigzag, 64));
-      int per_sm = 0;
-      MHMR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, huff_sync_kernel, 256, 0));
-      coop_blocks[dev] = std::max(1, per_sm) * device_sm_count();
-    }
-    MHMR_CUDA_CHECK(cudaMemcpyAsync(ws, blob.data(), up_bytes, cudaMemcpyHostToDevice, st));
-    MHMR_CUDA_CHECK(cudaMemsetAsync(status, 0, 4ll * B, st));
-    MHMR_CUDA_CHECK(cudaMemsetAsync(ws + o_done, 0, o_dst - o_done, st));   // done, flags
-    MHMR_CUDA_CHECK(cudaMemsetAsync(ws + o_dst, 0, dst_bytes, st));          // the zero slack after each stream
-    MHMR_CUDA_CHECK(cudaMemsetAsync(coef_out ? static_cast<void*>(coef_out) : static_cast<void*>(ws + o_coef), 0,
-                                    2 * coef_elems, st));
-    seg_count_kernel<<<NC, 256, 0, st>>>(ctx.ph, reinterpret_cast<const Chunk*>(ws + o_ch), kept, marks);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    seg_scan_kernel<<<B, 1024, 0, st>>>(ctx.ph, ctx.iv, kept, marks, status);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    seg_write_kernel<<<NC, 256, 0, st>>>(ctx.ph, reinterpret_cast<const Chunk*>(ws + o_ch), kept, marks, ctx.iv,
-                                         status);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    plan_kernel<<<1, 1024, 0, st>>>(ctx);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    sub_map_kernel<<<(NS + 255) / 256, 256, 0, st>>>(ctx);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    const int grid = static_cast<int>(std::min<int64_t>(coop_blocks[dev], (NS + 255) / 256));
-    void* args[] = {&ctx};
-    MHMR_CUDA_CHECK(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(huff_sync_kernel), dim3(grid), dim3(256), args,
-                                                0, st));
-    sub_tile_sum_kernel<<<ctx.nparts, 1024, 0, st>>>(ctx);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    sub_tile_scan_kernel<<<1, 1024, 0, st>>>(ctx);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    sub_scan_kernel<<<ctx.nparts, 1024, 0, st>>>(ctx);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    huff_write_kernel<<<(NS + 255) / 256, 256, 0, st>>>(ctx);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    check_done_kernel<<<(NI + 255) / 256, 256, 0, st>>>(ctx);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    if (coef_out) return MHMR_OK;
+  MHMR_CUDA_CHECK(cudaGetDevice(&dev));
+  if (once.first()) {
+    MHMR_CUDA_CHECK(cudaMemcpyToSymbol(c_zigzag, kZigzag, 64));
+    int per_sm = 0;
+    MHMR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, huff_sync_kernel, 256, 0));
+    coop_blocks[dev] = std::max(1, per_sm) * device_sm_count();
+  }
+  TRY(ws.upload());
+  MHMR_CUDA_CHECK(cudaMemsetAsync(status, 0, 4ll * B, st));
+  MHMR_CUDA_CHECK(cudaMemsetAsync(ctx.done, 0, ws.dev<uint8_t>(r_dst) - ws.dev<uint8_t>(r_done), st));   // done, flags
+  MHMR_CUDA_CHECK(cudaMemsetAsync(ws.dev<uint8_t>(r_dst), 0, dst_bytes, st));   // the zero slack after each stream
+  MHMR_CUDA_CHECK(cudaMemsetAsync(coef_out ? coef_out : ws.dev<int16_t>(r_coef), 0, 2 * coef_elems, st));
+  seg_count_kernel<<<NC, 256, 0, st>>>(ctx.ph, dch, kept, marks);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  seg_scan_kernel<<<B, 1024, 0, st>>>(ctx.ph, ctx.iv, kept, marks, status);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  seg_write_kernel<<<NC, 256, 0, st>>>(ctx.ph, dch, kept, marks, ctx.iv, status);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  plan_kernel<<<1, 1024, 0, st>>>(ctx);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  sub_map_kernel<<<(NS + 255) / 256, 256, 0, st>>>(ctx);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  const int grid = static_cast<int>(std::min<int64_t>(coop_blocks[dev], (NS + 255) / 256));
+  void* args[] = {&ctx};
+  MHMR_CUDA_CHECK(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(huff_sync_kernel), dim3(grid), dim3(256), args,
+                                              0, st));
+  sub_tile_sum_kernel<<<ctx.nparts, 1024, 0, st>>>(ctx);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  sub_tile_scan_kernel<<<1, 1024, 0, st>>>(ctx);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  sub_scan_kernel<<<ctx.nparts, 1024, 0, st>>>(ctx);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  huff_write_kernel<<<(NS + 255) / 256, 256, 0, st>>>(ctx);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  check_done_kernel<<<(NI + 255) / 256, 256, 0, st>>>(ctx);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  if (!coef_out) {
     idct_kernel<<<static_cast<int>((nblocks + 31) / 32), 256, 0, st>>>(
-        ctx.ph, ctx.tab, reinterpret_cast<const PlaneRef*>(ws + o_pl), static_cast<int>(planes.size()),
-        static_cast<int>(nblocks), status);
+        ctx.ph, ctx.tab, ws.dev<const PlaneRef>(r_pl), static_cast<int>(planes.size()), static_cast<int>(nblocks), status);
     MHMR_CUDA_CHECK(cudaGetLastError());
     const dim3 cgrid((maxW + 255) / 256, std::min(maxH, 1024), B);
     color_kernel<<<cgrid, 256, 0, st>>>(ctx.ph);
     MHMR_CUDA_CHECK(cudaGetLastError());
-    return MHMR_OK;
-  };
-  const int rc = run_all();
-  const cudaError_t fe = cudaFreeAsync(ws, st);
-  if (rc != MHMR_OK) return rc;
-  MHMR_CUDA_CHECK(fe);
-  return MHMR_OK;
+  }
+  return ws.release();
 }
 
 }  // namespace

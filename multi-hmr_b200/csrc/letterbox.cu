@@ -151,8 +151,6 @@ struct Tables {
   const int32_t* row(int offset, int taps, int i) const { return data.data() + offset + static_cast<int64_t>(i) * (taps + 2); }
 };
 
-size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
-
 }  // namespace
 
 extern "C" {
@@ -165,8 +163,6 @@ int mhmr_op_letterbox_u8(const int64_t* photos, int B, int S, int pad, uint8_t* 
   std::vector<LbImage> imgs(B);
   std::vector<int> box(4 * B);
   Tables tab;
-  size_t ws_bytes = 0;
-  std::vector<size_t> ws_off(B);
   for (int b = 0; b < B; ++b) {
     const int64_t* d = photos + 4 * b;
     const int64_t H = d[1], W = d[2], pitch = d[3];
@@ -214,47 +210,40 @@ int mhmr_op_letterbox_u8(const int64_t* photos, int B, int S, int pad, uint8_t* 
       im.ws_cols = 0;
       im.last = vert;
     }
-    ws_off[b] = ws_bytes;
-    ws_bytes += align256(static_cast<size_t>(im.ws_rows) * 3 * im.ws_cols);
     box[4 * b] = im.x0; box[4 * b + 1] = im.y0; box[4 * b + 2] = nw; box[4 * b + 3] = nh;
   }
   MHMR_REQUIRE(tab.data.size() < (1ull << 31), "letterbox: coefficient tables too large");
 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t desc_bytes = align256(sizeof(LbImage) * B), tab_bytes = align256(4 * tab.data.size());
-  uint8_t* dev = nullptr;
-  MHMR_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&dev), desc_bytes + tab_bytes + ws_bytes, st));
+  CallScratch ws(st);
+  const size_t r_imgs = ws.region(sizeof(LbImage) * B, true), r_tab = ws.region(4 * tab.data.size(), true);
+  std::vector<size_t> r_ws(B);
+  for (int b = 0; b < B; ++b) r_ws[b] = ws.region(static_cast<size_t>(imgs[b].ws_rows) * 3 * imgs[b].ws_cols);
+  TRY(ws.allocate());
   int max_cols = 0, max_rows = 0;
   for (int b = 0; b < B; ++b) {
     LbImage& im = imgs[b];
     if (im.ws_rows > 0) {
-      im.ws = dev + desc_bytes + tab_bytes + ws_off[b];
+      im.ws = ws.dev<uint8_t>(r_ws[b]);
       im.last.src = im.ws;
       max_cols = std::max(max_cols, im.ws_cols);
       max_rows = std::max(max_rows, im.ws_rows);
     }
   }
-  std::vector<uint8_t> blob(desc_bytes + tab_bytes);
-  std::copy_n(reinterpret_cast<const uint8_t*>(imgs.data()), sizeof(LbImage) * B, blob.data());
-  std::copy_n(reinterpret_cast<const uint8_t*>(tab.data.data()), 4 * tab.data.size(), blob.data() + desc_bytes);
-  const LbImage* d_imgs = reinterpret_cast<const LbImage*>(dev);
-  const int32_t* d_tab = reinterpret_cast<const int32_t*>(dev + desc_bytes);
-  auto run = [&]() -> int {
-    MHMR_CUDA_CHECK(cudaMemcpyAsync(dev, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
-    if (max_rows > 0) {
-      const dim3 grid((3 * max_cols + kThreads - 1) / kThreads, std::min(max_rows, 65535), B);
-      letterbox_first_pass_kernel<<<grid, kThreads, 0, st>>>(d_imgs, d_tab);
-      MHMR_CUDA_CHECK(cudaGetLastError());
-    }
-    const dim3 grid((3 * S + kThreads - 1) / kThreads, std::min(S, 65535), B);
-    letterbox_last_pass_kernel<<<grid, kThreads, 0, st>>>(d_imgs, d_tab, out, S, pad);
+  std::copy_n(imgs.data(), B, ws.host<LbImage>(r_imgs));
+  std::copy_n(tab.data.data(), tab.data.size(), ws.host<int32_t>(r_tab));
+  const LbImage* d_imgs = ws.dev<const LbImage>(r_imgs);
+  const int32_t* d_tab = ws.dev<const int32_t>(r_tab);
+  TRY(ws.upload());
+  if (max_rows > 0) {
+    const dim3 grid((3 * max_cols + kThreads - 1) / kThreads, std::min(max_rows, 65535), B);
+    letterbox_first_pass_kernel<<<grid, kThreads, 0, st>>>(d_imgs, d_tab);
     MHMR_CUDA_CHECK(cudaGetLastError());
-    return MHMR_OK;
-  };
-  const int rc = run();
-  const cudaError_t fe = cudaFreeAsync(dev, st);
-  if (rc != MHMR_OK) return rc;
-  MHMR_CUDA_CHECK(fe);
+  }
+  const dim3 grid((3 * S + kThreads - 1) / kThreads, std::min(S, 65535), B);
+  letterbox_last_pass_kernel<<<grid, kThreads, 0, st>>>(d_imgs, d_tab, out, S, pad);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  TRY(ws.release());
   if (boxes != nullptr) std::copy(box.begin(), box.end(), boxes);
   return MHMR_OK;
 }

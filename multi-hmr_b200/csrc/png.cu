@@ -38,7 +38,7 @@
 // only [0, expected length).  The unfilter reads and writes only the inflated buffer (rows of the expected length,
 // filter byte included) and writes the output at rows < H, columns < 3 W, of the caller's pitch.  Candidate and chain
 // lists are capped; a capped search only loses speed, a capped chain flags the photo.  The workspace is
-// stream-ordered (cudaMallocAsync / cudaFreeAsync).
+// stream-ordered (CallScratch).
 #include "common.cuh"
 
 #include <algorithm>
@@ -808,8 +808,6 @@ bool parse(const uint8_t* d, int64_t n, Header* h) {
 
 int channels(int ctype) { return ctype == 0 ? 1 : ctype == 2 ? 3 : ctype == 3 ? 1 : ctype == 4 ? 2 : 4; }
 
-size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
-
 struct Stream {
   const uint8_t* src;   // device
   int64_t nbytes, expect;
@@ -824,13 +822,12 @@ struct Stream {
 int run(const std::vector<Stream>& ss, int32_t* status, int32_t* counts, void* stream) {
   const int B = static_cast<int>(ss.size());
   std::vector<PPhoto> ph(B);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
-  const size_t o_ph = take(sizeof(PPhoto) * B);
-  const size_t up_bytes = off;
-  const size_t o_st = take(sizeof(PState) * B), o_cs = take(4ll * (B + 1));
-  std::vector<size_t> o_words(B), o_bm(B), o_cand(B), o_chain(B), o_sym(B), o_inf(B);
-  std::vector<int> cand_start(B + 1, 0);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallScratch ws(st);
+  const size_t r_ph = ws.region(sizeof(PPhoto) * B, true), r_cs = ws.region(4ll * (B + 1), true);
+  const size_t r_st = ws.region(sizeof(PState) * B);
+  std::vector<size_t> r_words(B), r_bm(B), r_cand(B), r_chain(B), r_sym(B), r_inf(B);
+  int* cand_start = ws.host<int>(r_cs);
   int64_t words = 0, ncand = 0;
   for (int b = 0; b < B; ++b) {
     const Stream& s = ss[b];
@@ -852,77 +849,66 @@ int run(const std::vector<Stream>& ss, int32_t* status, int32_t* counts, void* s
     words += nw;
     cand_start[b] = static_cast<int>(ncand);
     ncand += P.ncand_cap;
-    o_words[b] = take(s.nbytes + kSlack);
-    o_bm[b] = take(4 * nw);
-    o_cand[b] = take(8ll * P.ncand_cap);
-    o_chain[b] = take(16ll * P.nchain_cap);
-    o_sym[b] = take(4 * s.expect);
-    o_inf[b] = s.out_inf ? 0 : take(s.expect);
+    r_words[b] = ws.region(s.nbytes + kSlack);
+    r_bm[b] = ws.region(4 * nw);
+    r_cand[b] = ws.region(8ll * P.ncand_cap);
+    r_chain[b] = ws.region(16ll * P.nchain_cap);
+    r_sym[b] = ws.region(4 * s.expect);
+    r_inf[b] = s.out_inf ? 0 : ws.region(s.expect);
   }
   cand_start[B] = static_cast<int>(ncand);
   MHMR_REQUIRE(ncand < (1ll << 31) && words * 32 < (1ll << 62), "png: batch too large for one call");
-  const size_t o_meas = take(sizeof(Meas) * ncand);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  uint8_t* ws = nullptr;
-  MHMR_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&ws), off, st));
+  const size_t r_meas = ws.region(sizeof(Meas) * ncand);
+  TRY(ws.allocate());
   for (int b = 0; b < B; ++b) {
     PPhoto& P = ph[b];
-    P.words = reinterpret_cast<const uint32_t*>(ws + o_words[b]);
-    P.bitmap = reinterpret_cast<uint32_t*>(ws + o_bm[b]);
-    P.cand = reinterpret_cast<int64_t*>(ws + o_cand[b]);
-    P.chain = reinterpret_cast<int64_t*>(ws + o_chain[b]);
-    P.sym = reinterpret_cast<uint32_t*>(ws + o_sym[b]);
-    P.inf = ss[b].out_inf ? ss[b].out_inf : ws + o_inf[b];
+    P.words = ws.dev<const uint32_t>(r_words[b]);
+    P.bitmap = ws.dev<uint32_t>(r_bm[b]);
+    P.cand = ws.dev<int64_t>(r_cand[b]);
+    P.chain = ws.dev<int64_t>(r_chain[b]);
+    P.sym = ws.dev<uint32_t>(r_sym[b]);
+    P.inf = ss[b].out_inf ? ss[b].out_inf : ws.dev<uint8_t>(r_inf[b]);
   }
-  std::vector<uint8_t> blob(up_bytes);
-  std::memcpy(blob.data() + o_ph, ph.data(), sizeof(PPhoto) * B);
-  const PPhoto* dph = reinterpret_cast<const PPhoto*>(ws + o_ph);
-  PState* dst = reinterpret_cast<PState*>(ws + o_st);
-  int* dcs = reinterpret_cast<int*>(ws + o_cs);
-  Meas* dmeas = reinterpret_cast<Meas*>(ws + o_meas);
-  auto run_all = [&]() -> int {
-    MHMR_CUDA_CHECK(cudaMemcpyAsync(ws, blob.data(), up_bytes, cudaMemcpyHostToDevice, st));
-    MHMR_CUDA_CHECK(cudaMemcpyAsync(dcs, cand_start.data(), 4ll * (B + 1), cudaMemcpyHostToDevice, st));
-    MHMR_CUDA_CHECK(cudaMemsetAsync(status, 0, 4ll * B, st));
+  std::memcpy(ws.host<PPhoto>(r_ph), ph.data(), sizeof(PPhoto) * B);
+  const PPhoto* dph = ws.dev<const PPhoto>(r_ph);
+  PState* dst = ws.dev<PState>(r_st);
+  int* dcs = ws.dev<int>(r_cs);
+  Meas* dmeas = ws.dev<Meas>(r_meas);
+  TRY(ws.upload());
+  MHMR_CUDA_CHECK(cudaMemsetAsync(status, 0, 4ll * B, st));
+  for (int b = 0; b < B; ++b) {
+    uint8_t* copy = ws.dev<uint8_t>(r_words[b]);
+    MHMR_CUDA_CHECK(cudaMemsetAsync(copy, 0, align256(ss[b].nbytes + kSlack), st));
+    if (ss[b].nbytes) MHMR_CUDA_CHECK(cudaMemcpyAsync(copy, ss[b].src, ss[b].nbytes, cudaMemcpyDeviceToDevice, st));
+  }
+  if (words > 0) {
+    search_kernel<<<static_cast<unsigned>((words * 32 + 255) / 256), 256, 0, st>>>(dph, B, words);
+    MHMR_CUDA_CHECK(cudaGetLastError());
+  }
+  compact_kernel<<<B, 1024, 0, st>>>(dph, dst);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  measure_kernel<<<static_cast<unsigned>((ncand + 127) / 128), 128, 0, st>>>(dph, dst, dcs, B,
+                                                                               static_cast<int>(ncand), dmeas);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  chain_kernel<<<B, 32, 0, st>>>(dph, dst, dcs, dmeas, status);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  emit_kernel<<<dim3(8, B), 64, 0, st>>>(dph, dst, status);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  resolve_kernel<<<B, 1024, 0, st>>>(dph, dst, status);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  unfilter_kernel<<<B, kUnfilterWarps * 32, 0, st>>>(dph, status);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  if (counts) {
     for (int b = 0; b < B; ++b) {
-      MHMR_CUDA_CHECK(cudaMemsetAsync(ws + o_words[b], 0, align256(ss[b].nbytes + kSlack), st));
-      if (ss[b].nbytes)
-        MHMR_CUDA_CHECK(cudaMemcpyAsync(ws + o_words[b], ss[b].src, ss[b].nbytes, cudaMemcpyDeviceToDevice, st));
+      // chain blocks, candidates, slow-path blocks, inflated bytes (low 32 bits)
+      const PState* s = dst + b;
+      MHMR_CUDA_CHECK(cudaMemcpyAsync(counts + 4 * b, &s->nchain, 4, cudaMemcpyDeviceToDevice, st));
+      MHMR_CUDA_CHECK(cudaMemcpyAsync(counts + 4 * b + 1, &s->ncand, 4, cudaMemcpyDeviceToDevice, st));
+      MHMR_CUDA_CHECK(cudaMemcpyAsync(counts + 4 * b + 2, &s->nslow, 4, cudaMemcpyDeviceToDevice, st));
+      MHMR_CUDA_CHECK(cudaMemcpyAsync(counts + 4 * b + 3, &s->total, 4, cudaMemcpyDeviceToDevice, st));
     }
-    if (words > 0) {
-      search_kernel<<<static_cast<unsigned>((words * 32 + 255) / 256), 256, 0, st>>>(dph, B, words);
-      MHMR_CUDA_CHECK(cudaGetLastError());
-    }
-    compact_kernel<<<B, 1024, 0, st>>>(dph, dst);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    measure_kernel<<<static_cast<unsigned>((ncand + 127) / 128), 128, 0, st>>>(dph, dst, dcs, B,
-                                                                                 static_cast<int>(ncand), dmeas);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    chain_kernel<<<B, 32, 0, st>>>(dph, dst, dcs, dmeas, status);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    emit_kernel<<<dim3(8, B), 64, 0, st>>>(dph, dst, status);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    resolve_kernel<<<B, 1024, 0, st>>>(dph, dst, status);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    unfilter_kernel<<<B, kUnfilterWarps * 32, 0, st>>>(dph, status);
-    MHMR_CUDA_CHECK(cudaGetLastError());
-    if (counts) {
-      for (int b = 0; b < B; ++b) {
-        // chain blocks, candidates, slow-path blocks, inflated bytes (low 32 bits)
-        const PState* s = dst + b;
-        MHMR_CUDA_CHECK(cudaMemcpyAsync(counts + 4 * b, &s->nchain, 4, cudaMemcpyDeviceToDevice, st));
-        MHMR_CUDA_CHECK(cudaMemcpyAsync(counts + 4 * b + 1, &s->ncand, 4, cudaMemcpyDeviceToDevice, st));
-        MHMR_CUDA_CHECK(cudaMemcpyAsync(counts + 4 * b + 2, &s->nslow, 4, cudaMemcpyDeviceToDevice, st));
-        MHMR_CUDA_CHECK(cudaMemcpyAsync(counts + 4 * b + 3, &s->total, 4, cudaMemcpyDeviceToDevice, st));
-      }
-    }
-    return MHMR_OK;
-  };
-  const int rc = run_all();
-  const cudaError_t fe = cudaFreeAsync(ws, st);
-  if (rc != MHMR_OK) return rc;
-  MHMR_CUDA_CHECK(fe);
-  return MHMR_OK;
+  }
+  return ws.release();
 }
 
 }  // namespace

@@ -337,26 +337,20 @@ int train_loss_smplx(const SmplxDeviceModel& bm, SmplxGradScratch& gs, const Tra
 
   // stream-ordered scratch: fp64 partials, then fp32 coefficients, upstream and intermediate gradients
   const size_t Pz = static_cast<size_t>(P);
-  const size_t nf = 16 + Pz * (kJ * 3 + 3ull * V + kJ * 2 + 2ull * V + 3 + 3 + 9 + kRot * 3 + kRot * 9 + nb + 10 + 2 + 1);
-  char* buf = nullptr;
-  MHMR_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&buf), chunks * 3 * sizeof(double) + nf * 4, st));
-  double* part = reinterpret_cast<double*>(buf);
-  float* f = reinterpret_cast<float*>(buf + chunks * 3 * sizeof(double));
-  auto take = [&f](size_t k) { float* r = f; f += k; return r; };
-  float* coef = take(16);
-  float* g_j3d = take(Pz * kJ * 3);
-  float* g_v3d = take(Pz * V * 3);
-  float* g_j2d = take(Pz * kJ * 2);
-  float* g_v2d = take(Pz * V * 2);
-  float* g_tp = take(Pz * 3);
-  float* g_tr = take(Pz * 3);
-  float* K_det = take(Pz * 9);
-  float* d_rotvec = take(Pz * kRot * 3);
-  float* dR = take(Pz * kRot * 9);
-  float* d_shape = take(Pz * nb);
-  float* d_expr = take(Pz * 10);
-  float* d_loc = take(Pz * 2);
-  float* d_dist = take(Pz);
+  CallScratch ws(st);
+  const size_t r_part = ws.region(chunks * 3 * sizeof(double));
+  auto f32 = [&ws](size_t n) { return ws.region(n * 4); };
+  const size_t r_coef = f32(16), r_j3d = f32(Pz * kJ * 3), r_v3d = f32(Pz * V * 3), r_j2d = f32(Pz * kJ * 2),
+               r_v2d = f32(Pz * V * 2), r_tp = f32(Pz * 3), r_tr = f32(Pz * 3), r_K = f32(Pz * 9),
+               r_rotvec = f32(Pz * kRot * 3), r_dR = f32(Pz * kRot * 9), r_shape = f32(Pz * nb), r_expr = f32(Pz * 10),
+               r_loc = f32(Pz * 2), r_dist = f32(Pz);
+  TRY(ws.allocate());
+  double* part = ws.dev<double>(r_part);
+  float *coef = ws.dev<float>(r_coef), *g_j3d = ws.dev<float>(r_j3d), *g_v3d = ws.dev<float>(r_v3d),
+        *g_j2d = ws.dev<float>(r_j2d), *g_v2d = ws.dev<float>(r_v2d), *g_tp = ws.dev<float>(r_tp),
+        *g_tr = ws.dev<float>(r_tr), *K_det = ws.dev<float>(r_K), *d_rotvec = ws.dev<float>(r_rotvec),
+        *dR = ws.dev<float>(r_dR), *d_shape = ws.dev<float>(r_shape), *d_expr = ws.dev<float>(r_expr),
+        *d_loc = ws.dev<float>(r_loc), *d_dist = ws.dev<float>(r_dist);
 
   loss_partials_kernel<<<chunks, kThreads, 0, st>>>(a, ch, part);
   MHMR_CUDA_CHECK(cudaGetLastError());
@@ -374,19 +368,14 @@ int train_loss_smplx(const SmplxDeviceModel& bm, SmplxGradScratch& gs, const Tra
     BodyGrads g;
     g.v3d = g_v3d; g.j3d = g_j3d; g.tp = g_tp;
     if (two_d) { g.v2d = g_v2d; g.j2d = g_j2d; }
-    const int rc = smplx_backward(bm, gs, P, yh.rotvec, yh.shape, yh.expression, yh.loc, yh.dist, K_det, g, g_tr,
-                                  d_rotvec, d_shape, d_expr, d_loc, d_dist, st, dR);
-    if (rc != MHMR_OK) {
-      cudaFreeAsync(buf, st);
-      return rc;
-    }
+    TRY(smplx_backward(bm, gs, P, yh.rotvec, yh.shape, yh.expression, yh.loc, yh.dist, K_det, g, g_tr, d_rotvec, d_shape,
+                       d_expr, d_loc, d_dist, st, dR));
     const float focal_norm = static_cast<float>(A.img_size / (2.0 * tan(30.0 * 3.14159265358979323846 / 180.0)));
     dec_grad_kernel<<<P, 128, 0, st>>>(a, coef, yh.dec, 318 + nb + 13, K_det, focal_norm, dR, d_shape, d_expr, d_loc,
                                        d_dist, A.d_dec, A.d_offset);
     MHMR_CUDA_CHECK(cudaGetLastError());
   }
-  MHMR_CUDA_CHECK(cudaFreeAsync(buf, st));
-  return MHMR_OK;
+  return ws.release();
 }
 
 }  // namespace mhmr
