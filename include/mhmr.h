@@ -93,6 +93,31 @@ int mhmr_op_normalize_u8(const void* img_u8, const float* lut, float* out, int B
  * the workspace is stream-ordered (cudaMallocAsync / cudaFreeAsync).  Nothing else waits for the device. */
 int mhmr_op_letterbox_u8(const int64_t* photos, int B, int S, int pad, uint8_t* out, int32_t* boxes, void* stream);
 
+/* Image.resize((w, h)) with Pillow's BICUBIC resampler for photos of any size, each to its own output size, byte for
+ * byte: the coefficient rows and passes of mhmr_op_letterbox_u8 without the pad.
+ *   photos  HOST int64 [B, 8]: device address, H, W, row pitch in bytes (>= 3 W) of each uint8 RGB HWC photo, then
+ *           device address, h, w, row pitch in bytes (>= 3 w) of its uint8 [h, w, 3] output
+ * Every argument is checked before any launch (sides in [1, 2^20]); B == 0 does nothing.  At most two kernel launches
+ * for the whole batch; the descriptors and tables go up in one cudaMemcpyAsync from pageable memory, the workspace is
+ * stream-ordered, nothing waits for the device. */
+int mhmr_op_resize_u8(const int64_t* photos, int B, void* stream);
+
+/* JPEG files encoded on the device, byte for byte as Pillow's `Image.fromarray(img).save(f, "JPEG", quality=q,
+ * subsampling=s)` writes uint8 RGB and L images: SOI, APP0 JFIF 1.01, DQT (jpeg_set_quality's tables), SOF0, the four
+ * Annex K Huffman tables (two for gray), SOS, the entropy-coded segment (islow fDCT, libjpeg's downsampling and edge
+ * replication, dummy blocks), EOI.
+ *   photos  HOST int64 [B, 9]: device address of the image, H, W, row pitch in bytes (>= channels x W), channels (3
+ *           RGB, 1 gray), quality (1-100), subsampling (0 4:4:4, 1 4:2:2, 2 4:2:0; for gray it sets only SOF0's
+ *           sampling byte, 0x11 / 0x21 / 0x22), device address of the output, its capacity in bytes
+ *   sizes   device int64 [B]: each file's size in bytes
+ *   status  device int32 [B]: 0, or 1 when the file is longer than its capacity; nothing of such a file is written
+ *           (its size is still the size it needs).  A capacity of 1024 + 415 x (the scan's blocks) bytes always
+ *           suffices: 1660 bits per block at most, every byte stuffed.
+ * Every argument is checked before any launch (sides in [1, 65535]); B == 0 does nothing.  Eight kernel launches and
+ * a memset for the whole batch; the descriptors, tables and headers go up in one cudaMemcpyAsync from pageable
+ * memory; the workspace is stream-ordered (about 340 bytes per block); nothing waits for the device. */
+int mhmr_op_jpeg_encode(const int64_t* photos, int B, int64_t* sizes, int32_t* status, void* stream);
+
 /* JPEG photos decoded on the device, byte for byte as Pillow's `Image.open(f).convert("RGB")` (libjpeg-turbo's
  * default path: islow IDCT, fancy upsampling, fixed-point YCbCr -> RGB).  The device takes baseline / extended
  * sequential Huffman files (SOF0, SOF1 at 8 bits) with 8-bit quantisation tables and one scan holding every component:

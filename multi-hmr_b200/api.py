@@ -3,7 +3,8 @@
 
     open_image, get_camera_parameters, load_model, forward_model
 
-plus `open_images`, the batched form of `open_image`.  JPEG and PNG decoding (of the files the device takes), the
+plus `open_images`, the batched form of `open_image`, and `create_jpeg`, the dataset conversion of
+datasets/bedlam.py:449-479.  JPEG and PNG decoding (of the files the device takes), the
 letterbox (resize + pad) and the forward are H100-native; other files are decoded on the host (PIL), as in the
 reference.
 """
@@ -134,6 +135,56 @@ def open_image(img_path, img_size, device=torch.device("cuda"), fused=False):
     img_pil = ImageOps.pad(img_pil, size=(img_size, img_size))
     x = torch.from_numpy(normalize_rgb(np.asarray(img_pil))).unsqueeze(0).to(device)
     return x, img_pil_full
+
+
+def create_jpeg(root_dir, target_size=512, device=torch.device("cuda"), batch=16):
+    """datasets/bedlam.py:449-479 on the device, writing the same files byte for byte: every `.png` under `root_dir`
+    whose name does not start with '.', in `os.walk` order, opened as RGB, resized (BICUBIC) so that its long side is
+    `target_size` (the other `int(side * target_size / long_side)`; the width counts as the long side only when it is
+    strictly longer) and saved as a default-quality JPEG next to it as `<name>_<target_size>.jpg`, or unresized as
+    `<name>.jpg` when `target_size` is None.  Files go through the device `batch` at a time: PNG decode
+    (`preprocess.decode_png`; Pillow for the files it does not take), resize, JPEG encode."""
+    import sys
+
+    from PIL import Image
+
+    from .preprocess import decode_png, encode_jpeg, resize
+
+    device = torch.device(device)
+    log_freq = 1000
+    print(f"ROOT_DIR: {root_dir}")
+    jobs = [os.path.join(dirpath, fn) for dirpath, _, filenames in os.walk(root_dir)
+            for fn in filenames if fn[-4:] == ".png" and fn[0] != "."]
+    tot = 0
+    for k in range(0, len(jobs), batch):
+        paths = jobs[k:k + batch]
+        blobs = []
+        for path in paths:
+            with open(path, "rb") as fh:
+                blobs.append(fh.read())
+        photos, ok = decode_png(blobs, device)
+        for i, path in enumerate(paths):
+            if not ok[i]:
+                photos[i] = _upload_pil(Image.open(path).convert("RGB"), device)
+        if target_size is not None:
+            sizes = []
+            for p in photos:
+                height, width = p.shape[:2]
+                if width > height:
+                    sizes.append((target_size, int(float(height) * float(target_size / float(width)))))
+                else:
+                    sizes.append((int(float(width) * float(target_size / float(height))), target_size))
+            photos = resize(photos, sizes)
+            names = [p[:-4] + f"_{target_size}.jpg" for p in paths]
+        else:
+            names = [p[:-4] + ".jpg" for p in paths]
+        for name, data in zip(names, encode_jpeg(photos)):
+            with open(name, "wb") as fh:
+                fh.write(data)
+            tot += 1
+            if tot % log_freq == 0:
+                print(f"Converted {tot} images so far")
+                sys.stdout.flush()
 
 
 def get_focalLength_from_fieldOfView(fov=60, img_size=512):

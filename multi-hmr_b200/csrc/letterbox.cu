@@ -39,6 +39,8 @@ struct LbImage {
   uint8_t* ws;         // [ws_rows, ws_cols, 3]
   int ws_rows, ws_cols;
   int x0, y0, nw, nh;  // the resized photo's box in the S x S output
+  uint8_t* out;        // resize only: the [nh, nw, 3] output, `out_pitch` bytes per row
+  int64_t out_pitch;
 };
 
 // One output byte: clip8((2^21 + sum_t src * k[t]) >> 22), summed in int32 as Pillow does.  The sum cannot overflow:
@@ -85,6 +87,17 @@ __global__ void __launch_bounds__(kThreads) letterbox_last_pass_kernel(const LbI
     if (in_x && y >= im.y0 && y < im.y0 + im.nh) v = resample_byte(im.last, tab, y - im.y0, x - im.x0, c);
     out[(static_cast<int64_t>(blockIdx.z) * S + y) * 3 * S + j] = v;
   }
+}
+
+// Image.resize's last pass: one output byte per thread, straight into each photo's own output rows.
+__global__ void __launch_bounds__(kThreads) resize_last_pass_kernel(const LbImage* __restrict__ imgs,
+                                                                    const int32_t* __restrict__ tab) {
+  const LbImage& im = imgs[blockIdx.z];
+  const int j = blockIdx.x * kThreads + threadIdx.x;
+  if (j >= 3 * im.nw) return;
+  const int x = j / 3, c = j - 3 * x;
+  for (int y = blockIdx.y; y < im.nh; y += gridDim.y)
+    im.out[static_cast<int64_t>(y) * im.out_pitch + j] = resample_byte(im.last, tab, y, x, c);
 }
 
 // ---- host: Pillow's arithmetic (plain double operations; the x86-64 host build emits no fused multiply-add) --------
@@ -151,6 +164,37 @@ struct Tables {
   const int32_t* row(int offset, int taps, int i) const { return data.data() + offset + static_cast<int64_t>(i) * (taps + 2); }
 };
 
+// Image.resize((nw, nh), BICUBIC) of one photo as passes over the shared coefficient rows: which axis goes first, the
+// workspace it needs, and the source of the last pass (see the top of this file).  False if a coefficient row could
+// overflow the int32 sum.
+bool plan(Tables& tab, const uint8_t* src, int64_t pitch, int64_t H, int64_t W, int nw, int nh, LbImage& im) {
+  int hoff, htaps, voff, vtaps;
+  if (!tab.get(static_cast<int>(W), nw, &hoff, &htaps) || !tab.get(static_cast<int>(H), nh, &voff, &vtaps)) return false;
+  const LbPass horiz{src, pitch, 0, 0, hoff, htaps}, vert{src, pitch, 0, 1, voff, vtaps};
+  if (H > 100 * W && nh < H) {  // vertical first: photo -> ws [nh, W], then horizontal ws -> out
+    im.first = vert;
+    im.ws_rows = nh;
+    im.ws_cols = static_cast<int>(W);
+    im.last = horiz;
+    im.last.pitch = 3 * W;
+  } else if (nw != W) {  // horizontal over the rows the vertical windows touch, then vertical ws -> out
+    const int y_first = tab.row(voff, vtaps, 0)[0];
+    const int32_t* lastrow = tab.row(voff, vtaps, nh - 1);
+    im.first = horiz;
+    im.first.row0 = y_first;
+    im.ws_rows = lastrow[0] + lastrow[1] - y_first;
+    im.ws_cols = nw;
+    im.last = vert;
+    im.last.row0 = y_first;
+    im.last.pitch = 3ll * nw;
+  } else {  // the width stays: one (vertical or identity) pass from the photo
+    im.ws_rows = 0;
+    im.ws_cols = 0;
+    im.last = vert;
+  }
+  return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -184,32 +228,8 @@ int mhmr_op_letterbox_u8(const int64_t* photos, int B, int S, int pad, uint8_t* 
     im.nh = nh;
     im.x0 = round_half_even((S - nw) * 0.5);  // ImageOps.pad, centering 0.5
     im.y0 = round_half_even((S - nh) * 0.5);
-    const uint8_t* src = reinterpret_cast<const uint8_t*>(d[0]);
-    int hoff, htaps, voff, vtaps;
-    const bool tables_ok = tab.get(static_cast<int>(W), nw, &hoff, &htaps) && tab.get(static_cast<int>(H), nh, &voff, &vtaps);
-    MHMR_REQUIRE(tables_ok, "letterbox: a coefficient row could overflow the int32 sum");
-    const LbPass horiz{src, pitch, 0, 0, hoff, htaps}, vert{src, pitch, 0, 1, voff, vtaps};
-    if (H > 100 * W && nh < H) {  // vertical first: photo -> ws [nh, W], then horizontal ws -> out
-      im.first = vert;
-      im.ws_rows = nh;
-      im.ws_cols = static_cast<int>(W);
-      im.last = horiz;
-      im.last.pitch = 3 * W;
-    } else if (nw != W) {  // horizontal over the rows the vertical windows touch, then vertical ws -> out
-      const int y_first = tab.row(voff, vtaps, 0)[0];
-      const int32_t* lastrow = tab.row(voff, vtaps, nh - 1);
-      im.first = horiz;
-      im.first.row0 = y_first;
-      im.ws_rows = lastrow[0] + lastrow[1] - y_first;
-      im.ws_cols = nw;
-      im.last = vert;
-      im.last.row0 = y_first;
-      im.last.pitch = 3ll * nw;
-    } else {  // the width stays: one (vertical or identity) pass from the photo
-      im.ws_rows = 0;
-      im.ws_cols = 0;
-      im.last = vert;
-    }
+    MHMR_REQUIRE(plan(tab, reinterpret_cast<const uint8_t*>(d[0]), pitch, H, W, nw, nh, im),
+                 "letterbox: a coefficient row could overflow the int32 sum");
     box[4 * b] = im.x0; box[4 * b + 1] = im.y0; box[4 * b + 2] = nw; box[4 * b + 3] = nh;
   }
   MHMR_REQUIRE(tab.data.size() < (1ull << 31), "letterbox: coefficient tables too large");
@@ -245,6 +265,65 @@ int mhmr_op_letterbox_u8(const int64_t* photos, int B, int S, int pad, uint8_t* 
   MHMR_CUDA_CHECK(cudaGetLastError());
   TRY(ws.release());
   if (boxes != nullptr) std::copy(box.begin(), box.end(), boxes);
+  return MHMR_OK;
+}
+
+int mhmr_op_resize_u8(const int64_t* photos, int B, void* stream) {
+  MHMR_REQUIRE(B >= 0 && B <= 65535, "resize: 0 <= B <= 65535 photos");
+  if (B == 0) return MHMR_OK;
+  MHMR_REQUIRE(photos != nullptr, "null argument");
+  std::vector<LbImage> imgs(B);
+  Tables tab;
+  int max_nw = 0, max_nh = 0;
+  for (int b = 0; b < B; ++b) {
+    const int64_t* d = photos + 8 * b;
+    const int64_t H = d[1], W = d[2], pitch = d[3], nh = d[5], nw = d[6], out_pitch = d[7];
+    MHMR_REQUIRE(d[0] != 0 && d[4] != 0, "resize: null photo or output");
+    MHMR_REQUIRE(H >= 1 && W >= 1 && H <= (1 << 20) && W <= (1 << 20), "resize: photo sides in [1, 2^20]");
+    MHMR_REQUIRE(nh >= 1 && nw >= 1 && nh <= (1 << 20) && nw <= (1 << 20), "resize: output sides in [1, 2^20]");
+    MHMR_REQUIRE(pitch >= 3 * W && out_pitch >= 3 * nw, "resize: row pitch below 3 W bytes");
+    LbImage& im = imgs[b];
+    im.nw = static_cast<int>(nw);
+    im.nh = static_cast<int>(nh);
+    im.out = reinterpret_cast<uint8_t*>(d[4]);
+    im.out_pitch = out_pitch;
+    MHMR_REQUIRE(plan(tab, reinterpret_cast<const uint8_t*>(d[0]), pitch, H, W, im.nw, im.nh, im),
+                 "resize: a coefficient row could overflow the int32 sum");
+    max_nw = std::max(max_nw, im.nw);
+    max_nh = std::max(max_nh, im.nh);
+  }
+  MHMR_REQUIRE(tab.data.size() < (1ull << 31), "resize: coefficient tables too large");
+
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CallScratch ws(st);
+  const size_t r_imgs = ws.region(sizeof(LbImage) * B, true), r_tab = ws.region(4 * tab.data.size(), true);
+  std::vector<size_t> r_ws(B);
+  for (int b = 0; b < B; ++b) r_ws[b] = ws.region(static_cast<size_t>(imgs[b].ws_rows) * 3 * imgs[b].ws_cols);
+  TRY(ws.allocate());
+  int max_cols = 0, max_rows = 0;
+  for (int b = 0; b < B; ++b) {
+    LbImage& im = imgs[b];
+    if (im.ws_rows > 0) {
+      im.ws = ws.dev<uint8_t>(r_ws[b]);
+      im.last.src = im.ws;
+      max_cols = std::max(max_cols, im.ws_cols);
+      max_rows = std::max(max_rows, im.ws_rows);
+    }
+  }
+  std::copy_n(imgs.data(), B, ws.host<LbImage>(r_imgs));
+  std::copy_n(tab.data.data(), tab.data.size(), ws.host<int32_t>(r_tab));
+  const LbImage* d_imgs = ws.dev<const LbImage>(r_imgs);
+  const int32_t* d_tab = ws.dev<const int32_t>(r_tab);
+  TRY(ws.upload());
+  if (max_rows > 0) {
+    const dim3 grid((3 * max_cols + kThreads - 1) / kThreads, std::min(max_rows, 65535), B);
+    letterbox_first_pass_kernel<<<grid, kThreads, 0, st>>>(d_imgs, d_tab);
+    MHMR_CUDA_CHECK(cudaGetLastError());
+  }
+  const dim3 grid((3 * max_nw + kThreads - 1) / kThreads, std::min(max_nh, 65535), B);
+  resize_last_pass_kernel<<<grid, kThreads, 0, st>>>(d_imgs, d_tab);
+  MHMR_CUDA_CHECK(cudaGetLastError());
+  TRY(ws.release());
   return MHMR_OK;
 }
 

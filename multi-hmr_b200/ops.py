@@ -81,6 +81,88 @@ def letterbox_u8(photos, S, pad=0):
     return out, boxes
 
 
+def resize_u8(photos, sizes):
+    """Photos (a list of uint8 [H, W, 3] CUDA tensors on one device, of any sizes; rows may be padded) and their
+    (w, h) output sizes -> uint8 [h, w, 3] tensors on that device: `Image.resize((w, h))` with Pillow's BICUBIC
+    resampler, byte for byte (`mhmr_op_resize_u8`)."""
+    _cuda(*photos)
+    assert len(photos) == len(sizes)
+    if not photos:
+        return []
+    dev = photos[0].device
+    desc = torch.empty(len(photos), 8, dtype=torch.int64)
+    keep, outs = [], []
+    for i, (p, (w, h)) in enumerate(zip(photos, sizes)):
+        assert p.dtype == torch.uint8 and p.dim() == 3 and p.shape[2] == 3 and p.device == dev, \
+            "uint8 [H, W, 3] photos on one device expected"
+        if not (p.stride(2) == 1 and p.stride(1) == 3 and (p.shape[0] == 1 or p.stride(0) >= 3 * p.shape[1])):
+            p = p.contiguous()
+        keep.append(p)
+        o = torch.empty(int(h), int(w), 3, dtype=torch.uint8, device=dev)
+        outs.append(o)
+        desc[i] = torch.tensor([p.data_ptr(), p.shape[0], p.shape[1], p.stride(0) if p.shape[0] > 1 else 3 * p.shape[1],
+                                o.data_ptr(), int(h), int(w), 3 * int(w)])
+    with torch.cuda.device(dev):
+        call("mhmr_op_resize_u8", desc, len(photos), stream())
+    return outs
+
+
+def jpeg_scan_blocks(h, w, channels, subsampling):
+    """Blocks of the scan `jpeg_encode` writes: ceil(W/8) x ceil(H/8) for gray, MCUs x blocks per MCU otherwise."""
+    if channels == 1:
+        return -(-w // 8) * -(-h // 8)
+    hs, vs = (1, 1) if subsampling == 0 else (2, 1) if subsampling == 1 else (2, 2)
+    return -(-w // (8 * hs)) * -(-h // (8 * vs)) * (hs * vs + 2)
+
+
+def jpeg_capacity(h, w, channels, subsampling):
+    """Bytes that always hold the file (`mhmr_op_jpeg_encode`'s bound): 1024 + 415 per block of the scan."""
+    return 1024 + 415 * jpeg_scan_blocks(h, w, channels, subsampling)
+
+
+def jpeg_encode(images, qualities, subsamplings):
+    """uint8 [H, W, 3] RGB or [H, W] gray CUDA tensors on one device (rows may be padded), with each one's quality
+    (1-100) and subsampling (0, 1, 2) -> the JPEG files' bytes Pillow's `save` writes (`mhmr_op_jpeg_encode`).  Every
+    output gets the worst-case capacity, so none overflows; the sizes and statuses come back in one host sync and
+    the files' bytes in one copy after it."""
+    _cuda(*images)
+    if not images:
+        return []
+    dev = images[0].device
+    desc = torch.empty(len(images), 9, dtype=torch.int64)
+    keep, offs, total = [], [], 0
+    for im, s in zip(images, subsamplings):
+        ch = 1 if im.dim() == 2 else im.shape[2]
+        offs.append((total, jpeg_capacity(im.shape[0], im.shape[1], ch, s)))
+        total += offs[-1][1]
+    out = torch.empty(total, dtype=torch.uint8, device=dev)
+    for i, (im, q, s, (off, cap)) in enumerate(zip(images, qualities, subsamplings, offs)):
+        assert im.dtype == torch.uint8 and im.device == dev and (im.dim() == 2 or (im.dim() == 3 and im.shape[2] == 3)), \
+            "uint8 [H, W, 3] or [H, W] images on one device expected"
+        ch = 1 if im.dim() == 2 else 3
+        if not (im.stride(-1) == 1 and (ch == 1 or im.stride(1) == 3) and (im.shape[0] == 1 or im.stride(0) >= ch * im.shape[1])):
+            im = im.contiguous()
+        keep.append(im)
+        desc[i] = torch.tensor([im.data_ptr(), im.shape[0], im.shape[1],
+                                im.stride(0) if im.shape[0] > 1 else ch * im.shape[1], ch, int(q), int(s),
+                                out.data_ptr() + off, cap])
+    B = len(images)
+    res = torch.empty(12 * B, dtype=torch.uint8, device=dev)   # int64 sizes, then int32 statuses: one read-back
+    with torch.cuda.device(dev):
+        call("mhmr_op_jpeg_encode", desc, B, res[:8 * B].view(torch.int64), res[8 * B:].view(torch.int32), stream())
+        host = res.cpu()
+    sizes, status = host[:8 * B].view(torch.int64).tolist(), host[8 * B:].view(torch.int32).tolist()
+    if any(status):
+        raise RuntimeError(f"jpeg_encode: a file overflowed its worst-case capacity (statuses {status})")
+    with torch.cuda.device(dev):
+        data = torch.cat([out[o:o + n] for (o, _), n in zip(offs, sizes)]).cpu().numpy().tobytes()
+    files, pos = [], 0
+    for n in sizes:
+        files.append(data[pos:pos + n])
+        pos += n
+    return files
+
+
 def jpeg_info(data):
     """(width, height, components, luma h, luma v, eligible) of a JPEG file's bytes (host only, `mhmr_jpeg_info`):
     eligible files are the ones `jpeg_decode` takes; the sizes are 0 for the others."""
